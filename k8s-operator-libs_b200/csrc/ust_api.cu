@@ -87,6 +87,9 @@ struct ust_handle {
   int64_t launches = 0;
   int num_sms = 0;
   size_t stream_smem = 0;   // dynamic shared memory of the streaming kernel (largest variant)
+  size_t l2_bytes = 0;      // L2 cache of the device
+  int stream_ctas_per_sm = 0;   // streaming CTAs an SM holds (occupancy API, fewest over the variants)
+  unsigned long long verify_ctas = 0;  // verification CTAs launched since the workspace was cleared (UstWorkspace::verify_done)
   bool ws_dirty = false;
   bool pdl = true;          // launch the kernels of a call with programmatic dependent launch (UST_PDL=0 turns it off: tuning)
   bool stamps = false;      // UST_STAMPS: per-CTA %globaltimer stamps (diagnostics)
@@ -173,6 +176,12 @@ struct ust_handle {
     if (e_ != cudaSuccess) return (h)->fail(UST_ERR_CUDA, "%s failed: %s", #call, cudaGetErrorString(e_)); \
   } while (0)
 
+// after a call that failed half-way: the workspace starts over (with it the count of finished verification CTAs)
+static cudaError_t clear_workspace(ust_handle* h, cudaStream_t st) {
+  h->verify_ctas = 0;
+  return cudaMemsetAsync(h->ws, 0, sizeof(UstWorkspace), st);
+}
+
 static bool policy_active(const ust_policy* p) { return p != nullptr && p->auto_upgrade != 0; }
 
 // tables depend on these fields only
@@ -206,16 +215,17 @@ static int ensure_tables(ust_handle* h, const ust_policy* p, cudaStream_t st) {
 }
 
 // Tiling of a shard: tiles of UST_TILE_NODES nodes; smaller tiles (halved, multiples of 128) when the snapshot is so small that
-// full-size tiles would leave SMs without work. One persistent CTA per SM, never more CTAs than tiles.
+// full-size tiles would leave CTAs without work. UST_STREAM_GRID_PER_SM persistent CTAs per SM, never more CTAs than tiles.
+static int max_grid(const ust_handle* h) { return h->num_sms * UST_STREAM_GRID_PER_SM; }
 static int pick_tile_nodes(const ust_handle* h, int64_t n) {
   int tn = UST_TILE_NODES;
-  // at least one tile per SM; a CTA keeps up to UST_STAGES tiles in flight at once, so a small snapshot is one load
+  // at least one tile per CTA; a CTA keeps up to UST_STAGES tiles in flight at once, so a small snapshot is one load
   // round trip whatever its tile size - and larger tiles mean larger (more efficient) bulk copies
-  while (tn > 128 && n / tn < (int64_t)h->num_sms) { tn = (tn / 2) & ~127; if (tn < 128) tn = 128; }  // multiples of 128 nodes
+  while (tn > 128 && n / tn < (int64_t)max_grid(h)) { tn = (tn / 2) & ~127; if (tn < 128) tn = 128; }  // multiples of 128 nodes
   return tn;
 }
 static int pick_grid(const ust_handle* h, int tiles) {
-  const int g = tiles < h->num_sms ? tiles : h->num_sms;
+  const int g = tiles < max_grid(h) ? tiles : max_grid(h);
   return g < 1 ? 1 : g;
 }
 // rounds of a launch's tile range that a CTA takes in stride order before it starts claiming tiles by ticket
@@ -287,6 +297,10 @@ static int fill_params(ust_handle* h, const ust_policy* policy, int64_t n, const
   P.static_rounds = pick_static_rounds(h, tiles, grid);
   P.publish = 1;
   P.stamps = (h->stamps && grid <= UST_MAX_CTAS) ? 1 : 0;
+  // L2 priority of the streamed inputs. Inputs larger than the L2 (C3: 130 MB against 50 MB on an H100) are read with
+  // normal priority: evict-first made a 10 M-node call 2.7 % slower (DESIGN.md §3.1). Inputs that fit keep evict-first,
+  // which measured faster there (1 M nodes).
+  P.evict_first_inputs = (size_t)n * 13u <= h->l2_bytes ? 1 : 0;
   for (auto& b : h->s_candtile) {
     // growing a buffer frees the old one: nothing of an earlier call may still be using it
     if ((size_t)tiles + 1 > b.cap && h->last_stream) cudaStreamSynchronize(h->last_stream);
@@ -307,6 +321,7 @@ static int launch_verify(ust_handle* h, UstParams& P, cudaStream_t st, bool pdl)
   int e = ust_launch_verify(P, h->num_sms, st, (pdl && !P.split) ? 1 : 0);
   if (e) return h->fail(UST_ERR_CUDA, "verification kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
   h->launches += 1;
+  h->verify_ctas += (unsigned long long)h->num_sms;
   return UST_OK;
 }
 
@@ -344,7 +359,7 @@ static int apply_device(ust_handle* h, const ust_policy* policy, int64_t n, cons
   if (h->last_stream && h->last_stream != st) UST_CUDA(h, cudaStreamSynchronize(h->last_stream));
   h->last_stream = st;
   if (h->ws_dirty) {
-    UST_CUDA(h, cudaMemsetAsync(h->ws, 0, sizeof(UstWorkspace), st));
+    UST_CUDA(h, clear_workspace(h,st));
     h->ws_dirty = false;
   }
   int rc = ensure_tables(h, policy, st);
@@ -362,6 +377,7 @@ static int apply_device(ust_handle* h, const ust_policy* policy, int64_t n, cons
     // then the ordinary streaming pass with that byte as a fifth input stream
     UST_CUDA(h, h->s_podsum.reserve((size_t)n + 16));
     P.podsum = h->s_podsum.p;
+    P.evict_first_inputs = 1;  // the pod-list pass was not measured faster with evict-normal inputs
     int e = ust_launch_pod_summary(n, P.active, P.hot, P.pod_off, P.pod_flags, n_pods, P.podlut, P.podsum, h->num_sms * 6, st);
     if (e) return h->fail(UST_ERR_CUDA, "pod-summary kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 1;
@@ -390,7 +406,12 @@ static int apply_device(ust_handle* h, const ust_policy* policy, int64_t n, cons
     for (int j = 0; j < 3; j++) relaxed = relaxed && !overlaps(in[i], h->prev_out[j]);     // read / write
   P.relaxed = relaxed ? 1 : 0;
   h->relaxed_calls += relaxed ? 1 : 0;
-  if (relaxed) P.static_rounds = P.n_tiles / grid + 3;  // no tickets: a CTA's tiles are fixed, the next call fills the tail
+  if (relaxed) {
+    P.static_rounds = P.n_tiles / grid + 3;  // no tickets: a CTA's tiles are fixed, the next call fills the tail
+    // the last verification kernel enqueued is the previous call's; every one before it must have finished before this
+    // call touches its parity's set (DESIGN.md §3.3)
+    P.verify_before = h->verify_ctas - (unsigned long long)h->num_sms;
+  }
   h->prev_n = -1;
   int e = ust_launch_stream(P, grid, st, h->pdl ? 1 : 0);
   if (e) return h->fail(UST_ERR_CUDA, "streaming kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
@@ -458,7 +479,7 @@ static int apply_pipelined(ust_handle* h, const ust_policy* policy, int64_t n, c
   if (h->last_stream && h->last_stream != up) UST_CUDA(h, cudaStreamSynchronize(h->last_stream));
   h->last_stream = up;
   if (h->ws_dirty) {
-    UST_CUDA(h, cudaMemsetAsync(h->ws, 0, sizeof(UstWorkspace), up));
+    UST_CUDA(h, clear_workspace(h,up));
     h->ws_dirty = false;
   }
   int rc = ensure_tables(h, policy, up);
@@ -611,7 +632,12 @@ int ust_create(ust_handle** out, int device) {
   if (const char* v = getenv("UST_STATIC_PCT")) { h->static_pct = atoi(v); if (h->static_pct < 0) h->static_pct = 0; if (h->static_pct > 100) h->static_pct = 100; }
   h->stamps = getenv("UST_STAMPS") != nullptr;
   if (const char* v = getenv("UST_OVERLAP")) h->overlap_calls = atoi(v) != 0;
-  int rc = ust_stream_config(device, &h->num_sms, &h->stream_smem);
+  {
+    int l2 = 0;
+    if ((e = cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, device)) != cudaSuccess) return bail("cudaDeviceGetAttribute", e);
+    h->l2_bytes = (size_t)l2;
+  }
+  int rc = ust_stream_config(device, &h->num_sms, &h->stream_smem, &h->stream_ctas_per_sm);
   if (rc != 0 || h->num_sms < 1) {
     g_create_error = std::string("no sm_90a kernel image usable on this device: ") + cudaGetErrorString((cudaError_t)rc);
     ust_destroy(h);
@@ -1034,7 +1060,7 @@ int ust_build_state(ust_handle* h, int64_t n_pods, const uint8_t* state, const i
     UST_CUDA(h, cudaMalloc(&h->ds_count_dev, h->ds_count_cap * sizeof(unsigned long long)));
     UST_CUDA(h, cudaMemsetAsync(h->ds_count_dev, 0, h->ds_count_cap * sizeof(unsigned long long), st));
   }
-  if (h->ws_dirty) { UST_CUDA(h, cudaMemsetAsync(h->ws, 0, sizeof(UstWorkspace), st)); h->ws_dirty = false; }
+  if (h->ws_dirty) { UST_CUDA(h, clear_workspace(h,st)); h->ws_dirty = false; }
   if (N) {
     UST_CUDA(h, cudaMemcpyAsync(h->s_hot.p, state, N, cudaMemcpyHostToDevice, st));
     UST_CUDA(h, cudaMemcpyAsync(h->s_ds.p, ds_idx, N * 4, cudaMemcpyHostToDevice, st));
@@ -1092,7 +1118,7 @@ int ust_build_state_uids(ust_handle* h, int64_t n_pods, const uint8_t* state, co
     UST_CUDA(h, cudaMalloc(&h->ds_count_dev, h->ds_count_cap * sizeof(unsigned long long)));
     UST_CUDA(h, cudaMemsetAsync(h->ds_count_dev, 0, h->ds_count_cap * sizeof(unsigned long long), st));
   }
-  if (h->ws_dirty) { UST_CUDA(h, cudaMemsetAsync(h->ws, 0, sizeof(UstWorkspace), st)); h->ws_dirty = false; }
+  if (h->ws_dirty) { UST_CUDA(h, clear_workspace(h,st)); h->ws_dirty = false; }
   if (N) {
     UST_CUDA(h, cudaMemcpyAsync(h->s_hot.p, state, N, cudaMemcpyHostToDevice, st));
     UST_CUDA(h, cudaMemcpyAsync(h->s_uid.p, owner_uid, N * 16, cudaMemcpyHostToDevice, st));
@@ -1150,10 +1176,38 @@ int ust_debug_stamps(ust_handle* h, unsigned long long* out, int n_ctas) {
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   UST_CUDA(h, cudaSetDevice(h->device));
   UST_CUDA(h, cudaDeviceSynchronize());
-  UST_CUDA(h, cudaMemcpy(out, h->ws->dbg, (size_t)n_ctas * 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  const unsigned last = (h->call_seq - 1u) & 1u;
+  UST_CUDA(h, cudaMemcpy(out, h->ws->dbg[last], (size_t)n_ctas * 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
   UST_CUDA(h, cudaMemcpy(out + (size_t)n_ctas * 4, h->ws->dbg2, 16 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));  // verification kernel
   return UST_OK;
 }
+
+// diagnostics: the streaming CTAs' stamps of the last two calls (UST_STAMPS). out[c][i][0..4] for c = 0 (the call before
+// the last one) and 1 (the last call), CTA i < n_ctas: entry, first tile landed, stream end, exit (%globaltimer ns), SM id
+int ust_debug_stamps_pair(ust_handle* h, unsigned long long* out, int n_ctas) {
+  if (!h || !out || n_ctas < 1 || n_ctas > UST_MAX_CTAS) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  h->prev_n = -1;
+  UST_CUDA(h, cudaSetDevice(h->device));
+  UST_CUDA(h, cudaDeviceSynchronize());
+  std::vector<unsigned long long> st((size_t)2 * UST_MAX_CTAS * 4);
+  std::vector<unsigned int> sm((size_t)2 * UST_MAX_CTAS);
+  UST_CUDA(h, cudaMemcpy(st.data(), h->ws->dbg, st.size() * sizeof(st[0]), cudaMemcpyDeviceToHost));
+  UST_CUDA(h, cudaMemcpy(sm.data(), h->ws->dbg_sm, sm.size() * sizeof(sm[0]), cudaMemcpyDeviceToHost));
+  const unsigned last = (h->call_seq - 1u) & 1u;
+  for (int c = 0; c < 2; c++) {
+    const unsigned par = c == 1 ? last : last ^ 1u;
+    for (int i = 0; i < n_ctas; i++) {
+      unsigned long long* o = out + ((size_t)c * n_ctas + i) * 5;
+      for (int k = 0; k < 4; k++) o[k] = st[((size_t)par * UST_MAX_CTAS + i) * 4 + k];
+      o[4] = sm[(size_t)par * UST_MAX_CTAS + i];
+    }
+  }
+  return UST_OK;
+}
+
+// diagnostics: streaming CTAs one SM holds (cudaOccupancyMaxActiveBlocksPerMultiprocessor, fewest over the kernel's variants)
+int ust_debug_stream_ctas_per_sm(ust_handle* h) { return h ? h->stream_ctas_per_sm : -1; }
 
 int ust_get_unique_id(void* out_bytes) {
   if (!out_bytes) return UST_ERR_INVALID_ARGUMENT;

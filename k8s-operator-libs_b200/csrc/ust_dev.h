@@ -26,6 +26,21 @@
 #define UST_CONSUMER_WARPS 12
 #endif
 #define UST_STREAM_THREADS (32 * (1 + UST_CONSUMER_WARPS))
+// Streaming CTAs that must fit on one SM together with one verification CTA (checked at compile time, ust_stream.cu).
+// 2 (a build variant, scripts/build_variants.py): the next call's CTA is resident and filling its ring while this
+// call's CTA still streams (DESIGN.md §3.1, §3.3)
+#ifndef UST_STREAM_CTAS_PER_SM
+#define UST_STREAM_CTAS_PER_SM 1
+#endif
+// CTAs a streaming launch has per SM (1: co-residency serves the next call; 2: one call fills both slots)
+#ifndef UST_STREAM_GRID_PER_SM
+#define UST_STREAM_GRID_PER_SM 1
+#endif
+#define UST_STREAM_MAXREG 64     /* __maxnreg__ of the streaming kernel */
+#ifndef UST_VERIFY_MAXREG
+#define UST_VERIFY_MAXREG 80     /* __maxnreg__ of the verification kernel */
+#endif
+#define UST_VERIFY_SMEM_MAX 6144 /* static shared memory of the verification kernel (asserted in ust_kernels.cu) */
 
 // Exchange vector (int64 lanes): what one shard contributes to / learns from the cluster-wide
 // constraint arithmetic (upgrade_inplace.go:49-62). Summed across shards; per-rank slots are one-hot,
@@ -70,7 +85,13 @@ struct UstWorkspace {
   // before that, which nobody is writing.
   unsigned long long hint_sig[2];
   int hint_cut[2];
-  unsigned long long dbg[UST_MAX_CTAS][4];  // %globaltimer stamps per streaming CTA: entry, first tile landed, stream end, exit
+  // verification CTAs that have exited, ever (since the workspace was last cleared): a relaxed streaming kernel waits
+  // until every verification kernel before the previous call's has finished before it touches its parity's set
+  unsigned long long verify_done;
+  // %globaltimer stamps per streaming CTA, by call parity: entry, first tile landed, stream end (all warps), exit;
+  // and the SM it ran on
+  unsigned long long dbg[2][UST_MAX_CTAS][4];
+  unsigned int dbg_sm[2][UST_MAX_CTAS];
   unsigned long long dbg2[16];              // verification kernel, CTA 0: woken, vector loaded, decided, done; 4..: inside the decision
 };
 
@@ -123,6 +144,8 @@ struct UstParams {
   int split;              // split mode: a host-launched collective reduces P.xchg between the two kernels
   int relaxed;            // the call does not depend on the previous call of the handle (see apply_device): its streaming kernel
                           // starts without waiting for that call's verification kernel and overlaps its tail
+  unsigned long long verify_before;  // relaxed: UstWorkspace::verify_done once every verification kernel before the previous call's has finished
+  int evict_first_inputs; // the input columns are read with L2 evict-first priority (the call's inputs fit in L2), else evict-normal
   int stamps;             // diagnostics: write %globaltimer stamps
   // fused multi-GPU exchange (world > 1): mailboxes of all ranks as mapped into this process, call number
   int fused_exchange;
@@ -133,7 +156,8 @@ struct UstParams {
 // kernel launchers; all return cudaError_t as int. `pdl` = launch with programmatic stream serialization.
 int ust_launch_stream(const UstParams& p, int grid, void* stream, int pdl);   // ust_stream.cu
 int ust_launch_verify(const UstParams& p, int grid, void* stream, int pdl);   // ust_kernels.cu
-int ust_stream_config(int device, int* num_sms, size_t* smem_bytes);          // also raises the dynamic shared-memory limit
+// also raises the dynamic shared-memory limit; `ctas_per_sm` = streaming CTAs an SM holds (occupancy API, fewest over the variants)
+int ust_stream_config(int device, int* num_sms, size_t* smem_bytes, int* ctas_per_sm);
 int ust_launch_pod_summary(long long n, int active, const uint8_t* hot, const int32_t* pod_off, const uint16_t* pod_flags,
                            long long n_pods, const uint8_t* podlut, uint8_t* podsum, int grid, void* stream);
 int ust_launch_build_state(long long n, const uint8_t* hot, const int32_t* ds_idx, int n_ds, const int32_t* ds_desired,

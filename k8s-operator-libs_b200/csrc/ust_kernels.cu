@@ -331,9 +331,23 @@ __device__ void redo_range(const UstParams& P, Shared& S, int ta, int tb) {
 // ------------------------------------------------------------------------------------------------
 // Registers: an SM sub-partition has 16384. The streaming kernel's CTA puts 4 of its 13 warps (64 registers a thread) on
 // one sub-partition = 8192; this kernel's 12 warps come 3 to a sub-partition, so they must stay within 8192 / 96 = 85
-// registers a thread to be resident BESIDE the streaming CTA. At 96 this kernel only got onto an SM when the streaming
-// CTA left it - and the next call's streaming kernel, whose launch waits for every CTA here to have started, with it.
-__global__ void __maxnreg__(80) ust_verify_kernel(const __grid_constant__ UstParams P) {
+// registers a thread to be resident BESIDE the streaming CTA (asserted in ust_stream.cu). At 96 this
+// kernel only got onto an SM when a streaming CTA left it - and the next call's streaming kernel, whose launch waits
+// for every CTA here to have started, with it.
+static_assert(sizeof(Shared) <= UST_VERIFY_SMEM_MAX, "the streaming kernel's residency arithmetic assumes this bound");
+
+// this CTA is through with its call's parity set of the workspace (UstParams::verify_before; only counted where two
+// streaming CTAs share an SM - with one, residency alone keeps calls k and k+2 apart, DESIGN.md §3.3)
+__device__ __forceinline__ void verify_cta_done(const UstParams& P) {
+  if (UST_STREAM_CTAS_PER_SM < 2) return;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence();
+    atomicAdd(&P.ws->verify_done, 1ull);
+  }
+}
+
+__global__ void __maxnreg__(UST_VERIFY_MAXREG) ust_verify_kernel(const __grid_constant__ UstParams P) {
   __shared__ Shared S;
   const int t = threadIdx.x;
   // prologue (overlaps the streaming kernel): the transition table (4.4 KiB) by one TMA bulk copy - it was uploaded by
@@ -396,7 +410,7 @@ __global__ void __maxnreg__(80) ust_verify_kernel(const __grid_constant__ UstPar
   if (P.stamps && lead && t == 0) P.ws->dbg2[2] = now_ns();
   const int redo = S.D.redo;
   mbar_wait(&S.mbar, 0);  // never leave with the bulk copy in flight (it landed long ago)
-  if (redo == 0) return;  // the speculation held: every output of the streaming kernel is final
+  if (redo == 0) { verify_cta_done(P); return; }  // the speculation held: every output of the streaming kernel is final
   if (t == 0) {
     S.redo = redo; S.cut = S.D.cut; S.lo = S.D.lo; S.hi = S.D.hi; S.slots = S.D.slots_left;
     S.abort_key = S.D.abort_key; S.node_offset = S.D.node_offset;
@@ -424,6 +438,7 @@ __global__ void __maxnreg__(80) ust_verify_kernel(const __grid_constant__ UstPar
     }
   }
   if (P.stamps && lead && t == 0) P.ws->dbg2[3] = now_ns();
+  verify_cta_done(P);
 }
 
 // Pod-list summaries (rows 12-14 of the scope table: pod_manager.go:256-391, :122-229, drain_manager.go:58-139).

@@ -11,7 +11,8 @@
 //     bucket, upgrade_inplace.go:71). The producer's elected lane claims tiles (a strided static part, then an atomic
 //     ticket so that every SM runs dry at the same moment) and moves each tile's four input columns - state (1 B),
 //     flags (4), pod_rev (4), ds_idx (4) per node - into one stage of a shared-memory ring with TMA bulk copies
-//     (cp.async.bulk, UBLKCP in SASS) that complete on the stage's "full" mbarrier. Bytes in flight are bounded by
+//     (cp.async.bulk, UBLKCP in SASS) that complete on the stage's "full" mbarrier (L2 evict-first only when the
+//     inputs fit in L2). Bytes in flight are bounded by
 //     the ring (UST_STAGES x 39 KiB per SM), not by registers;
 //   * the per-policy transition table (4.4 KiB, built by the host: ust_lut.h) arrives the same way, once per CTA;
 //   * consumer warps wait on "full", evaluate 128-node groups straight out of shared memory - one 16-byte lookup
@@ -42,7 +43,7 @@ static_assert(kGroups % kCW == 0 || kCW > kGroups, "consumer warps must divide t
 #ifndef UST_HOT_REP
 #define UST_HOT_REP 8
 #endif
-constexpr int kHotRep = UST_HOT_REP;              // replicas of the hot-byte table: 8 = one per 16-byte bank group
+constexpr int kHotRep = UST_HOT_REP;              // replicas of the hot-byte table: 8 = one per 16-byte bank group (16 KiB)
 static_assert(kHotRep == 1 || kHotRep == 8, "hot-byte table: plain or one replica per bank group");
 constexpr int kHotShift = kHotRep == 8 ? 7 : 4;   // byte offset of entry b (replica 0) = b << kHotShift
 constexpr uint32_t kHotMask = 0x7Fu << kHotShift;
@@ -75,6 +76,20 @@ struct __align__(128) SS {
   int last;
   long long V[UST_V_LEN];          // split mode: the vector the last CTA publishes
 };
+
+// Residency on an H100 SM (228 KiB shared memory, 1 KiB of it reserved per CTA; 65536 registers, 16384 per
+// sub-partition, a CTA's warp w on sub-partition w % 4): UST_STREAM_CTAS_PER_SM streaming CTAs and one verification CTA
+// at the same time. With two, the CTA of call k+1 is resident and filling its ring while call k's still streams, so the
+// SM's memory pipe does not drain between calls (DESIGN.md §3.1, §3.3). Losing this is a silent slow-down, hence here.
+constexpr int kSmemPerSM = 228 * 1024, kSmemReservedPerCTA = 1024, kRegsPerSM = 65536, kRegsPerSubPartition = 16384;
+constexpr int kStreamWarps = kThreads / 32, kVerifyWarps = UST_VERIFY_THREADS / 32;
+static_assert(UST_STREAM_CTAS_PER_SM * (sizeof(SS<true>) + kSmemReservedPerCTA) + UST_VERIFY_SMEM_MAX + kSmemReservedPerCTA <= kSmemPerSM,
+              "shared memory: the streaming CTAs (pod-list variant) and a verification CTA must fit on one SM");
+static_assert(UST_STREAM_CTAS_PER_SM * kStreamWarps * 32 * UST_STREAM_MAXREG + kVerifyWarps * 32 * UST_VERIFY_MAXREG <= kRegsPerSM,
+              "registers: the streaming CTAs and a verification CTA must fit on one SM");
+static_assert(UST_STREAM_CTAS_PER_SM * ((kStreamWarps + 3) / 4) * 32 * UST_STREAM_MAXREG +
+                      ((kVerifyWarps + 3) / 4) * 32 * UST_VERIFY_MAXREG <= kRegsPerSubPartition,
+              "registers: the streaming CTAs and a verification CTA must fit on one SM sub-partition");
 
 // Byte-sliced SIMD-in-register counting. The hot-byte table maps a hot byte to sixteen 4-bit one-hot increments packed
 // in 64 bits (fields 0-13: state code, 14: unavailable, 15: upgrade candidate) next to the node's table window; a
@@ -221,7 +236,8 @@ __device__ void produce(const UstParams& P, SS<PODS>& S) {
   const int tn = P.tile_nodes, G = (int)gridDim.x, R = P.static_rounds;
   const int t_end = P.tile_end;
   const int dyn_base = P.tile_begin + R * G;
-  const uint64_t pol = policy_evict_first();
+  // L2 priority of the input columns (UstParams::evict_first_inputs)
+  const uint64_t pol = P.evict_first_inputs ? policy_evict_first() : policy_evict_normal();
   unsigned int* ticket = &P.ws->ticket[P.parity][P.seg];
   int pA = 0x7FFFFFFF, pB = 0x7FFFFFFF;
   if (lane == 0) {
@@ -301,7 +317,7 @@ __device__ void consume(const UstParams& P, SS<PODS>& S, int cw) {
     mbar_wait(&S.full[s], ph);
     const int tile = *reinterpret_cast<volatile int*>(&S.tile_of[s]);
     if (tile < 0) break;
-    if (P.stamps && it == 0 && cw == 0 && lane == 0) P.ws->dbg[blockIdx.x][1] = now_ns();
+    if (P.stamps && it == 0 && cw == 0 && lane == 0) P.ws->dbg[P.parity][blockIdx.x][1] = now_ns();
     const Stage<PODS>& st = S.st[s];
     const long long base = (long long)tile * tn;
     const long long rem = P.n - base;
@@ -347,14 +363,19 @@ __device__ void consume(const UstParams& P, SS<PODS>& S, int cw) {
 }
 
 template <bool DS_SMEM, bool OUTCOME, bool PODS>
-__global__ void __maxnreg__(64) ust_stream_kernel(const __grid_constant__ UstParams P) {
+__global__ void __maxnreg__(UST_STREAM_MAXREG) ust_stream_kernel(const __grid_constant__ UstParams P) {
   extern __shared__ __align__(128) unsigned char ust_smem[];
   SS<PODS>& S = *reinterpret_cast<SS<PODS>*>(ust_smem);
   const int t = threadIdx.x, warp = t >> 5;
   UstWorkspace* ws = P.ws;
   // the next kernel of the stream (the verification kernel) may be made resident now: it waits for this grid itself
   griddep_launch_dependents();
-  if (P.stamps && t == 0) ws->dbg[blockIdx.x][0] = now_ns();
+  if (P.stamps && t == 0) {
+    ws->dbg[P.parity][blockIdx.x][0] = now_ns();
+    unsigned sm;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+    ws->dbg_sm[P.parity][blockIdx.x] = sm;
+  }
   if (warp == 0) {
     if (t == 0) {
       for (int s = 0; s < kStages; s++) { mbar_init(&S.full[s], 1); mbar_init(&S.empty[s], kCW); }
@@ -380,6 +401,14 @@ __global__ void __maxnreg__(64) ust_stream_kernel(const __grid_constant__ UstPar
     if (DS_SMEM)
       for (int i = ct; i <= P.n_ds; i += cn) S.dsrev[i] = i < P.n_ds ? __ldg(P.ds_rev + i) : 0;
     if (ct == 0) {
+      if (UST_STREAM_CTAS_PER_SM > 1 && P.relaxed) {
+        // This call shares its parity's set (hint slot, spec_used, cand_tile) with the call before the previous one,
+        // whose verification kernel may still read it: wait until that kernel - and every one before it - has left.
+        // Nothing is spent here in practice (the previous call's whole streaming pass ran in between), and nothing
+        // waited for can be starved: those CTAs were all resident before this grid could launch.
+        while ((unsigned long long)ld_acquire_gpu(reinterpret_cast<const long long*>(&ws->verify_done)) < P.verify_before)
+          __nanosleep(64);
+      }
       S.errinv = 0;
       S.spec_before = 0;
       // speculative cut: the previous call's, when it was made under the same signature; else the policy default
@@ -394,11 +423,11 @@ __global__ void __maxnreg__(64) ust_stream_kernel(const __grid_constant__ UstPar
     mbar_wait(&S.lutbar, 0);
     consume<DS_SMEM, OUTCOME, PODS>(P, S, warp - 1);
   }
-  if (P.stamps && t == 32) ws->dbg[blockIdx.x][2] = now_ns();
   // this CTA has run out of tiles: add its counts to the shard's (reductions, nobody waits for them) and leave.
   // The previous call's verification kernel must be through with the workspace first (it is, unless this call started
   // early: then this is where it waits).
   __syncthreads();
+  if (P.stamps && t == 0) ws->dbg[P.parity][blockIdx.x][2] = now_ns();
   griddep_wait();
   unsigned long long* acc = ws->acc[P.parity];
   if (blockIdx.x == 0 && P.seg == 0 && t >= 64 && t < 64 + 18 + 1 + UST_MAX_SEGMENTS) {
@@ -413,7 +442,7 @@ __global__ void __maxnreg__(64) ust_stream_kernel(const __grid_constant__ UstPar
   else if (t == 15) { if (S.cnt[15]) atomicAdd(&acc[UST_V_CANDIDATES], (unsigned long long)S.cnt[15]); }
   else if (t == 32) { if (S.errinv) atomicMax(&ws->errinv[P.parity], S.errinv); }
   else if (t == 33) { if (S.spec_before) atomicAdd(&acc[UST_STATE_EXCLUDED], (unsigned long long)S.spec_before); }  // lane 14 is free: "not in snapshot" is derived
-  if (P.stamps && t == 0) ws->dbg[blockIdx.x][3] = now_ns();
+  if (P.stamps && t == 0) ws->dbg[P.parity][blockIdx.x][3] = now_ns();
   if (!(P.split && P.publish)) return;
   // ---- split mode (a host-launched collective follows): the last CTA of the call's last streaming launch publishes
   // this shard's lanes of the exchange vector
@@ -460,14 +489,19 @@ cudaError_t launch_variant(const UstParams& p, int grid, cudaStream_t st, int pd
 }
 
 template <bool DS_SMEM, bool OUTCOME, bool PODS>
-cudaError_t config_variant() {
-  // the whole 228 KiB as shared memory: the verification kernel's CTA (5.6 KiB, ptxas sm_90a) must fit beside this kernel's, or it
-  // cannot become resident - and trigger the next call's launch - before this one has left the SM
+cudaError_t config_variant(int* ctas_per_sm) {
+  // the whole 228 KiB as shared memory: the streaming CTAs and the verification kernel's CTA (5.6 KiB, ptxas sm_90a) must
+  // fit together, or the next call's CTA cannot become resident before this one has left the SM
   cudaError_t e = cudaFuncSetAttribute(ust_stream_kernel<DS_SMEM, OUTCOME, PODS>, cudaFuncAttributePreferredSharedMemoryCarveout,
                                        (int)cudaSharedmemCarveoutMaxShared);
   if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(ust_stream_kernel<DS_SMEM, OUTCOME, PODS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                              (int)sizeof(SS<PODS>));
+  e = cudaFuncSetAttribute(ust_stream_kernel<DS_SMEM, OUTCOME, PODS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)sizeof(SS<PODS>));
+  if (e != cudaSuccess) return e;
+  int blocks = 0;
+  e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, ust_stream_kernel<DS_SMEM, OUTCOME, PODS>, kThreads, sizeof(SS<PODS>));
+  if (e == cudaSuccess && blocks < *ctas_per_sm) *ctas_per_sm = blocks;
+  return e;
 }
 
 }  // namespace
@@ -487,16 +521,18 @@ int ust_launch_stream(const UstParams& p, int grid, void* stream, int pdl) {
   }
 }
 
-int ust_stream_config(int device, int* num_sms, size_t* smem_bytes) {
+int ust_stream_config(int device, int* num_sms, size_t* smem_bytes, int* ctas_per_sm) {
   cudaError_t e;
-  if ((e = config_variant<true, true, true>()) != cudaSuccess) return (int)e;
-  if ((e = config_variant<true, true, false>()) != cudaSuccess) return (int)e;
-  if ((e = config_variant<true, false, true>()) != cudaSuccess) return (int)e;
-  if ((e = config_variant<true, false, false>()) != cudaSuccess) return (int)e;
-  if ((e = config_variant<false, true, true>()) != cudaSuccess) return (int)e;
-  if ((e = config_variant<false, true, false>()) != cudaSuccess) return (int)e;
-  if ((e = config_variant<false, false, true>()) != cudaSuccess) return (int)e;
-  if ((e = config_variant<false, false, false>()) != cudaSuccess) return (int)e;
+  int c = 1 << 30;
+  if ((e = config_variant<true, true, true>(&c)) != cudaSuccess) return (int)e;
+  if ((e = config_variant<true, true, false>(&c)) != cudaSuccess) return (int)e;
+  if ((e = config_variant<true, false, true>(&c)) != cudaSuccess) return (int)e;
+  if ((e = config_variant<true, false, false>(&c)) != cudaSuccess) return (int)e;
+  if ((e = config_variant<false, true, true>(&c)) != cudaSuccess) return (int)e;
+  if ((e = config_variant<false, true, false>(&c)) != cudaSuccess) return (int)e;
+  if ((e = config_variant<false, false, true>(&c)) != cudaSuccess) return (int)e;
+  if ((e = config_variant<false, false, false>(&c)) != cudaSuccess) return (int)e;
+  *ctas_per_sm = c;
   int sms = 0;
   if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device)) != cudaSuccess) return (int)e;
   *num_sms = sms;

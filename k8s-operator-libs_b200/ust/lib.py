@@ -142,6 +142,25 @@ class Handle:
         fn.argtypes = [C.c_void_p]
         return int(fn(self._h))
 
+    def stream_ctas_per_sm(self):
+        """diagnostics: streaming CTAs one SM holds (occupancy API at ust_create, fewest over the kernel's variants)"""
+        fn = self._lib.ust_debug_stream_ctas_per_sm
+        fn.restype = C.c_int
+        fn.argtypes = [C.c_void_p]
+        return int(fn(self._h))
+
+    def stamps_pair(self, n_ctas):
+        """diagnostics (UST_STAMPS set before the handle was created): the streaming CTAs' %globaltimer stamps of the last
+        two calls, uint64 array [2 (call before the last, last call), n_ctas, 5 (entry, first tile landed, stream end,
+        exit, SM id)]"""
+        fn = self._lib.ust_debug_stamps_pair
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
+        out = np.zeros((2, n_ctas, 5), dtype=np.uint64)
+        rc = fn(self._h, out.ctypes.data, n_ctas)
+        if rc:
+            raise UstError(rc, self.last_error())
+        return out
+
     def stream(self):
         """cudaStream_t of the handle's own stream (as an int)."""
         return int(self._lib.ust_stream(self._h))

@@ -11,14 +11,17 @@ CSRC = os.path.join(ROOT, "k8s-operator-libs_b200", "csrc")
 OUT = os.path.join(ROOT, "build_variants")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
          "-Xcompiler", "-fvisibility=hidden", "-Xcompiler", "-ffp-contract=off", "--fmad=false"]
+TWO_PER_SM = ["-DUST_STREAM_CTAS_PER_SM=2", "-DUST_HOT_REP=1"]   # two streaming CTAs (and a verification CTA) per SM
 VARIANTS = {
-    "t3072w12s4": ["-DUST_TILE_NODES=3072", "-DUST_STAGES=4", "-DUST_CONSUMER_WARPS=12"],
-    "t3072w12s3": ["-DUST_TILE_NODES=3072", "-DUST_STAGES=3", "-DUST_CONSUMER_WARPS=12"],
-    "t3072w8s4": ["-DUST_TILE_NODES=3072", "-DUST_STAGES=4", "-DUST_CONSUMER_WARPS=8"],
-    "t2048w8s4": ["-DUST_TILE_NODES=2048", "-DUST_STAGES=4", "-DUST_CONSUMER_WARPS=8"],
-    "t2048w8s6": ["-DUST_TILE_NODES=2048", "-DUST_STAGES=6", "-DUST_CONSUMER_WARPS=8"],
-    "t4096w16s3": ["-DUST_TILE_NODES=4096", "-DUST_STAGES=3", "-DUST_CONSUMER_WARPS=16"],
-    "rep1": ["-DUST_HOT_REP=1"],
+    "t3072w12s4": [],   # the default geometry: one streaming CTA per SM
+    "t3072w8s4": ["-DUST_CONSUMER_WARPS=8"],
+    # two streaming CTAs per SM: the next call's CTA fills its ring while the previous call's still streams
+    "t1536w6s4": ["-DUST_TILE_NODES=1536", "-DUST_STAGES=4", "-DUST_CONSUMER_WARPS=6"] + TWO_PER_SM,
+    "t3072w6s2": ["-DUST_TILE_NODES=3072", "-DUST_STAGES=2", "-DUST_CONSUMER_WARPS=6"] + TWO_PER_SM,
+    "t1792w7s3": ["-DUST_TILE_NODES=1792", "-DUST_STAGES=3", "-DUST_CONSUMER_WARPS=7"] + TWO_PER_SM,
+    "t1536w6s4g2": ["-DUST_TILE_NODES=1536", "-DUST_STAGES=4", "-DUST_CONSUMER_WARPS=6", "-DUST_STREAM_GRID_PER_SM=2"] + TWO_PER_SM,
+    "t1536w6s4v256r64": ["-DUST_TILE_NODES=1536", "-DUST_STAGES=4", "-DUST_CONSUMER_WARPS=6", "-DUST_VERIFY_THREADS=256",
+                         "-DUST_VERIFY_MAXREG=64"] + TWO_PER_SM,
 }
 
 
