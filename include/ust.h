@@ -291,6 +291,40 @@ int ust_apply_state_delta_sparse(ust_handle* h, const ust_policy* policy, int64_
                                  const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx,
                                  int32_t n_ds, const int32_t* ds_rev, int64_t max_out, int64_t* out_idx,
                                  uint8_t* out_next_state, uint16_t* out_actions, int64_t* n_out, ust_counters* out);
+/* Membership change of the resident snapshot: nodes that left the cluster and nodes that joined it, without a new upload.
+ * Removal and insertion positions refer to the resident snapshot of n nodes:
+ *   remove_idx[n_remove]      strictly increasing, each in [0, n)
+ *   insert_before[n_insert]   non-decreasing, each in [0, n]; state / flags / pod_rev / ds_idx hold the n_insert new nodes
+ * New node order: for each old position p = 0..n, first the inserted nodes with insert_before == p (in the order given),
+ * then old node p unless it is removed (p < n). The new snapshot has n - n_remove + n_insert nodes. */
+typedef struct ust_splice {
+  int64_t n_remove;
+  const int64_t* remove_idx;
+  int64_t n_insert;
+  const int64_t* insert_before;
+  const uint8_t* state;
+  const uint32_t* flags;
+  const int32_t* pod_rev;
+  const int32_t* ds_idx;
+} ust_splice;
+
+/* ust_apply_state_delta_sparse on a snapshot whose membership changed. The splice is applied on the device first (one
+ * pass over the resident columns and the previous call's outputs), then the n_changed overwrites exactly as in
+ * ust_apply_state_delta, with idx as distinct indices into the NEW snapshot, then the whole new snapshot is evaluated.
+ * Sparse outputs are in new-index order: every inserted node is reported, a surviving node when its (next_state,
+ * actions) differ from what the previous call returned for it, a removed node never. UST_ERR_TRUNCATED and
+ * ust_fetch_outputs (then with the new node count) work as in ust_apply_state_delta_sparse (a reference-level abort returns
+ * its own code, also when *n_out > max_out: then nothing is written to the out_* arrays); counters, aborts and error
+ * codes are those of ust_apply_state on the spliced arrays. splice == NULL or an empty splice: exactly
+ * ust_apply_state_delta_sparse. A violated contract (unsorted or duplicate remove_idx, insert_before out of range or
+ * decreasing, NULL insert arrays with n_insert > 0, idx outside the new snapshot, no resident snapshot or outputs, more
+ * than one rank set up by ust_comm_init) returns UST_ERR_INVALID_ARGUMENT before any device work: the resident snapshot
+ * stays as it was. The speculation hint of the slot cut is kept per snapshot size: the first call after a size change
+ * runs without one (same outputs, only slower). */
+int ust_apply_state_delta_splice(ust_handle* h, const ust_policy* policy, const ust_splice* splice, int64_t n_changed,
+                                 const int64_t* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
+                                 const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, int64_t max_out, int64_t* out_idx,
+                                 uint8_t* out_next_state, uint16_t* out_actions, int64_t* n_out, ust_counters* out);
 /* The full outputs of the last call on the resident snapshot (n_nodes entries each). */
 int ust_fetch_outputs(ust_handle* h, uint8_t* next_state, uint16_t* actions);
 

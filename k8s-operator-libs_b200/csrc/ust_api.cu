@@ -148,6 +148,16 @@ struct ust_handle {
   DevBuf<uint8_t> d_state;
   DevBuf<uint32_t> d_flags;
   DevBuf<int32_t> d_rev, d_ds;
+  // membership splice: the second buffer set the splice kernel writes (swapped with the resident columns and the previous
+  // outputs afterwards; allocated on the first splice), the removal / insertion lists and the inserted nodes
+  DevBuf<uint8_t> x_hot, x_next;
+  DevBuf<uint32_t> x_flags;
+  DevBuf<int32_t> x_rev, x_ds;
+  DevBuf<uint16_t> x_actions;
+  DevBuf<long long> i_rm, i_before;
+  DevBuf<uint8_t> i_state;
+  DevBuf<uint32_t> i_flags;
+  DevBuf<int32_t> i_rev, i_ds;
   DevBuf<int32_t> sim_entered, sim_wait, sim_valid;  // timed rollout simulation: per-node clocks
 
   // multi-GPU
@@ -674,6 +684,8 @@ void ust_destroy(ust_handle* h) {
   h->s_hot.release(); h->s_next.release(); h->s_outcome.release(); h->s_flags.release();
   h->s_rev.release(); h->s_ds.release(); h->s_dsrev.release(); h->s_podoff.release(); h->s_dsdesired.release();
   h->s_actions.release(); h->s_podflags.release(); h->s_podsum.release(); h->s_candtile[0].release(); h->s_candtile[1].release(); h->s_uid.release(); h->s_dsuid.release(); h->s_dsorder.release(); h->s_rev16.release(); h->s_ds8.release(); h->d_idx.release(); h->d_state.release(); h->d_flags.release(); h->d_rev.release(); h->d_ds.release(); h->sim_entered.release(); h->sim_wait.release(); h->sim_valid.release();
+  h->x_hot.release(); h->x_next.release(); h->x_flags.release(); h->x_rev.release(); h->x_ds.release(); h->x_actions.release();
+  h->i_rm.release(); h->i_before.release(); h->i_state.release(); h->i_flags.release(); h->i_rev.release(); h->i_ds.release();
   for (auto& ev : h->seg_done) if (ev) cudaEventDestroy(ev);
   for (auto& ev : h->seg_up) if (ev) cudaEventDestroy(ev);
   if (h->stream_h2d) cudaStreamDestroy(h->stream_h2d);
@@ -778,16 +790,32 @@ int ust_apply_state(ust_handle* h, const ust_policy* policy, int64_t n, const ui
   return keep(finish_with_counters(h, st, out));
 }
 
-// ust_apply_state_delta and ust_apply_state_delta_sparse: scatter the re-encoded nodes into the resident snapshot,
-// evaluate everything, return all outputs (dense) or the outputs that differ from the previous call's (sparse).
-static int delta_common(ust_handle* h, const ust_policy* policy, int64_t n_changed, const int64_t* idx, const uint8_t* state,
-                        const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev,
-                        bool sparse, uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome, int64_t max_out,
-                        int64_t* out_idx, int64_t* n_out, ust_counters* out) {
-  const int64_t n = h->resident_n;
-  if (n < 0) return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident snapshot: call ust_apply_state (without pod lists) first");
+// ust_apply_state_delta, _delta_sparse and _delta_splice: splice the resident snapshot (optional: nodes leave and join),
+// scatter the re-encoded nodes into it, evaluate everything, return all outputs (dense) or the outputs that differ from
+// the previous call's (sparse).
+static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splice* sp, int64_t n_changed, const int64_t* idx,
+                        const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds,
+                        const int32_t* ds_rev, bool sparse, uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome,
+                        int64_t max_out, int64_t* out_idx, int64_t* n_out, ust_counters* out) {
+  const int64_t n_old = h->resident_n;
+  if (n_old < 0) return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident snapshot: call ust_apply_state (without pod lists) first");
   if (sparse && !h->outputs_resident)
     return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident outputs to compare with: the previous call must be an ApplyState on this snapshot");
+  // the splice, checked in full before anything is touched
+  const int64_t n_rm = sp ? sp->n_remove : 0, n_ins = sp ? sp->n_insert : 0;
+  if (n_rm < 0 || n_ins < 0 || n_rm > n_old || (n_rm > 0 && !sp->remove_idx) ||
+      (n_ins > 0 && (!sp->insert_before || !sp->state || !sp->flags || !sp->pod_rev || !sp->ds_idx)))
+    return h->fail(UST_ERR_INVALID_ARGUMENT, "bad splice");
+  for (int64_t k = 0; k < n_rm; k++)
+    if (sp->remove_idx[k] < (k ? sp->remove_idx[k - 1] + 1 : 0) || sp->remove_idx[k] >= n_old)
+      return h->fail(UST_ERR_INVALID_ARGUMENT, "splice: remove_idx[%lld] = %lld is not strictly increasing in [0, %lld)", (long long)k,
+                     (long long)sp->remove_idx[k], (long long)n_old);
+  for (int64_t k = 0; k < n_ins; k++)
+    if (sp->insert_before[k] < (k ? sp->insert_before[k - 1] : 0) || sp->insert_before[k] > n_old)
+      return h->fail(UST_ERR_INVALID_ARGUMENT, "splice: insert_before[%lld] = %lld is not non-decreasing in [0, %lld]", (long long)k,
+                     (long long)sp->insert_before[k], (long long)n_old);
+  const int64_t n = n_old - n_rm + n_ins;
+  if (n >= (1LL << 40)) return h->fail(UST_ERR_INVALID_ARGUMENT, "too many nodes");
   if (n_changed < 0 || (n_changed > 0 && (!idx || !state || !flags || !pod_rev || !ds_idx)))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
   if (!sparse && n > 0 && (!next_state || !actions)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
@@ -800,6 +828,15 @@ static int delta_common(ust_handle* h, const ust_policy* policy, int64_t n_chang
   StreamDrain drain(h);
   cudaStream_t st = h->stream;
   const size_t N = (size_t)n, M = (size_t)n_changed;
+  if (n_rm || n_ins) {
+    // the previous outputs travel with the snapshot; the pair this call writes must hold the new size as well
+    const size_t R = (size_t)n_rm, I = (size_t)n_ins;
+    UST_CUDA(h, h->x_hot.reserve(N + 16)); UST_CUDA(h, h->x_flags.reserve(N + 4)); UST_CUDA(h, h->x_rev.reserve(N + 4));
+    UST_CUDA(h, h->x_ds.reserve(N + 4)); UST_CUDA(h, h->x_next.reserve(N + 16)); UST_CUDA(h, h->x_actions.reserve(N + 8));
+    UST_CUDA(h, h->s_next_prev.reserve(N + 16)); UST_CUDA(h, h->s_actions_prev.reserve(N + 8));
+    UST_CUDA(h, h->i_rm.reserve(R + 1)); UST_CUDA(h, h->i_before.reserve(I + 1)); UST_CUDA(h, h->i_state.reserve(I + 16));
+    UST_CUDA(h, h->i_flags.reserve(I + 4)); UST_CUDA(h, h->i_rev.reserve(I + 4)); UST_CUDA(h, h->i_ds.reserve(I + 4));
+  }
   UST_CUDA(h, h->s_dsrev.reserve((size_t)n_ds + 1));
   if (actuator_outcome) UST_CUDA(h, h->s_outcome.reserve(N + 16));
   UST_CUDA(h, h->d_idx.reserve(M + 1)); UST_CUDA(h, h->d_state.reserve(M + 16)); UST_CUDA(h, h->d_flags.reserve(M + 4));
@@ -815,6 +852,25 @@ static int delta_common(ust_handle* h, const ust_policy* policy, int64_t n_chang
   h->resident_n = -1;  // until the patched snapshot has been evaluated
   h->outputs_resident = false;
   if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsrev.p, ds_rev, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
+  if (n_rm || n_ins) {
+    const size_t R = (size_t)n_rm, I = (size_t)n_ins;
+    if (R) UST_CUDA(h, cudaMemcpyAsync(h->i_rm.p, sp->remove_idx, R * 8, cudaMemcpyHostToDevice, st));
+    if (I) {
+      UST_CUDA(h, cudaMemcpyAsync(h->i_before.p, sp->insert_before, I * 8, cudaMemcpyHostToDevice, st));
+      UST_CUDA(h, cudaMemcpyAsync(h->i_state.p, sp->state, I, cudaMemcpyHostToDevice, st));
+      UST_CUDA(h, cudaMemcpyAsync(h->i_flags.p, sp->flags, I * 4, cudaMemcpyHostToDevice, st));
+      UST_CUDA(h, cudaMemcpyAsync(h->i_rev.p, sp->pod_rev, I * 4, cudaMemcpyHostToDevice, st));
+      UST_CUDA(h, cudaMemcpyAsync(h->i_ds.p, sp->ds_idx, I * 4, cudaMemcpyHostToDevice, st));
+    }
+    int e = ust_launch_splice((long long)n_old, (long long)n_rm, h->i_rm.p, (long long)n_ins, h->i_before.p, h->i_state.p, h->i_flags.p,
+                              h->i_rev.p, h->i_ds.p, h->s_hot.p, h->s_flags.p, h->s_rev.p, h->s_ds.p, h->s_next.p, h->s_actions.p,
+                              h->x_hot.p, h->x_flags.p, h->x_rev.p, h->x_ds.p, h->x_next.p, h->x_actions.p, st);
+    if (e) return h->fail(UST_ERR_CUDA, "splice kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    h->launches += 1;
+    // the spliced set becomes the resident one (the previous outputs in s_next / s_actions, as after any call)
+    std::swap(h->s_hot, h->x_hot); std::swap(h->s_flags, h->x_flags); std::swap(h->s_rev, h->x_rev); std::swap(h->s_ds, h->x_ds);
+    std::swap(h->s_next, h->x_next); std::swap(h->s_actions, h->x_actions);
+  }
   if (M) {
     static_assert(sizeof(long long) == sizeof(int64_t), "index width");
     UST_CUDA(h, cudaMemcpyAsync(h->d_idx.p, idx, M * 8, cudaMemcpyHostToDevice, st));
@@ -869,7 +925,7 @@ int ust_apply_state_delta(ust_handle* h, const ust_policy* policy, int64_t n_cha
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  return delta_common(h, policy, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, false, next_state, actions,
+  return delta_common(h, policy, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, false, next_state, actions,
                       actuator_outcome, 0, nullptr, nullptr, out);
 }
 
@@ -880,7 +936,20 @@ int ust_apply_state_delta_sparse(ust_handle* h, const ust_policy* policy, int64_
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  return delta_common(h, policy, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
+  return delta_common(h, policy, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
+                      nullptr, max_out, out_idx, n_out, out);
+}
+
+int ust_apply_state_delta_splice(ust_handle* h, const ust_policy* policy, const ust_splice* splice, int64_t n_changed,
+                                 const int64_t* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
+                                 const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, int64_t max_out, int64_t* out_idx,
+                                 uint8_t* out_next_state, uint16_t* out_actions, int64_t* n_out, ust_counters* out) {
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
+  // node indices of a shard are global ranges (ust_comm_init): a splice would have to move them on every rank
+  if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_splice runs on one GPU");
+  return delta_common(h, policy, splice, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
                       nullptr, max_out, out_idx, n_out, out);
 }
 

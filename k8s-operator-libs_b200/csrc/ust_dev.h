@@ -175,6 +175,12 @@ int ust_launch_build_state_uids(long long n, const uint8_t* hot, const void* own
                                 unsigned long long* ds_count, UstWorkspace* ws, ust_counters* out, int grid, void* stream);
 int ust_launch_patch(long long m, const long long* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
                      const int32_t* ds_idx, uint8_t* hot_out, uint32_t* flags_out, int32_t* rev_out, int32_t* ds_out, void* stream);
+// membership splice (ust_apply_state_delta_splice): the resident columns and the previous outputs, rewritten in the new node
+// order into the o_* arrays (n - n_rm + n_ins entries); rm / ib sorted and checked by the caller
+int ust_launch_splice(long long n, long long n_rm, const long long* rm, long long n_ins, const long long* ib, const uint8_t* ins_hot,
+                      const uint32_t* ins_flags, const int32_t* ins_rev, const int32_t* ins_ds, const uint8_t* hot, const uint32_t* flags,
+                      const int32_t* rev, const int32_t* ds, const uint8_t* next, const uint16_t* act, uint8_t* o_hot, uint32_t* o_flags,
+                      int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, void* stream);
 // rollout simulation: the clock of the feedback between two reconciles (include/ust.h, ust_sim_options)
 struct UstSimParams {
   int timed;            // 0: whatever a node waits for has happened by the next reconcile

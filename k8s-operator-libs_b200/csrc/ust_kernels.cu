@@ -12,7 +12,8 @@
 // every tile with the reference's abort semantics (nodes the sequential passes had not reached stay untouched,
 // common_manager.go:462-523).
 // Around it: ust_pod_summary_kernel (pod lists -> one byte per node), ust_build_state*_kernel (BuildState),
-// ust_patch_kernel / ust_feedback_kernel (delta updates, rollout simulation), ust_widen_kernel (packed host format).
+// ust_patch_kernel / ust_splice_kernel / ust_feedback_kernel (delta updates, membership changes, rollout simulation),
+// ust_widen_kernel (packed host format).
 #include <climits>
 
 #include "ust_common.cuh"
@@ -766,6 +767,115 @@ __global__ void __launch_bounds__(kThreads) ust_patch_kernel(long long m, const 
   }
 }
 
+// Membership splice of the resident snapshot (ust_apply_state_delta_splice): one pass over the old columns and the previous
+// call's outputs that writes every surviving node at its new index in a second buffer set, and the inserted nodes beside
+// them (previous output next_state = 0xFF, which no state code equals, so the diff reports them). A CTA owns
+// kSpliceTile old positions [b0, b1) of 0..n (position n holds no node, only the inserts at the end). It finds the
+// parts of the two sorted lists that fall in its range once, by binary search, and turns them into per-position new
+// indices in shared memory:
+//   old node i          -> i - #removed < i + #inserts with insert_before <= i
+//   insert k at pos p   -> p - #removed < p + k
+// 16 B read + 16 B written per surviving node.
+constexpr int kSpliceTile = 2048;
+constexpr int kSplicePer = kSpliceTile / kThreads;  // contiguous positions per thread in the scan
+static_assert(kSplicePer * kThreads == kSpliceTile, "splice tile");
+
+__device__ __forceinline__ long long splice_lower_bound(const long long* __restrict__ a, long long len, long long v) {
+  long long lo = 0, hi = len;
+  while (lo < hi) {
+    const long long mid = (lo + hi) >> 1;
+    if (__ldg(a + mid) < v) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+__global__ void __launch_bounds__(kThreads) ust_splice_kernel(long long n, long long n_rm, const long long* __restrict__ rm,
+                                                              long long n_ins, const long long* __restrict__ ib,
+                                                              const uint8_t* __restrict__ ins_hot, const uint32_t* __restrict__ ins_flags,
+                                                              const int32_t* __restrict__ ins_rev, const int32_t* __restrict__ ins_ds,
+                                                              const uint8_t* __restrict__ hot, const uint32_t* __restrict__ flags,
+                                                              const int32_t* __restrict__ rev, const int32_t* __restrict__ ds,
+                                                              const uint8_t* __restrict__ next, const uint16_t* __restrict__ act,
+                                                              uint8_t* __restrict__ o_hot, uint32_t* __restrict__ o_flags,
+                                                              int32_t* __restrict__ o_rev, int32_t* __restrict__ o_ds,
+                                                              uint8_t* __restrict__ o_next, uint16_t* __restrict__ o_act) {
+  __shared__ long long s_dst[kSpliceTile];   // inserts at or before the position (range-relative), then old node's new index
+  __shared__ long long s_base[kSpliceTile];  // position - removed before it: insert k at the position goes to s_base + k
+  __shared__ uint8_t s_rm[kSpliceTile];
+  __shared__ long long s_bounds[4];
+  __shared__ long long s_wmax[kWarps];
+  __shared__ int s_wsum[kWarps];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const long long b0 = (long long)blockIdx.x * kSpliceTile;
+  const long long b1 = b0 + kSpliceTile < n + 1 ? b0 + kSpliceTile : n + 1;
+  const int len = (int)(b1 - b0);
+  if (t < 4) s_bounds[t] = t < 2 ? splice_lower_bound(rm, n_rm, t ? b1 : b0) : splice_lower_bound(ib, n_ins, t == 3 ? b1 : b0);
+  for (int j = t; j < kSpliceTile; j += kThreads) { s_dst[j] = 0; s_rm[j] = 0; }
+  __syncthreads();
+  const long long r0 = s_bounds[0], r1 = s_bounds[1], q0 = s_bounds[2], q1 = s_bounds[3];
+  for (long long k = r0 + t; k < r1; k += kThreads) s_rm[__ldg(rm + k) - b0] = 1;
+  for (long long k = q0 + t; k < q1; k += kThreads) {
+    const long long p = __ldg(ib + k);
+    if (k + 1 == q1 || __ldg(ib + k + 1) != p) s_dst[p - b0] = k + 1 - q0;  // last insert at p: inserts at or before p
+  }
+  __syncthreads();
+  // running max of the insert counts (they only grow with the position), exclusive running sum of the removals
+  long long vi[kSplicePer];
+  int vr[kSplicePer];
+  long long mx = 0;
+  int sm = 0;
+#pragma unroll
+  for (int e = 0; e < kSplicePer; e++) {
+    const int j = t * kSplicePer + e;
+    mx = s_dst[j] > mx ? s_dst[j] : mx;
+    vi[e] = mx;
+    vr[e] = sm;
+    sm += s_rm[j];
+  }
+  long long wmx = mx;
+  int wsm = sm;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const long long u = __shfl_up_sync(kFull, wmx, o);
+    const int v = __shfl_up_sync(kFull, wsm, o);
+    if (lane >= o) { wmx = u > wmx ? u : wmx; wsm += v; }
+  }
+  if (lane == 31) { s_wmax[warp] = wmx; s_wsum[warp] = wsm; }
+  long long pmx = __shfl_up_sync(kFull, wmx, 1);
+  int psm = __shfl_up_sync(kFull, wsm, 1);
+  if (lane == 0) { pmx = 0; psm = 0; }
+  __syncthreads();
+  for (int w = 0; w < warp; w++) { pmx = s_wmax[w] > pmx ? s_wmax[w] : pmx; psm += s_wsum[w]; }
+#pragma unroll
+  for (int e = 0; e < kSplicePer; e++) {
+    const int j = t * kSplicePer + e;
+    const long long base = b0 + j - (r0 + psm + vr[e]);
+    s_base[j] = base;
+    s_dst[j] = base + q0 + (vi[e] > pmx ? vi[e] : pmx);
+  }
+  __syncthreads();
+  const int old_len = b1 <= n ? len : len - 1;  // position n is no node
+#pragma unroll 4
+  for (int j = t; j < old_len; j += kThreads) {
+    const long long i = b0 + j;
+    const uint8_t h = __ldcs(hot + i);
+    const uint32_t f = __ldcs(flags + i);
+    const int32_t r = __ldcs(rev + i);
+    const int32_t d = __ldcs(ds + i);
+    const uint8_t x = __ldcs(next + i);
+    const uint16_t a = __ldcs(act + i);
+    if (s_rm[j]) continue;
+    const long long o = s_dst[j];
+    o_hot[o] = h; o_flags[o] = f; o_rev[o] = r; o_ds[o] = d; o_next[o] = x; o_act[o] = a;
+  }
+  for (long long k = q0 + t; k < q1; k += kThreads) {
+    const long long o = s_base[__ldg(ib + k) - b0] + k;
+    o_hot[o] = __ldg(ins_hot + k); o_flags[o] = __ldg(ins_flags + k); o_rev[o] = __ldg(ins_rev + k); o_ds[o] = __ldg(ins_ds + k);
+    o_next[o] = 0xFF;
+    o_act[o] = 0;
+  }
+}
+
 // Rollout simulation (SURVEY 8f.3): the state feedback between two reconciles. Untimed (sp.timed == 0): "ideal actuators" - every call
 // the reference makes through its providers takes effect, every asynchronous actuator succeeds, and whatever a node
 // is waiting for (jobs, pod readiness, validation) has happened by the next reconcile. One streaming pass, in place:
@@ -1038,6 +1148,15 @@ int ust_launch_patch(long long m, const long long* idx, const uint8_t* state, co
   const long long grid = (m + kThreads - 1) / kThreads;
   ust_patch_kernel<<<(unsigned)(grid > 65535 * 16 ? 65535 * 16 : grid), kThreads, 0, (cudaStream_t)stream>>>(
       m, idx, state, flags, pod_rev, ds_idx, hot_out, flags_out, rev_out, ds_out);
+  return (int)cudaGetLastError();
+}
+int ust_launch_splice(long long n, long long n_rm, const long long* rm, long long n_ins, const long long* ib, const uint8_t* ins_hot,
+                      const uint32_t* ins_flags, const int32_t* ins_rev, const int32_t* ins_ds, const uint8_t* hot, const uint32_t* flags,
+                      const int32_t* rev, const int32_t* ds, const uint8_t* next, const uint16_t* act, uint8_t* o_hot, uint32_t* o_flags,
+                      int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, void* stream) {
+  const long long grid = n / kSpliceTile + 1;  // positions 0..n
+  ust_splice_kernel<<<(unsigned)grid, kThreads, 0, (cudaStream_t)stream>>>(n, n_rm, rm, n_ins, ib, ins_hot, ins_flags, ins_rev, ins_ds, hot,
+                                                                           flags, rev, ds, next, act, o_hot, o_flags, o_rev, o_ds, o_next, o_act);
   return (int)cudaGetLastError();
 }
 int ust_launch_feedback(long long n, uint8_t* hot, uint32_t* flags, int32_t* pod_rev, const int32_t* ds_idx, int n_ds,

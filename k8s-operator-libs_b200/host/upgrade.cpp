@@ -633,18 +633,35 @@ int ClusterUpgradeStateManagerImpl::EvaluateCached(const ust_policy& policy, boo
     const size_t i = (size_t)changed[j];
     st[j] = k.state[i]; fl[j] = k.flags[i]; rv[j] = k.pod_rev[i]; di[j] = k.ds_idx[i];
   }
+  // nodes that joined: their columns from the cache, at the positions the splice gives them
+  const Cache::Splice& ps = k.pending;
+  const size_t ni = ps.insert_at.size();
+  std::vector<uint8_t> ist(ni + 1);
+  std::vector<uint32_t> ifl(ni + 1);
+  std::vector<int32_t> irv(ni + 1), idi(ni + 1);
+  for (size_t j = 0; j < ni; j++) {
+    const size_t i = (size_t)ps.insert_at[j];
+    ist[j] = k.state[i]; ifl[j] = k.flags[i]; irv[j] = k.pod_rev[i]; idi[j] = k.ds_idx[i];
+  }
+  const ust_splice splice = {(int64_t)ps.remove_idx.size(), ps.remove_idx.data(), (int64_t)ni, ps.insert_before.data(),
+                             ist.data(), ifl.data(), irv.data(), idi.data()};
   const int64_t cap = (int64_t)(n / 4 + 1024);
   std::vector<int64_t> oi((size_t)cap + 1);
   std::vector<uint8_t> on((size_t)cap + 1);
   std::vector<uint16_t> oa((size_t)cap + 1);
   int64_t n_out = 0;
-  int rc = ust_apply_state_delta_sparse(handle_, &policy, (int64_t)m, ix.data(), st.data(), fl.data(), rv.data(), di.data(),
-                                        (int32_t)k.ds_rev.size(), dsrev.data(), cap, oi.data(), on.data(), oa.data(), &n_out, c);
-  if (rc == UST_ERR_TRUNCATED) {
-    stats_.outputs_received += (int64_t)n;
-    return ust_fetch_outputs(handle_, k.next.data(), k.actions.data());
-  }
+  int rc = ust_apply_state_delta_splice(handle_, &policy, ps.empty() ? nullptr : &splice, (int64_t)m, ix.data(), st.data(), fl.data(),
+                                        rv.data(), di.data(), (int32_t)k.ds_rev.size(), dsrev.data(), cap, oi.data(), on.data(), oa.data(),
+                                        &n_out, c);
   if (rc == UST_ERR_CUDA || rc == UST_ERR_INVALID_ARGUMENT || rc == UST_ERR_COMM) return rc;
+  if (n_out > cap) {
+    // More changed outputs than the arrays hold: nothing was written to them. That is UST_ERR_TRUNCATED, or a
+    // reference-level abort, which keeps its own code. Either way the call's full outputs are resident: fetch them all.
+    stats_.outputs_received += (int64_t)n;
+    const int frc = ust_fetch_outputs(handle_, k.next.data(), k.actions.data());
+    if (frc != UST_OK) return frc;
+    return rc == UST_ERR_TRUNCATED ? UST_OK : rc;
+  }
   for (int64_t j = 0; j < n_out; j++) { k.next[(size_t)oi[(size_t)j]] = on[(size_t)j]; k.actions[(size_t)oi[(size_t)j]] = oa[(size_t)j]; }
   stats_.outputs_received += n_out;
   return rc;
@@ -677,9 +694,12 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
     };
     std::vector<int64_t> changed;
     // Slots follow BuildState's list order (NodeUpgradeState::ListIndex), of which every bucket's slice order is a
-    // subsequence: walk the entries in that order, check that the cached slots still increase along it, append the
-    // nodes the cache has not seen. Entries without a ListIndex take their position in the bucket walk instead.
+    // subsequence: walk the entries in that order and check that the cached slots still increase along it. A node the
+    // cache has not seen joins right after the last cached slot before it; a cached slot no entry names has left.
+    // Entries without a ListIndex take their position in the bucket walk instead.
     bool orderBroken = false;
+    std::vector<std::pair<int64_t, const NodeUpgradeState*>> joins;  // (insert before old slot, entry), in list order
+    std::vector<char> present(k.slots.size(), 0);
     {
       std::vector<std::pair<int64_t, const NodeUpgradeState*>> order;
       int64_t pos = 0;
@@ -698,26 +718,73 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
       if (haveIndex) std::stable_sort(order.begin(), order.end(), [](const auto& x, const auto& y) { return x.first < y.first; });
       long long lastSlot = -1;
       for (const auto& o : order) {
-        auto ins = k.slotOf.emplace(o.second->Node->Name, k.slots.size());
-        if (ins.second) {  // a node the cache has not seen: the snapshot grows
-          k.slots.emplace_back();
-          k.state.push_back(UST_STATE_EXCLUDED); k.flags.push_back(0); k.pod_rev.push_back(0); k.ds_idx.push_back(-1);
-          k.deferredMsg.emplace_back();
-          full = true;
-        }
-        const long long slot = (long long)ins.first->second;
+        auto it = k.idOf.find(o.second->Node->Name);
+        if (it == k.idOf.end()) { joins.emplace_back(lastSlot + 1, o.second); continue; }
+        const long long slot = (long long)k.slotOfId[it->second];
         if (slot < lastSlot) orderBroken = true;
+        present[(size_t)slot] = 1;
         lastSlot = slot;
       }
     }
     if (orderBroken && attempt == 0) { ResetIncremental(); continue; }  // re-encode in this snapshot's order
+    // The splice: the host arrays move to the new node order (linear), the same change is kept for the device
+    // (Cache::pending). Joined slots start empty and are encoded by the walk below.
+    Cache::Splice sp;
+    for (size_t i = 0; i < k.slots.size(); i++)
+      if (!present[i]) sp.remove_idx.push_back((int64_t)i);
+    std::vector<char> joined;
+    if (!sp.remove_idx.empty() || !joins.empty()) {
+      const size_t nOld = k.slots.size(), nNew = nOld - sp.remove_idx.size() + joins.size();
+      Cache nk;
+      nk.slots.reserve(nNew); nk.state.reserve(nNew); nk.flags.reserve(nNew); nk.pod_rev.reserve(nNew); nk.ds_idx.reserve(nNew);
+      nk.next.reserve(nNew); nk.actions.reserve(nNew); nk.deferredMsg.reserve(nNew);
+      joined.assign(nNew, 0);
+      size_t j = 0;
+      Error dup;
+      for (size_t p = 0; p <= nOld; p++) {
+        for (; j < joins.size() && joins[j].first == (int64_t)p; j++) {
+          const std::string& name = joins[j].second->Node->Name;
+          size_t id = k.slotOfId.size();
+          if (!k.freeIds.empty()) { id = k.freeIds.back(); k.freeIds.pop_back(); } else k.slotOfId.push_back(0);
+          if (!k.idOf.emplace(name, id).second) { dup = Errorf("node " + name + " appears twice in the snapshot"); k.freeIds.push_back(id); continue; }
+          sp.insert_before.push_back((int64_t)p);
+          sp.insert_at.push_back((int64_t)nk.slots.size());
+          joined[nk.slots.size()] = 1;
+          nk.slots.emplace_back();
+          nk.slots.back().name = name;
+          nk.slots.back().id = id;
+          nk.state.push_back(UST_STATE_EXCLUDED); nk.flags.push_back(0); nk.pod_rev.push_back(0); nk.ds_idx.push_back(-1);
+          nk.next.push_back(0); nk.actions.push_back(0); nk.deferredMsg.emplace_back();
+        }
+        if (p == nOld) break;
+        if (!present[p]) {  // the node left: its name and id go, its entries are not carried over
+          k.idOf.erase(k.slots[p].name);
+          k.freeIds.push_back(k.slots[p].id);
+          continue;
+        }
+        nk.slots.push_back(std::move(k.slots[p]));
+        nk.state.push_back(k.state[p]); nk.flags.push_back(k.flags[p]); nk.pod_rev.push_back(k.pod_rev[p]); nk.ds_idx.push_back(k.ds_idx[p]);
+        nk.next.push_back(p < k.next.size() ? k.next[p] : 0); nk.actions.push_back(p < k.actions.size() ? k.actions[p] : 0);
+        nk.deferredMsg.push_back(std::move(k.deferredMsg[p]));
+      }
+      if (dup) { ResetIncremental(); return dup; }
+      k.slots.swap(nk.slots); k.state.swap(nk.state); k.flags.swap(nk.flags); k.pod_rev.swap(nk.pod_rev); k.ds_idx.swap(nk.ds_idx);
+      k.next.swap(nk.next); k.actions.swap(nk.actions); k.deferredMsg.swap(nk.deferredMsg);
+      for (size_t i = 0; i < k.slots.size(); i++) k.slotOfId[k.slots[i].id] = i;
+    }
+    if (!full) {
+      stats_.inserted += (int64_t)sp.insert_at.size();
+      stats_.removed += (int64_t)sp.remove_idx.size();
+    }
+    k.pending = full ? Cache::Splice() : std::move(sp);
+    stats_.slots = (int64_t)k.slots.size();
     // this reconcile's view in pass order (what Replay walks): entry, its slot
     EncodedSnapshot view;
     view.policy = pol;
     std::vector<size_t> slotOfView;
     auto visit = [&](NodeUpgradeState* ns, int code) -> Error {
       const Node& n = *ns->Node;
-      const size_t i = k.slotOf.at(n.Name);
+      const size_t i = k.slotOfId[k.idOf.at(n.Name)];
       Cache::Slot& sl = k.slots[i];
       if (sl.seen) return Errorf("node " + n.Name + " appears twice in the snapshot");
       sl.seen = true;
@@ -735,7 +802,7 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
         stats_.encoded++;
         if (hot != k.state[i] || f != k.flags[i] || rev != k.pod_rev[i] || ds != k.ds_idx[i]) {
           k.state[i] = hot; k.flags[i] = f; k.pod_rev[i] = rev; k.ds_idx[i] = ds;
-          changed.push_back((int64_t)i);
+          if (joined.empty() || !joined[i]) changed.push_back((int64_t)i);  // a joined node travels with the splice
         }
         k.deferredMsg[i] = deferred;
         sl.sig = versioned ? sig : std::string();
@@ -773,13 +840,6 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
       if (attempt == 0) continue;
       return Errorf("incremental ApplyState: a bucket's slice order contradicts the list order");
     }
-    // nodes that left the snapshot keep their slot, as "not in snapshot"
-    for (size_t i = 0; i < k.slots.size(); i++)
-      if (!k.slots[i].seen && (k.state[i] & UST_HOT_STATE_MASK) != UST_STATE_EXCLUDED) {
-        k.state[i] = UST_STATE_EXCLUDED; k.flags[i] = 0; k.pod_rev[i] = 0; k.ds_idx[i] = -1;
-        k.slots[i].sig.clear(); k.slots[i].code = UST_STATE_EXCLUDED;
-        changed.push_back((int64_t)i);
-      }
     std::sort(changed.begin(), changed.end());
     if (full) stats_.full_uploads++;
     const int rc = EvaluateCached(pol, full, changed, &k, &last_);

@@ -284,20 +284,39 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
   // (upgrade_state.go:140-161, common_manager.go:229-604); the provider calls skipped for an unchanged object are
   // GetPodControllerRevisionHash and IsWaitingForSafeDriverLoad, both pure functions of the object in the reference's
   // own implementations (pod_manager.go:84-89, safe_driver_load_manager.go:51-53).
-  // Falls back to a full encode + upload when the snapshot grew, when a bucket's slice order no longer follows the
-  // cached order (slots are handed out in slice order, upgrade_inplace.go:71), or on the first call.
+  // Nodes that join the cluster are inserted at their list position among the cached slots and encoded on their own;
+  // nodes that leave are removed with their slot. Both travel to the device as one splice of the resident snapshot
+  // (ust_apply_state_delta_splice). Falls back to a full encode + upload on the first call and when the surviving nodes'
+  // list order no longer follows the cached order (slots are handed out in slice order, upgrade_inplace.go:71).
   Error ApplyStateIncremental(ClusterUpgradeState* currentState, const DriverUpgradePolicySpec* upgradePolicy);
-  struct IncrementalStats { int64_t reconciles = 0, full_uploads = 0, encoded = 0, reused = 0, outputs_received = 0; };
+  struct IncrementalStats {
+    int64_t reconciles = 0, full_uploads = 0, encoded = 0, reused = 0, outputs_received = 0;
+    int64_t inserted = 0, removed = 0;  // nodes that joined / left the cached snapshot by a splice
+    int64_t slots = 0;                  // size of the cached snapshot after the last reconcile
+  };
   const IncrementalStats& Stats() const { return stats_; }
   void ResetIncremental();
 
  protected:
   // The device half of ApplyStateIncremental: evaluate the cached snapshot. full: upload all of it and fetch all
-  // outputs; else upload the entries `changed` and patch the outputs that differ into cache_.next / cache_.actions.
+  // outputs; else apply cache->pending to the resident snapshot, upload the entries `changed` and patch the outputs that
+  // differ into cache_.next / cache_.actions (whose entries already follow the splice).
   // Returns the ABI's return code. (Virtual so that the host-logic test can put the oracle behind the same cache.)
   struct Cache {
-    struct Slot { std::string sig; int code = UST_STATE_EXCLUDED; bool seen = false; };
-    std::unordered_map<std::string, size_t> slotOf;  // node name -> SoA index
+    struct Slot { std::string name, sig; size_t id = 0; int code = UST_STATE_EXCLUDED; bool seen = false; };
+    // Node name -> stable id of its slot, id -> SoA index. A splice moves slots; the ids stay, so only slotOfId is
+    // rewritten (one linear pass), and only the names that joined or left touch the hash map.
+    std::unordered_map<std::string, size_t> idOf;
+    std::vector<size_t> slotOfId;
+    std::vector<size_t> freeIds;
+    // The membership change the host arrays went through since the device last saw them, in the terms of ust_splice
+    // (indices into the previous snapshot); insert_at[k] is the new index of inserted node k, whose columns are
+    // state[insert_at[k]] etc. Empty after a full upload.
+    struct Splice {
+      std::vector<int64_t> remove_idx, insert_before, insert_at;
+      bool empty() const { return remove_idx.empty() && insert_before.empty(); }
+    };
+    Splice pending;
     std::vector<Slot> slots;
     std::vector<uint8_t> state, next;
     std::vector<uint32_t> flags;

@@ -87,6 +87,12 @@ class Pods(C.Structure):
     _fields_ = [("pod_off", C.c_void_p), ("pod_flags", C.c_void_p), ("n_pods", C.c_int64)]
 
 
+class Splice(C.Structure):
+    """ust_splice: nodes removed from / inserted into the resident snapshot (raw host addresses)."""
+    _fields_ = [("n_remove", C.c_int64), ("remove_idx", C.c_void_p), ("n_insert", C.c_int64), ("insert_before", C.c_void_p),
+                ("state", C.c_void_p), ("flags", C.c_void_p), ("pod_rev", C.c_void_p), ("ds_idx", C.c_void_p)]
+
+
 def make_policy(auto_upgrade=True, max_parallel_upgrades=0, max_unavailable=None, pod_deletion_enabled=False,
                 validation_enabled=False, pod_deletion=None, drain=None, wait_for_completion=None,
                 use_maintenance_operator=False, evaluate_actuators=False):
