@@ -53,10 +53,18 @@ struct NcclApi {
 NcclApi g_nccl;
 std::mutex g_nccl_mu;
 
+// A growable device buffer that owns its memory. Move-only: std::swap hands the allocations over, a copy would free
+// them twice.
 template <class T>
 struct DevBuf {
   T* p = nullptr;
   size_t cap = 0;  // elements
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
   cudaError_t reserve(size_t n) {
     if (n <= cap) return cudaSuccess;
     size_t want = cap ? cap : 1024;
@@ -69,7 +77,46 @@ struct DevBuf {
     cap = want;
     return cudaSuccess;
   }
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+};
+
+// The four input columns of a set of nodes. The padding lets the kernels' 16-byte loads run past the last node.
+struct Columns {
+  DevBuf<uint8_t> hot;
+  DevBuf<uint32_t> flags;
+  DevBuf<int32_t> rev, ds;
+  cudaError_t reserve(size_t n) {
+    cudaError_t e = hot.reserve(n + 16);
+    if (e == cudaSuccess) e = flags.reserve(n + 4);
+    if (e == cudaSuccess) e = rev.reserve(n + 4);
+    if (e == cudaSuccess) e = ds.reserve(n + 4);
+    return e;
+  }
+  // nodes [first, first + count) of the host columns; null rev / ds are not copied (packed format: widened on the device)
+  cudaError_t upload(const uint8_t* state, const uint32_t* f, const int32_t* r, const int32_t* d, size_t first, size_t count,
+                     cudaStream_t st) {
+    if (!count) return cudaSuccess;
+    cudaError_t e = cudaMemcpyAsync(hot.p + first, state + first, count, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(flags.p + first, f + first, count * 4, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess && r) e = cudaMemcpyAsync(rev.p + first, r + first, count * 4, cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess && d) e = cudaMemcpyAsync(ds.p + first, d + first, count * 4, cudaMemcpyHostToDevice, st);
+    return e;
+  }
+};
+
+// Nodes given by index: the re-encoded nodes of a delta call, the inserted nodes of a splice.
+struct IndexedColumns {
+  DevBuf<long long> idx;
+  Columns cols;
+};
+
+// The outputs of one evaluation.
+struct Outputs {
+  DevBuf<uint8_t> next;
+  DevBuf<uint16_t> actions;
+  cudaError_t reserve(size_t n) {
+    cudaError_t e = next.reserve(n + 16);
+    return e == cudaSuccess ? actions.reserve(n + 8) : e;
+  }
 };
 
 }  // namespace
@@ -104,10 +151,11 @@ struct ust_handle {
   int64_t relaxed_calls = 0;   // diagnostics
   bool overlap_calls = true;  // UST_OVERLAP=0 turns the overlap of independent back-to-back calls off (tuning)
   cudaStream_t last_stream = nullptr;  // stream of the previous device-resident call (calls on another stream are ordered behind it)
+  // set by adopt_resident / drop_resident only
   int64_t resident_n = -1;  // nodes of the snapshot the last ust_apply_state left in the staging arrays (-1 = none)
   int32_t resident_n_ds = 0;  // ... and the size of its DaemonSet table
-  ust_counters* hist_dev = nullptr;  // rollout simulation: one ust_counters per simulated reconcile
-  size_t hist_cap = 0;
+  bool outputs_resident = false;  // `outs` holds the outputs of the last call on the resident snapshot
+  DevBuf<ust_counters> sim_hist;  // rollout simulation: one ust_counters per simulated reconcile
   int segments = 6;      // upload / compute / download pipeline depth of the host path (UST_SEGMENTS, tuning)
   bool no_hint = false;  // UST_NO_HINT=1 (tuning): every call speculates from the policy default, never from the previous call
 
@@ -121,43 +169,34 @@ struct ust_handle {
   ust_counters* counters_dev = nullptr;
   ust_counters* counters_host = nullptr;  // pinned
   long long* xchg_dev = nullptr;
-  unsigned long long* ds_count_dev = nullptr;
-  size_t ds_count_cap = 0;
+  DevBuf<unsigned long long> ds_count;  // BuildState: pods per DaemonSet (zero between calls)
 
-  // staging for the host-pointer API
-  DevBuf<uint8_t> s_hot, s_next, s_outcome;
-  DevBuf<uint32_t> s_flags;
-  DevBuf<int32_t> s_rev, s_ds, s_dsrev, s_podoff, s_dsdesired;
+  // staging for the host-pointer API; `staged` and `outs` hold the resident snapshot and its outputs
+  Columns staged;
+  Outputs outs;
+  DevBuf<uint8_t> s_outcome;
+  DevBuf<int32_t> s_dsrev, s_podoff, s_dsdesired;
   DevBuf<uint16_t> s_rev16;          // packed host format: interned pod revisions / DaemonSet indices as uploaded
   DevBuf<int8_t> s_ds8;
-  DevBuf<uint16_t> s_actions, s_podflags;
+  DevBuf<uint16_t> s_podflags;
   DevBuf<uint8_t> s_podsum;
   DevBuf<unsigned int> s_candtile[2];   // upgrade candidates per tile of the current call (by call parity: the previous
                                         // call's verification kernel may still be reading its own)
   // sparse delta outputs: the previous call's outputs, block counts, compacted entries
-  DevBuf<uint8_t> s_next_prev, sp_next;
-  DevBuf<uint16_t> s_actions_prev, sp_actions;
+  Outputs outs_prev, outs_sparse;
   DevBuf<unsigned int> sp_blocks;
   DevBuf<long long> sp_idx;
   long long* sp_count_dev = nullptr;
   long long* sp_count_host = nullptr;  // pinned
-  bool outputs_resident = false;       // s_next / s_actions hold the outputs of the last call on the resident snapshot
   DevBuf<uint64_t> s_uid, s_dsuid;   // BuildState owner join: pod owner UIDs, DaemonSet UID hash table (+ s_dsorder: slot -> index)
   DevBuf<int32_t> s_dsorder;
-  DevBuf<long long> d_idx;           // delta updates: indices and values of the changed nodes
-  DevBuf<uint8_t> d_state;
-  DevBuf<uint32_t> d_flags;
-  DevBuf<int32_t> d_rev, d_ds;
-  // membership splice: the second buffer set the splice kernel writes (swapped with the resident columns and the previous
-  // outputs afterwards; allocated on the first splice), the removal / insertion lists and the inserted nodes
-  DevBuf<uint8_t> x_hot, x_next;
-  DevBuf<uint32_t> x_flags;
-  DevBuf<int32_t> x_rev, x_ds;
-  DevBuf<uint16_t> x_actions;
-  DevBuf<long long> i_rm, i_before;
-  DevBuf<uint8_t> i_state;
-  DevBuf<uint32_t> i_flags;
-  DevBuf<int32_t> i_rev, i_ds;
+  IndexedColumns changed;            // delta updates: indices and values of the changed nodes
+  // membership splice: the second set the splice kernel writes (swapped with the resident columns and the previous
+  // outputs afterwards; allocated on the first splice), the removal list and the inserted nodes with their positions
+  Columns splice_cols;
+  Outputs splice_outs;
+  DevBuf<long long> removed;
+  IndexedColumns inserted;
   DevBuf<int32_t> sim_entered, sim_wait, sim_valid;  // timed rollout simulation: per-node clocks
 
   // multi-GPU
@@ -252,10 +291,22 @@ static int check_aligned(ust_handle* h, const void* p, const char* what) {
   return UST_OK;
 }
 
-static int fill_params(ust_handle* h, const ust_policy* policy, int64_t n, const uint8_t* state, const uint32_t* flags,
-                       const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev,
-                       const int32_t* pod_off, const uint16_t* pod_flags, uint8_t* next_state, uint16_t* actions,
-                       uint8_t* outcome, ust_counters* out_dev, UstParams* out, int* grid_out) {
+// The start of every evaluation enqueued on `st` (apply_device, apply_pipelined): orders it behind the previous call,
+// builds the tables and the launch parameters, and takes the call's exchange epoch and workspace parity.
+static int begin_call(ust_handle* h, const ust_policy* policy, int64_t n, const uint8_t* state, const uint32_t* flags,
+                      const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev,
+                      const int32_t* pod_off, const uint16_t* pod_flags, uint8_t* next_state, uint16_t* actions,
+                      uint8_t* outcome, ust_counters* out_dev, cudaStream_t st, UstParams* out, int* grid_out) {
+  // a handle's workspace, tables and counters serve one call at a time: a call on another stream than the previous
+  // one is ordered behind it (calls on the same stream are ordered by the stream)
+  if (h->last_stream && h->last_stream != st) UST_CUDA(h, cudaStreamSynchronize(h->last_stream));
+  h->last_stream = st;
+  if (h->ws_dirty) {
+    UST_CUDA(h, clear_workspace(h, st));
+    h->ws_dirty = false;
+  }
+  int rc = ensure_tables(h, policy, st);
+  if (rc) return rc;
   const bool active = policy_active(policy);
   UstParams P;
   memset(&P, 0, sizeof(P));
@@ -317,6 +368,11 @@ static int fill_params(ust_handle* h, const ust_policy* policy, int64_t n, const
     cudaError_t ce = b.reserve((size_t)tiles + 1);
     if (ce != cudaSuccess) return h->fail(UST_ERR_CUDA, "cudaMalloc failed: %s", cudaGetErrorString(ce));
   }
+  if (P.fused_exchange) P.epoch = ++h->epoch;  // collective call number: identical on every rank
+  P.parity = (int)(h->call_seq++ & 1u);
+  P.cand_tile = h->s_candtile[P.parity].p;
+  h->prev_n = -1;
+  h->ws_dirty = true;  // cleared again once every launch of this call has been enqueued successfully
   *out = P;
   *grid_out = grid;
   return UST_OK;
@@ -364,24 +420,13 @@ static int apply_device(ust_handle* h, const ust_policy* policy, int64_t n, cons
     if (ptrs[i]) { int rc = check_aligned(h, ptrs[i], names[i]); if (rc) return rc; }
   if (pod_off && pod_flags) { int rc = check_aligned(h, pod_flags, "pod_flags"); if (rc) return rc; }
   UST_CUDA(h, cudaSetDevice(h->device));
-  // a handle's workspace, tables and counters serve one call at a time: a call on another stream than the previous
-  // one is ordered behind it (calls on the same stream are ordered by the stream)
-  if (h->last_stream && h->last_stream != st) UST_CUDA(h, cudaStreamSynchronize(h->last_stream));
-  h->last_stream = st;
-  if (h->ws_dirty) {
-    UST_CUDA(h, clear_workspace(h,st));
-    h->ws_dirty = false;
-  }
-  int rc = ensure_tables(h, policy, st);
-  if (rc) return rc;
-
+  const bool prev_known = h->prev_n >= 0;  // the previous call's buffers (begin_call forgets them)
   UstParams P;
   int grid = 0;
-  rc = fill_params(h, policy, n, state, flags, pod_rev, ds_idx, n_ds, ds_rev, pod_off, pod_flags, next_state, actions, outcome,
-                   out_dev, &P, &grid);
+  int rc = begin_call(h, policy, n, state, flags, pod_rev, ds_idx, n_ds, ds_rev, pod_off, pod_flags, next_state, actions,
+                      outcome, out_dev, st, &P, &grid);
   if (rc) return rc;
 
-  h->ws_dirty = true;  // cleared again once every launch of this call has been enqueued successfully
   if (P.eval_pods) {
     // pod lists: one byte per node first (only the nodes whose actuator looks at its pods are read),
     // then the ordinary streaming pass with that byte as a fifth input stream
@@ -392,9 +437,6 @@ static int apply_device(ust_handle* h, const ust_policy* policy, int64_t n, cons
     if (e) return h->fail(UST_ERR_CUDA, "pod-summary kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 1;
   }
-  if (P.fused_exchange) P.epoch = ++h->epoch;  // collective call number: identical on every rank
-  P.parity = (int)(h->call_seq++ & 1u);
-  P.cand_tile = h->s_candtile[P.parity].p;
   // Independent back-to-back calls overlap: when the last thing enqueued on the handle's own stream is the previous
   // call's verification kernel and this call reads nothing that call writes and writes nothing that call reads or
   // writes, its streaming kernel does not wait for it (programmatic dependent launch without the initial wait: the
@@ -407,7 +449,7 @@ static int apply_device(ust_handle* h, const ust_policy* policy, int64_t n, cons
   auto overlaps = [](const ust_handle::Span& a, const ust_handle::Span& b) {
     return a.len && b.len && a.p < b.p + b.len && b.p < a.p + a.len;
   };
-  bool relaxed = chain && h->pdl && h->overlap_calls && st == h->stream && h->prev_n >= 0 && !P.eval_pods && !P.split;
+  bool relaxed = chain && h->pdl && h->overlap_calls && st == h->stream && prev_known && !P.eval_pods && !P.split;
   for (int i = 0; relaxed && i < 3; i++) {
     for (int j = 0; j < 3; j++) relaxed = relaxed && !overlaps(outs[i], h->prev_out[j]);   // write / write
     for (int j = 0; j < 4; j++) relaxed = relaxed && !overlaps(outs[i], h->prev_in[j]);    // write / read (that call's redo)
@@ -422,7 +464,6 @@ static int apply_device(ust_handle* h, const ust_policy* policy, int64_t n, cons
     // call touches its parity's set (DESIGN.md §3.3)
     P.verify_before = h->verify_ctas - (unsigned long long)h->num_sms;
   }
-  h->prev_n = -1;
   int e = ust_launch_stream(P, grid, st, h->pdl ? 1 : 0);
   if (e) return h->fail(UST_ERR_CUDA, "streaming kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
   h->launches += 1;
@@ -477,32 +518,63 @@ struct StreamDrain {
 
 #pragma GCC visibility push(default)
 
+// Host columns of ust_apply_state (wide), or of ust_apply_state_packed: uint16 pod revisions and int8 DaemonSet
+// indices, 3 instead of 8 bytes per node over PCIe, widened on the device (rev and ds are then null).
+struct HostNodes {
+  const uint8_t* state;
+  const uint32_t* flags;
+  const int32_t* rev;
+  const int32_t* ds;
+  const uint16_t* rev16;
+  const int8_t* ds8;
+};
+
+static int upload_nodes(ust_handle* h, const HostNodes& in, size_t first, size_t count, cudaStream_t st) {
+  UST_CUDA(h, h->staged.upload(in.state, in.flags, in.rev, in.ds, first, count, st));
+  if (in.rev16 && count) {
+    UST_CUDA(h, cudaMemcpyAsync(h->s_rev16.p + first, in.rev16 + first, count * 2, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, cudaMemcpyAsync(h->s_ds8.p + first, in.ds8 + first, count, cudaMemcpyHostToDevice, st));
+  }
+  return UST_OK;
+}
+
+static int widen_nodes(ust_handle* h, size_t first, size_t count, cudaStream_t st) {
+  int we = ust_launch_widen((long long)count, h->s_rev16.p + first, h->s_ds8.p + first, h->staged.rev.p + first,
+                            h->staged.ds.p + first, 4 * h->num_sms, st);
+  if (we) return h->fail(UST_ERR_CUDA, "widen kernel launch failed: %s", cudaGetErrorString((cudaError_t)we));
+  h->launches += 1;
+  return UST_OK;
+}
+
+static void drop_resident(ust_handle* h) {
+  h->resident_n = -1;
+  h->outputs_resident = false;
+}
+
+// The snapshot in `staged` stays resident after a call that produced counters (a reference-level abort and
+// UST_ERR_TRUNCATED included), with the call's outputs unless `outputs` is false. A call that failed keeps nothing.
+static int adopt_resident(ust_handle* h, int rc, int64_t n, int32_t n_ds, bool outputs = true) {
+  if (rc != UST_ERR_CUDA && rc != UST_ERR_INVALID_ARGUMENT && rc != UST_ERR_COMM && rc != UST_ERR_NIL_STATE) {
+    h->resident_n = n;
+    h->resident_n_ds = n_ds;
+    h->outputs_resident = outputs;
+  }
+  return rc;
+}
+
 // Pipelined host path: the snapshot is cut into segments of whole tiles; segment s+1 uploads while segment
 // s streams through the kernel and segment s-1's results download (PCIe is full duplex). The streaming pass
 // is speculative, so a segment's outputs are final unless the end-of-call verification had to redo tiles —
 // then (rare) the outputs are downloaded again.
-static int apply_pipelined(ust_handle* h, const ust_policy* policy, int64_t n, const uint8_t* state, const uint32_t* flags,
-                           const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, uint8_t* next_state,
-                           uint16_t* actions, uint8_t* outcome, ust_counters* out, const uint16_t* rev16 = nullptr,
-                           const int8_t* ds8 = nullptr) {
+static int apply_pipelined(ust_handle* h, const ust_policy* policy, int64_t n, const HostNodes& in, int32_t n_ds,
+                           uint8_t* next_state, uint16_t* actions, uint8_t* outcome, ust_counters* out) {
   cudaStream_t up = h->stream, down = h->stream_d2h, h2d = h->stream_h2d;  // up = compute stream of the call
-  if (h->last_stream && h->last_stream != up) UST_CUDA(h, cudaStreamSynchronize(h->last_stream));
-  h->last_stream = up;
-  if (h->ws_dirty) {
-    UST_CUDA(h, clear_workspace(h,up));
-    h->ws_dirty = false;
-  }
-  int rc = ensure_tables(h, policy, up);
-  if (rc) return rc;
   UstParams P;
   int grid = 0;
-  rc = fill_params(h, policy, n, h->s_hot.p, h->s_flags.p, h->s_rev.p, h->s_ds.p, n_ds, h->s_dsrev.p, nullptr, nullptr,
-                   h->s_next.p, h->s_actions.p, outcome ? h->s_outcome.p : nullptr, nullptr, &P, &grid);
+  int rc = begin_call(h, policy, n, h->staged.hot.p, h->staged.flags.p, h->staged.rev.p, h->staged.ds.p, n_ds, h->s_dsrev.p,
+                      nullptr, nullptr, h->outs.next.p, h->outs.actions.p, outcome ? h->s_outcome.p : nullptr, nullptr, up,
+                      &P, &grid);
   if (rc) return rc;
-  if (P.fused_exchange) P.epoch = ++h->epoch;
-  P.parity = (int)(h->call_seq++ & 1u);
-  P.cand_tile = h->s_candtile[P.parity].p;
-  h->prev_n = -1;
   const int tiles = P.n_tiles;
   // Segments: the uploads are the critical path (PCIe), every segment adds copy-engine turnarounds, and what follows
   // the last upload - its kernels and the download of its outputs - is exposed. So: few segments, and a last one of
@@ -510,10 +582,6 @@ static int apply_pipelined(ust_handle* h, const ust_policy* policy, int64_t n, c
   const int kSegments = h->segments;  // <= UST_MAX_SEGMENTS: one ticket counter and one event pair per streaming launch
   const int last_tiles = (kSegments > 1 && tiles >= 64) ? tiles / 16 : 0;
   const int per = last_tiles ? (tiles - last_tiles + kSegments - 2) / (kSegments - 1) : (tiles + kSegments - 1) / kSegments;
-  h->ws_dirty = true;
-  const bool dbg = getenv("UST_DEBUG_PIPE") != nullptr;
-  cudaEvent_t ev[4];
-  if (dbg) { for (auto& e : ev) cudaEventCreate(&e); cudaEventRecord(ev[0], up); }
   // uploads start once the compute stream has reached this call (tables, DaemonSet table, previous call's reads)
   UST_CUDA(h, cudaEventRecord(h->d2h_done, up));
   UST_CUDA(h, cudaStreamWaitEvent(h2d, h->d2h_done, 0));
@@ -522,23 +590,13 @@ static int apply_pipelined(ust_handle* h, const ust_policy* policy, int64_t n, c
     c1 = c0 + per < tiles - last_tiles ? c0 + per : (c0 < tiles - last_tiles ? tiles - last_tiles : tiles);
     const int64_t n0 = (int64_t)c0 * P.tile_nodes, n1 = c1 == tiles ? n : (int64_t)c1 * P.tile_nodes;
     const size_t len = (size_t)(n1 - n0);
-    if (len) {
-      UST_CUDA(h, cudaMemcpyAsync(h->s_hot.p + n0, state + n0, len, cudaMemcpyHostToDevice, h2d));
-      UST_CUDA(h, cudaMemcpyAsync(h->s_flags.p + n0, flags + n0, len * 4, cudaMemcpyHostToDevice, h2d));
-      if (rev16) {  // packed host format: 3 instead of 8 bytes per node over PCIe, widened on the device
-        UST_CUDA(h, cudaMemcpyAsync(h->s_rev16.p + n0, rev16 + n0, len * 2, cudaMemcpyHostToDevice, h2d));
-        UST_CUDA(h, cudaMemcpyAsync(h->s_ds8.p + n0, ds8 + n0, len, cudaMemcpyHostToDevice, h2d));
-      } else {
-        UST_CUDA(h, cudaMemcpyAsync(h->s_rev.p + n0, pod_rev + n0, len * 4, cudaMemcpyHostToDevice, h2d));
-        UST_CUDA(h, cudaMemcpyAsync(h->s_ds.p + n0, ds_idx + n0, len * 4, cudaMemcpyHostToDevice, h2d));
-      }
-    }
+    rc = upload_nodes(h, in, (size_t)n0, len, h2d);
+    if (rc) return rc;
     UST_CUDA(h, cudaEventRecord(h->seg_up[seg], h2d));
     UST_CUDA(h, cudaStreamWaitEvent(up, h->seg_up[seg], 0));
-    if (rev16 && len) {
-      int we = ust_launch_widen((long long)len, h->s_rev16.p + n0, h->s_ds8.p + n0, h->s_rev.p + n0, h->s_ds.p + n0, 4 * h->num_sms, up);
-      if (we) return h->fail(UST_ERR_CUDA, "widen kernel launch failed: %s", cudaGetErrorString((cudaError_t)we));
-      h->launches += 1;
+    if (in.rev16 && len) {
+      rc = widen_nodes(h, (size_t)n0, len, up);
+      if (rc) return rc;
     }
     UstParams Ps = P;
     Ps.tile_begin = c0;
@@ -554,35 +612,94 @@ static int apply_pipelined(ust_handle* h, const ust_policy* policy, int64_t n, c
     UST_CUDA(h, cudaEventRecord(h->seg_done[seg], up));
     UST_CUDA(h, cudaStreamWaitEvent(down, h->seg_done[seg], 0));
     if (len) {
-      UST_CUDA(h, cudaMemcpyAsync(next_state + n0, h->s_next.p + n0, len, cudaMemcpyDeviceToHost, down));
-      UST_CUDA(h, cudaMemcpyAsync(actions + n0, h->s_actions.p + n0, len * 2, cudaMemcpyDeviceToHost, down));
+      UST_CUDA(h, cudaMemcpyAsync(next_state + n0, h->outs.next.p + n0, len, cudaMemcpyDeviceToHost, down));
+      UST_CUDA(h, cudaMemcpyAsync(actions + n0, h->outs.actions.p + n0, len * 2, cudaMemcpyDeviceToHost, down));
       if (outcome) UST_CUDA(h, cudaMemcpyAsync(outcome + n0, h->s_outcome.p + n0, len, cudaMemcpyDeviceToHost, down));
     }
   }
-  if (dbg) { cudaEventRecord(ev[1], up); }
   rc = launch_verify(h, P, up, false);
   if (rc) return rc;
   h->ws_dirty = false;
   UST_CUDA(h, cudaMemcpyAsync(h->counters_host, h->counters_dev, sizeof(ust_counters), cudaMemcpyDeviceToHost, up));
-  if (dbg) { cudaEventRecord(ev[2], up); cudaEventRecord(ev[3], down); }
-  cudaError_t ce = cudaStreamSynchronize(up);
-  if (ce == cudaSuccess) ce = cudaStreamSynchronize(down);
-  if (dbg) {
-    float a, b, c;
-    cudaEventElapsedTime(&a, ev[0], ev[1]); cudaEventElapsedTime(&b, ev[0], ev[2]); cudaEventElapsedTime(&c, ev[0], ev[3]);
-    fprintf(stderr, "[ust pipe] uploads+stream kernels done %.3f ms, verify+counters %.3f ms, downloads done %.3f ms\n", a, b, c);
-    for (auto& e2 : ev) cudaEventDestroy(e2);
-  }
-  if (ce != cudaSuccess) {
-    h->ws_dirty = true;
-    return h->fail(UST_ERR_CUDA, "kernel execution failed: %s", cudaGetErrorString(ce));
-  }
-  if (h->counters_host->reserved[0] != 0) {  // the verification redid tiles: fetch the final outputs
-    UST_CUDA(h, cudaMemcpyAsync(next_state, h->s_next.p, (size_t)n, cudaMemcpyDeviceToHost, up));
-    UST_CUDA(h, cudaMemcpyAsync(actions, h->s_actions.p, (size_t)n * 2, cudaMemcpyDeviceToHost, up));
+  // the call ends when the segments' downloads have ended too
+  UST_CUDA(h, cudaEventRecord(h->d2h_done, down));
+  UST_CUDA(h, cudaStreamWaitEvent(up, h->d2h_done, 0));
+  rc = finish_with_counters(h, up, out, true);
+  if (rc != UST_ERR_CUDA && h->counters_host->reserved[0] != 0) {  // the verification redid tiles: fetch the final outputs
+    UST_CUDA(h, cudaMemcpyAsync(next_state, h->outs.next.p, (size_t)n, cudaMemcpyDeviceToHost, up));
+    UST_CUDA(h, cudaMemcpyAsync(actions, h->outs.actions.p, (size_t)n * 2, cudaMemcpyDeviceToHost, up));
     if (outcome) UST_CUDA(h, cudaMemcpyAsync(outcome, h->s_outcome.p, (size_t)n, cudaMemcpyDeviceToHost, up));
+    UST_CUDA(h, cudaStreamSynchronize(up));
   }
-  return finish_with_counters(h, up, out, h->counters_host->reserved[0] == 0);
+  return rc;
+}
+
+// ust_apply_state and ust_apply_state_packed after their argument checks: upload, evaluate, download. Snapshots of
+// 2^19 nodes or more take the pipelined path unless they come with pod lists; a call with pod lists is never resident.
+static int apply_host(ust_handle* h, const ust_policy* policy, int64_t n, const HostNodes& in, int32_t n_ds,
+                      const int32_t* ds_rev, const ust_pods* pods, uint8_t* next_state, uint16_t* actions,
+                      uint8_t* outcome, ust_counters* out) {
+  drop_resident(h);  // the staging arrays are overwritten from here on
+  UST_CUDA(h, cudaSetDevice(h->device));
+  StreamDrain drain(h);
+  cudaStream_t st = h->stream;
+  const size_t N = (size_t)n;
+  UST_CUDA(h, h->staged.reserve(N));
+  if (in.rev16) {
+    UST_CUDA(h, h->s_rev16.reserve(N + 8));
+    UST_CUDA(h, h->s_ds8.reserve(N + 16));
+  }
+  UST_CUDA(h, h->outs.reserve(N));
+  UST_CUDA(h, h->s_dsrev.reserve((size_t)n_ds + 1));
+  if (outcome) UST_CUDA(h, h->s_outcome.reserve(N + 16));
+  if (pods) {
+    UST_CUDA(h, h->s_podoff.reserve(N + 1));
+    UST_CUDA(h, h->s_podflags.reserve((size_t)pods->n_pods + 8));
+  }
+  if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsrev.p, ds_rev, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
+  if (!pods && n >= (1 << 19))
+    return adopt_resident(h, apply_pipelined(h, policy, n, in, n_ds, next_state, actions, outcome, out), n, n_ds);
+  int rc = upload_nodes(h, in, 0, N, st);
+  if (rc) return rc;
+  if (in.rev16 && N) {
+    rc = widen_nodes(h, 0, N, st);
+    if (rc) return rc;
+  }
+  if (pods) {
+    UST_CUDA(h, cudaMemcpyAsync(h->s_podoff.p, pods->pod_off, (N + 1) * 4, cudaMemcpyHostToDevice, st));
+    if (pods->n_pods) UST_CUDA(h, cudaMemcpyAsync(h->s_podflags.p, pods->pod_flags, (size_t)pods->n_pods * 2, cudaMemcpyHostToDevice, st));
+  }
+  rc = apply_device(h, policy, n, h->staged.hot.p, h->staged.flags.p, h->staged.rev.p, h->staged.ds.p, n_ds, h->s_dsrev.p,
+                    pods ? h->s_podoff.p : nullptr, pods ? h->s_podflags.p : nullptr, pods ? pods->n_pods : 0, h->outs.next.p,
+                    h->outs.actions.p, outcome ? h->s_outcome.p : nullptr, nullptr, st);
+  if (rc) return rc;
+  if (N) {
+    UST_CUDA(h, cudaMemcpyAsync(next_state, h->outs.next.p, N, cudaMemcpyDeviceToHost, st));
+    UST_CUDA(h, cudaMemcpyAsync(actions, h->outs.actions.p, N * 2, cudaMemcpyDeviceToHost, st));
+    if (outcome) UST_CUDA(h, cudaMemcpyAsync(outcome, h->s_outcome.p, N, cudaMemcpyDeviceToHost, st));
+  }
+  rc = finish_with_counters(h, st, out);
+  return pods ? rc : adopt_resident(h, rc, n, n_ds);
+}
+
+// The launch of ust_build_state / _uids once their inputs are enqueued: `launch(grid)` starts the counting kernel and
+// the finish kernel behind it.
+template <class Launch>
+static int build_state_launch(ust_handle* h, int64_t n_pods, int32_t n_ds, cudaStream_t st, Launch launch) {
+  if ((size_t)n_ds + 1 > h->ds_count.cap) {  // between calls only the finish kernel clears the counts
+    UST_CUDA(h, h->ds_count.reserve((size_t)n_ds + 1));
+    UST_CUDA(h, cudaMemsetAsync(h->ds_count.p, 0, h->ds_count.cap * sizeof(unsigned long long), st));
+  }
+  if (h->ws_dirty) { UST_CUDA(h, clear_workspace(h, st)); h->ws_dirty = false; }
+  int64_t grid = (n_pods + 1023) / 1024;  // 256 threads x 4 pods per iteration
+  if (grid < 1) grid = 1;
+  if (grid > 8 * h->num_sms) grid = 8 * h->num_sms;
+  h->ws_dirty = true;
+  int e = launch((int)grid);
+  if (e) return h->fail(UST_ERR_CUDA, "build-state kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+  h->ws_dirty = false;
+  h->launches += 2;
+  return UST_OK;
 }
 
 extern "C" {
@@ -671,7 +788,6 @@ void ust_destroy(ust_handle* h) {
   if (h->ws) cudaFree(h->ws);
   if (h->lut_dev) cudaFree(h->lut_dev);
   if (h->podlut_dev) cudaFree(h->podlut_dev);
-  if (h->hist_dev) cudaFree(h->hist_dev);
   if (h->lut_host) cudaFreeHost(h->lut_host);
   if (h->podlut_host) cudaFreeHost(h->podlut_host);
   if (h->counters_dev) cudaFree(h->counters_dev);
@@ -679,20 +795,13 @@ void ust_destroy(ust_handle* h) {
   if (h->xchg_dev) cudaFree(h->xchg_dev);
   if (h->sp_count_dev) cudaFree(h->sp_count_dev);
   if (h->sp_count_host) cudaFreeHost(h->sp_count_host);
-  h->s_next_prev.release(); h->sp_next.release(); h->s_actions_prev.release(); h->sp_actions.release(); h->sp_blocks.release(); h->sp_idx.release();
-  if (h->ds_count_dev) cudaFree(h->ds_count_dev);
-  h->s_hot.release(); h->s_next.release(); h->s_outcome.release(); h->s_flags.release();
-  h->s_rev.release(); h->s_ds.release(); h->s_dsrev.release(); h->s_podoff.release(); h->s_dsdesired.release();
-  h->s_actions.release(); h->s_podflags.release(); h->s_podsum.release(); h->s_candtile[0].release(); h->s_candtile[1].release(); h->s_uid.release(); h->s_dsuid.release(); h->s_dsorder.release(); h->s_rev16.release(); h->s_ds8.release(); h->d_idx.release(); h->d_state.release(); h->d_flags.release(); h->d_rev.release(); h->d_ds.release(); h->sim_entered.release(); h->sim_wait.release(); h->sim_valid.release();
-  h->x_hot.release(); h->x_next.release(); h->x_flags.release(); h->x_rev.release(); h->x_ds.release(); h->x_actions.release();
-  h->i_rm.release(); h->i_before.release(); h->i_state.release(); h->i_flags.release(); h->i_rev.release(); h->i_ds.release();
   for (auto& ev : h->seg_done) if (ev) cudaEventDestroy(ev);
   for (auto& ev : h->seg_up) if (ev) cudaEventDestroy(ev);
   if (h->stream_h2d) cudaStreamDestroy(h->stream_h2d);
   if (h->d2h_done) cudaEventDestroy(h->d2h_done);
   if (h->stream_d2h) cudaStreamDestroy(h->stream_d2h);
   if (h->stream) cudaStreamDestroy(h->stream);
-  delete h;
+  delete h;  // frees the DevBufs, on the device set above
 }
 
 void* ust_host_alloc(size_t bytes) {
@@ -743,51 +852,8 @@ int ust_apply_state(ust_handle* h, const ust_policy* policy, int64_t n, const ui
   if (pods && (!pods->pod_off || pods->n_pods < 0 || (pods->n_pods > 0 && !pods->pod_flags)))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad pod lists");
   if (pods) { int prc = check_pod_offsets_host(h, n, pods->pod_off, pods->n_pods); if (prc) return prc; }
-  UST_CUDA(h, cudaSetDevice(h->device));
-  StreamDrain drain(h);
-  cudaStream_t st = h->stream;
-  const size_t N = (size_t)n;
-  UST_CUDA(h, h->s_hot.reserve(N + 16));
-  UST_CUDA(h, h->s_flags.reserve(N + 4));
-  UST_CUDA(h, h->s_rev.reserve(N + 4));
-  UST_CUDA(h, h->s_ds.reserve(N + 4));
-  UST_CUDA(h, h->s_next.reserve(N + 16));
-  UST_CUDA(h, h->s_actions.reserve(N + 8));
-  UST_CUDA(h, h->s_dsrev.reserve((size_t)n_ds + 1));
-  if (actuator_outcome) UST_CUDA(h, h->s_outcome.reserve(N + 16));
-  if (pods) {
-    UST_CUDA(h, h->s_podoff.reserve(N + 1));
-    UST_CUDA(h, h->s_podflags.reserve((size_t)pods->n_pods + 8));
-  }
-  if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsrev.p, ds_rev, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
-  h->resident_n = -1;
-  h->outputs_resident = false;
-  auto keep = [&](int rc) {  // the uploaded snapshot stays usable unless the call itself failed (not the policy / the data)
-    if (rc != UST_ERR_CUDA && rc != UST_ERR_INVALID_ARGUMENT && rc != UST_ERR_COMM && rc != UST_ERR_NIL_STATE && !pods) { h->resident_n = n; h->resident_n_ds = n_ds; h->outputs_resident = true; }
-    return rc;
-  };
-  if (!pods && n >= (1 << 19))
-    return keep(apply_pipelined(h, policy, n, state, flags, pod_rev, ds_idx, n_ds, next_state, actions, actuator_outcome, out));
-  if (N) {
-    UST_CUDA(h, cudaMemcpyAsync(h->s_hot.p, state, N, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, cudaMemcpyAsync(h->s_flags.p, flags, N * 4, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, cudaMemcpyAsync(h->s_rev.p, pod_rev, N * 4, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, cudaMemcpyAsync(h->s_ds.p, ds_idx, N * 4, cudaMemcpyHostToDevice, st));
-  }
-  if (pods) {
-    UST_CUDA(h, cudaMemcpyAsync(h->s_podoff.p, pods->pod_off, (N + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (pods->n_pods) UST_CUDA(h, cudaMemcpyAsync(h->s_podflags.p, pods->pod_flags, (size_t)pods->n_pods * 2, cudaMemcpyHostToDevice, st));
-  }
-  int rc = apply_device(h, policy, n, h->s_hot.p, h->s_flags.p, h->s_rev.p, h->s_ds.p, n_ds, h->s_dsrev.p,
-                        pods ? h->s_podoff.p : nullptr, pods ? h->s_podflags.p : nullptr, pods ? pods->n_pods : 0, h->s_next.p,
-                        h->s_actions.p, actuator_outcome ? h->s_outcome.p : nullptr, nullptr, st);
-  if (rc) return rc;
-  if (N) {
-    UST_CUDA(h, cudaMemcpyAsync(next_state, h->s_next.p, N, cudaMemcpyDeviceToHost, st));
-    UST_CUDA(h, cudaMemcpyAsync(actions, h->s_actions.p, N * 2, cudaMemcpyDeviceToHost, st));
-    if (actuator_outcome) UST_CUDA(h, cudaMemcpyAsync(actuator_outcome, h->s_outcome.p, N, cudaMemcpyDeviceToHost, st));
-  }
-  return keep(finish_with_counters(h, st, out));
+  return apply_host(h, policy, n, HostNodes{state, flags, pod_rev, ds_idx, nullptr, nullptr}, n_ds, ds_rev, pods, next_state,
+                    actions, actuator_outcome, out);
 }
 
 // ust_apply_state_delta, _delta_sparse and _delta_splice: splice the resident snapshot (optional: nodes leave and join),
@@ -827,78 +893,65 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
   UST_CUDA(h, cudaSetDevice(h->device));
   StreamDrain drain(h);
   cudaStream_t st = h->stream;
-  const size_t N = (size_t)n, M = (size_t)n_changed;
-  if (n_rm || n_ins) {
-    // the previous outputs travel with the snapshot; the pair this call writes must hold the new size as well
-    const size_t R = (size_t)n_rm, I = (size_t)n_ins;
-    UST_CUDA(h, h->x_hot.reserve(N + 16)); UST_CUDA(h, h->x_flags.reserve(N + 4)); UST_CUDA(h, h->x_rev.reserve(N + 4));
-    UST_CUDA(h, h->x_ds.reserve(N + 4)); UST_CUDA(h, h->x_next.reserve(N + 16)); UST_CUDA(h, h->x_actions.reserve(N + 8));
-    UST_CUDA(h, h->s_next_prev.reserve(N + 16)); UST_CUDA(h, h->s_actions_prev.reserve(N + 8));
-    UST_CUDA(h, h->i_rm.reserve(R + 1)); UST_CUDA(h, h->i_before.reserve(I + 1)); UST_CUDA(h, h->i_state.reserve(I + 16));
-    UST_CUDA(h, h->i_flags.reserve(I + 4)); UST_CUDA(h, h->i_rev.reserve(I + 4)); UST_CUDA(h, h->i_ds.reserve(I + 4));
+  const size_t N = (size_t)n, M = (size_t)n_changed, R = (size_t)n_rm, I = (size_t)n_ins;
+  if (R || I) {  // the previous outputs travel with the snapshot
+    UST_CUDA(h, h->splice_cols.reserve(N));
+    UST_CUDA(h, h->splice_outs.reserve(N));
+    UST_CUDA(h, h->removed.reserve(R + 1));
+    UST_CUDA(h, h->inserted.idx.reserve(I + 1));
+    UST_CUDA(h, h->inserted.cols.reserve(I));
   }
   UST_CUDA(h, h->s_dsrev.reserve((size_t)n_ds + 1));
   if (actuator_outcome) UST_CUDA(h, h->s_outcome.reserve(N + 16));
-  UST_CUDA(h, h->d_idx.reserve(M + 1)); UST_CUDA(h, h->d_state.reserve(M + 16)); UST_CUDA(h, h->d_flags.reserve(M + 4));
-  UST_CUDA(h, h->d_rev.reserve(M + 4)); UST_CUDA(h, h->d_ds.reserve(M + 4));
-  if (sparse) {
-    UST_CUDA(h, h->s_next_prev.reserve(h->s_next.cap));
-    UST_CUDA(h, h->s_actions_prev.reserve(h->s_actions.cap));
+  UST_CUDA(h, h->changed.idx.reserve(M + 1));
+  UST_CUDA(h, h->changed.cols.reserve(M));
+  if (sparse) {  // the pair this call writes holds the new size as well
+    UST_CUDA(h, h->outs_prev.reserve(N));
     UST_CUDA(h, h->sp_blocks.reserve((size_t)ust_diff_blocks(n) + 1));
     UST_CUDA(h, h->sp_idx.reserve((size_t)max_out + 1));
-    UST_CUDA(h, h->sp_next.reserve((size_t)max_out + 16));
-    UST_CUDA(h, h->sp_actions.reserve((size_t)max_out + 8));
+    UST_CUDA(h, h->outs_sparse.reserve((size_t)max_out));
   }
-  h->resident_n = -1;  // until the patched snapshot has been evaluated
-  h->outputs_resident = false;
+  drop_resident(h);  // until the patched snapshot has been evaluated
   if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsrev.p, ds_rev, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
-  if (n_rm || n_ins) {
-    const size_t R = (size_t)n_rm, I = (size_t)n_ins;
-    if (R) UST_CUDA(h, cudaMemcpyAsync(h->i_rm.p, sp->remove_idx, R * 8, cudaMemcpyHostToDevice, st));
-    if (I) {
-      UST_CUDA(h, cudaMemcpyAsync(h->i_before.p, sp->insert_before, I * 8, cudaMemcpyHostToDevice, st));
-      UST_CUDA(h, cudaMemcpyAsync(h->i_state.p, sp->state, I, cudaMemcpyHostToDevice, st));
-      UST_CUDA(h, cudaMemcpyAsync(h->i_flags.p, sp->flags, I * 4, cudaMemcpyHostToDevice, st));
-      UST_CUDA(h, cudaMemcpyAsync(h->i_rev.p, sp->pod_rev, I * 4, cudaMemcpyHostToDevice, st));
-      UST_CUDA(h, cudaMemcpyAsync(h->i_ds.p, sp->ds_idx, I * 4, cudaMemcpyHostToDevice, st));
-    }
-    int e = ust_launch_splice((long long)n_old, (long long)n_rm, h->i_rm.p, (long long)n_ins, h->i_before.p, h->i_state.p, h->i_flags.p,
-                              h->i_rev.p, h->i_ds.p, h->s_hot.p, h->s_flags.p, h->s_rev.p, h->s_ds.p, h->s_next.p, h->s_actions.p,
-                              h->x_hot.p, h->x_flags.p, h->x_rev.p, h->x_ds.p, h->x_next.p, h->x_actions.p, st);
+  if (R || I) {
+    if (R) UST_CUDA(h, cudaMemcpyAsync(h->removed.p, sp->remove_idx, R * 8, cudaMemcpyHostToDevice, st));
+    if (I) UST_CUDA(h, cudaMemcpyAsync(h->inserted.idx.p, sp->insert_before, I * 8, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, h->inserted.cols.upload(sp->state, sp->flags, sp->pod_rev, sp->ds_idx, 0, I, st));
+    const Columns &in = h->inserted.cols, &s = h->staged, &x = h->splice_cols;
+    int e = ust_launch_splice((long long)n_old, (long long)n_rm, h->removed.p, (long long)n_ins, h->inserted.idx.p, in.hot.p, in.flags.p,
+                              in.rev.p, in.ds.p, s.hot.p, s.flags.p, s.rev.p, s.ds.p, h->outs.next.p, h->outs.actions.p,
+                              x.hot.p, x.flags.p, x.rev.p, x.ds.p, h->splice_outs.next.p, h->splice_outs.actions.p, st);
     if (e) return h->fail(UST_ERR_CUDA, "splice kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 1;
-    // the spliced set becomes the resident one (the previous outputs in s_next / s_actions, as after any call)
-    std::swap(h->s_hot, h->x_hot); std::swap(h->s_flags, h->x_flags); std::swap(h->s_rev, h->x_rev); std::swap(h->s_ds, h->x_ds);
-    std::swap(h->s_next, h->x_next); std::swap(h->s_actions, h->x_actions);
+    // the spliced set becomes the resident one (the previous outputs in `outs`, as after any call)
+    std::swap(h->staged, h->splice_cols);
+    std::swap(h->outs, h->splice_outs);
   }
   if (M) {
     static_assert(sizeof(long long) == sizeof(int64_t), "index width");
-    UST_CUDA(h, cudaMemcpyAsync(h->d_idx.p, idx, M * 8, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, cudaMemcpyAsync(h->d_state.p, state, M, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, cudaMemcpyAsync(h->d_flags.p, flags, M * 4, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, cudaMemcpyAsync(h->d_rev.p, pod_rev, M * 4, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, cudaMemcpyAsync(h->d_ds.p, ds_idx, M * 4, cudaMemcpyHostToDevice, st));
-    int e = ust_launch_patch((long long)n_changed, h->d_idx.p, h->d_state.p, h->d_flags.p, h->d_rev.p, h->d_ds.p, h->s_hot.p,
-                             h->s_flags.p, h->s_rev.p, h->s_ds.p, st);
+    UST_CUDA(h, cudaMemcpyAsync(h->changed.idx.p, idx, M * 8, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, h->changed.cols.upload(state, flags, pod_rev, ds_idx, 0, M, st));
+    const Columns &d = h->changed.cols, &s = h->staged;
+    int e = ust_launch_patch((long long)n_changed, h->changed.idx.p, d.hot.p, d.flags.p, d.rev.p, d.ds.p, s.hot.p, s.flags.p,
+                             s.rev.p, s.ds.p, st);
     if (e) return h->fail(UST_ERR_CUDA, "patch kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 1;
   }
-  if (sparse) {  // the previous call's outputs step aside; this call writes the other pair of arrays
-    std::swap(h->s_next, h->s_next_prev);
-    std::swap(h->s_actions, h->s_actions_prev);
-  }
-  int rc = apply_device(h, policy, n, h->s_hot.p, h->s_flags.p, h->s_rev.p, h->s_ds.p, n_ds, h->s_dsrev.p, nullptr, nullptr, 0,
-                        h->s_next.p, h->s_actions.p, actuator_outcome ? h->s_outcome.p : nullptr, nullptr, st);
+  if (sparse) std::swap(h->outs, h->outs_prev);  // the previous call's outputs step aside; this call writes the other pair
+  int rc = apply_device(h, policy, n, h->staged.hot.p, h->staged.flags.p, h->staged.rev.p, h->staged.ds.p, n_ds, h->s_dsrev.p,
+                        nullptr, nullptr, 0, h->outs.next.p, h->outs.actions.p, actuator_outcome ? h->s_outcome.p : nullptr,
+                        nullptr, st);
   if (rc) return rc;
   if (!sparse) {
     if (N) {
-      UST_CUDA(h, cudaMemcpyAsync(next_state, h->s_next.p, N, cudaMemcpyDeviceToHost, st));
-      UST_CUDA(h, cudaMemcpyAsync(actions, h->s_actions.p, N * 2, cudaMemcpyDeviceToHost, st));
+      UST_CUDA(h, cudaMemcpyAsync(next_state, h->outs.next.p, N, cudaMemcpyDeviceToHost, st));
+      UST_CUDA(h, cudaMemcpyAsync(actions, h->outs.actions.p, N * 2, cudaMemcpyDeviceToHost, st));
       if (actuator_outcome) UST_CUDA(h, cudaMemcpyAsync(actuator_outcome, h->s_outcome.p, N, cudaMemcpyDeviceToHost, st));
     }
   } else {
-    int e = ust_launch_diff((long long)n, h->s_next.p, h->s_actions.p, h->s_next_prev.p, h->s_actions_prev.p, h->sp_blocks.p,
-                            h->sp_count_dev, (long long)max_out, h->sp_idx.p, h->sp_next.p, h->sp_actions.p, st);
+    int e = ust_launch_diff((long long)n, h->outs.next.p, h->outs.actions.p, h->outs_prev.next.p, h->outs_prev.actions.p,
+                            h->sp_blocks.p, h->sp_count_dev, (long long)max_out, h->sp_idx.p, h->outs_sparse.next.p,
+                            h->outs_sparse.actions.p, st);
     if (e) return h->fail(UST_ERR_CUDA, "diff kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 3;
     UST_CUDA(h, cudaMemcpyAsync(h->sp_count_host, h->sp_count_dev, sizeof(long long), cudaMemcpyDeviceToHost, st));
@@ -907,12 +960,11 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
     *n_out = cnt;
     if (cnt <= max_out && cnt > 0) {
       UST_CUDA(h, cudaMemcpyAsync(out_idx, h->sp_idx.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, st));
-      UST_CUDA(h, cudaMemcpyAsync(next_state, h->sp_next.p, (size_t)cnt, cudaMemcpyDeviceToHost, st));
-      UST_CUDA(h, cudaMemcpyAsync(actions, h->sp_actions.p, (size_t)cnt * 2, cudaMemcpyDeviceToHost, st));
+      UST_CUDA(h, cudaMemcpyAsync(next_state, h->outs_sparse.next.p, (size_t)cnt, cudaMemcpyDeviceToHost, st));
+      UST_CUDA(h, cudaMemcpyAsync(actions, h->outs_sparse.actions.p, (size_t)cnt * 2, cudaMemcpyDeviceToHost, st));
     }
   }
-  rc = finish_with_counters(h, st, out);
-  if (rc != UST_ERR_CUDA && rc != UST_ERR_COMM) { h->resident_n = n; h->resident_n_ds = n_ds; h->outputs_resident = true; }
+  rc = adopt_resident(h, finish_with_counters(h, st, out), n, n_ds);
   if (sparse && (rc == UST_OK) && *n_out > max_out)
     return h->fail(UST_ERR_TRUNCATED, "%lld outputs changed, the caller's arrays hold %lld: fetch them with ust_fetch_outputs", (long long)*n_out, (long long)max_out);
   return rc;
@@ -962,8 +1014,8 @@ int ust_fetch_outputs(ust_handle* h, uint8_t* next_state, uint16_t* actions) {
   UST_CUDA(h, cudaSetDevice(h->device));
   const size_t N = (size_t)h->resident_n;
   if (N) {
-    UST_CUDA(h, cudaMemcpyAsync(next_state, h->s_next.p, N, cudaMemcpyDeviceToHost, h->stream));
-    UST_CUDA(h, cudaMemcpyAsync(actions, h->s_actions.p, N * 2, cudaMemcpyDeviceToHost, h->stream));
+    UST_CUDA(h, cudaMemcpyAsync(next_state, h->outs.next.p, N, cudaMemcpyDeviceToHost, h->stream));
+    UST_CUDA(h, cudaMemcpyAsync(actions, h->outs.actions.p, N * 2, cudaMemcpyDeviceToHost, h->stream));
   }
   UST_CUDA(h, cudaStreamSynchronize(h->stream));
   return UST_OK;
@@ -978,48 +1030,8 @@ int ust_apply_state_packed(ust_handle* h, const ust_policy* policy, int64_t n, c
   if (n < 0 || (n > 0 && (!state || !flags || !pod_rev16 || !ds_idx8 || !next_state || !actions)))
     return h->fail(UST_ERR_NIL_STATE, "currentState should not be empty");
   if (n_ds < 0 || n_ds > 127 || (n_ds > 0 && !ds_rev)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad DaemonSet table (the packed format holds at most 127 DaemonSets)");
-  UST_CUDA(h, cudaSetDevice(h->device));
-  StreamDrain drain(h);
-  cudaStream_t st = h->stream;
-  const size_t N = (size_t)n;
-  UST_CUDA(h, h->s_hot.reserve(N + 16));
-  UST_CUDA(h, h->s_flags.reserve(N + 4));
-  UST_CUDA(h, h->s_rev.reserve(N + 4));
-  UST_CUDA(h, h->s_ds.reserve(N + 4));
-  UST_CUDA(h, h->s_rev16.reserve(N + 8));
-  UST_CUDA(h, h->s_ds8.reserve(N + 16));
-  UST_CUDA(h, h->s_next.reserve(N + 16));
-  UST_CUDA(h, h->s_actions.reserve(N + 8));
-  UST_CUDA(h, h->s_dsrev.reserve((size_t)n_ds + 1));
-  if (actuator_outcome) UST_CUDA(h, h->s_outcome.reserve(N + 16));
-  if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsrev.p, ds_rev, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
-  h->resident_n = -1;
-  h->outputs_resident = false;
-  auto keep = [&](int rc) {
-    if (rc != UST_ERR_CUDA && rc != UST_ERR_INVALID_ARGUMENT && rc != UST_ERR_COMM && rc != UST_ERR_NIL_STATE) { h->resident_n = n; h->resident_n_ds = n_ds; h->outputs_resident = true; }
-    return rc;
-  };
-  if (n >= (1 << 19))
-    return keep(apply_pipelined(h, policy, n, state, flags, nullptr, nullptr, n_ds, next_state, actions, actuator_outcome, out,
-                                pod_rev16, ds_idx8));
-  if (N) {
-    UST_CUDA(h, cudaMemcpyAsync(h->s_hot.p, state, N, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, cudaMemcpyAsync(h->s_flags.p, flags, N * 4, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, cudaMemcpyAsync(h->s_rev16.p, pod_rev16, N * 2, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, cudaMemcpyAsync(h->s_ds8.p, ds_idx8, N, cudaMemcpyHostToDevice, st));
-    int we = ust_launch_widen((long long)n, h->s_rev16.p, h->s_ds8.p, h->s_rev.p, h->s_ds.p, 4 * h->num_sms, st);
-    if (we) return h->fail(UST_ERR_CUDA, "widen kernel launch failed: %s", cudaGetErrorString((cudaError_t)we));
-    h->launches += 1;
-  }
-  int rc = apply_device(h, policy, n, h->s_hot.p, h->s_flags.p, h->s_rev.p, h->s_ds.p, n_ds, h->s_dsrev.p, nullptr, nullptr, 0,
-                        h->s_next.p, h->s_actions.p, actuator_outcome ? h->s_outcome.p : nullptr, nullptr, st);
-  if (rc) return rc;
-  if (N) {
-    UST_CUDA(h, cudaMemcpyAsync(next_state, h->s_next.p, N, cudaMemcpyDeviceToHost, st));
-    UST_CUDA(h, cudaMemcpyAsync(actions, h->s_actions.p, N * 2, cudaMemcpyDeviceToHost, st));
-    if (actuator_outcome) UST_CUDA(h, cudaMemcpyAsync(actuator_outcome, h->s_outcome.p, N, cudaMemcpyDeviceToHost, st));
-  }
-  return keep(finish_with_counters(h, st, out));
+  return apply_host(h, policy, n, HostNodes{state, flags, nullptr, nullptr, pod_rev16, ds_idx8}, n_ds, ds_rev, nullptr,
+                    next_state, actions, actuator_outcome, out);
 }
 
 static int simulate_common(ust_handle* h, const ust_policy* policy, const ust_sim_options* opt, int32_t steps, ust_counters* history,
@@ -1040,13 +1052,9 @@ static int simulate_common(ust_handle* h, const ust_policy* policy, const ust_si
   cudaStream_t st = h->stream;
   const size_t N = (size_t)n;
   UST_CUDA(h, h->s_outcome.reserve(N + 16));
-  if ((size_t)steps + 1 > h->hist_cap) {
-    if (h->hist_dev) cudaFree(h->hist_dev);
-    h->hist_cap = (size_t)steps + 64;
-    UST_CUDA(h, cudaMalloc(&h->hist_dev, h->hist_cap * sizeof(ust_counters)));
-  }
-  h->resident_n = -1;
-  h->outputs_resident = false;
+  UST_CUDA(h, h->sim_hist.reserve((size_t)steps + 1));
+  const int32_t n_ds = h->resident_n_ds;
+  drop_resident(h);
   int grid = 8 * h->num_sms;
   UstSimParams sp;
   memset(&sp, 0, sizeof(sp));
@@ -1056,30 +1064,29 @@ static int simulate_common(ust_handle* h, const ust_policy* policy, const ust_si
     sp.wait_timeout = opt->wait_timeout_seconds; sp.job_seconds = opt->job_seconds; sp.validation_seconds = opt->validation_seconds;
     sp.validation_timeout = opt->validation_timeout_seconds; sp.maintenance_seconds = opt->maintenance_seconds;
     UST_CUDA(h, h->sim_entered.reserve(N + 1)); UST_CUDA(h, h->sim_wait.reserve(N + 1)); UST_CUDA(h, h->sim_valid.reserve(N + 1));
-    int e = ust_launch_sim_init(n, h->s_flags.p, h->sim_entered.p, h->sim_wait.p, h->sim_valid.p, grid, st);
+    int e = ust_launch_sim_init(n, h->staged.flags.p, h->sim_entered.p, h->sim_wait.p, h->sim_valid.p, grid, st);
     if (e) return h->fail(UST_ERR_CUDA, "simulation init kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 1;
   }
+  const Columns& s = h->staged;
   for (int32_t k = 0; k < steps; k++) {
-    int rc = apply_device(h, policy ? &pol : nullptr, n, h->s_hot.p, h->s_flags.p, h->s_rev.p, h->s_ds.p, h->resident_n_ds,
-                          h->s_dsrev.p, nullptr, nullptr, 0, h->s_next.p, h->s_actions.p, h->s_outcome.p, h->hist_dev + k, st);
+    int rc = apply_device(h, policy ? &pol : nullptr, n, s.hot.p, s.flags.p, s.rev.p, s.ds.p, n_ds, h->s_dsrev.p, nullptr, nullptr,
+                          0, h->outs.next.p, h->outs.actions.p, h->s_outcome.p, h->sim_hist.p + k, st);
     if (rc) return rc;
     sp.now = (long long)k * sp.dt;
-    int e = ust_launch_feedback(n, h->s_hot.p, h->s_flags.p, h->s_rev.p, h->s_ds.p, h->resident_n_ds, h->s_dsrev.p, h->s_next.p,
-                                h->s_actions.p, h->s_outcome.p, h->hist_dev + k, sp, h->sim_entered.p, h->sim_wait.p, h->sim_valid.p,
-                                grid, st);
+    int e = ust_launch_feedback(n, s.hot.p, s.flags.p, s.rev.p, s.ds.p, n_ds, h->s_dsrev.p, h->outs.next.p, h->outs.actions.p,
+                                h->s_outcome.p, h->sim_hist.p + k, sp, h->sim_entered.p, h->sim_wait.p, h->sim_valid.p, grid, st);
     if (e) return h->fail(UST_ERR_CUDA, "feedback kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 1;
   }
   std::vector<ust_counters> hist((size_t)steps);
-  if (steps) UST_CUDA(h, cudaMemcpyAsync(hist.data(), h->hist_dev, (size_t)steps * sizeof(ust_counters), cudaMemcpyDeviceToHost, st));
-  if (N && final_state) UST_CUDA(h, cudaMemcpyAsync(final_state, h->s_hot.p, N, cudaMemcpyDeviceToHost, st));
-  if (N && final_flags) UST_CUDA(h, cudaMemcpyAsync(final_flags, h->s_flags.p, N * 4, cudaMemcpyDeviceToHost, st));
-  if (N && final_pod_rev) UST_CUDA(h, cudaMemcpyAsync(final_pod_rev, h->s_rev.p, N * 4, cudaMemcpyDeviceToHost, st));
+  if (steps) UST_CUDA(h, cudaMemcpyAsync(hist.data(), h->sim_hist.p, (size_t)steps * sizeof(ust_counters), cudaMemcpyDeviceToHost, st));
+  if (N && final_state) UST_CUDA(h, cudaMemcpyAsync(final_state, s.hot.p, N, cudaMemcpyDeviceToHost, st));
+  if (N && final_flags) UST_CUDA(h, cudaMemcpyAsync(final_flags, s.flags.p, N * 4, cudaMemcpyDeviceToHost, st));
+  if (N && final_pod_rev) UST_CUDA(h, cudaMemcpyAsync(final_pod_rev, s.rev.p, N * 4, cudaMemcpyDeviceToHost, st));
   cudaError_t ce = cudaStreamSynchronize(st);
   if (ce != cudaSuccess) { h->ws_dirty = true; return h->fail(UST_ERR_CUDA, "kernel execution failed: %s", cudaGetErrorString(ce)); }
-  h->resident_n = n;  // the snapshot now holds the simulated state
-  h->outputs_resident = false;
+  adopt_resident(h, UST_OK, n, n_ds, false);  // the snapshot now holds the simulated state
   int32_t done = steps;
   int rc = UST_OK;
   for (int32_t k = 0; k < steps; k++)
@@ -1114,35 +1121,24 @@ int ust_build_state(ust_handle* h, int64_t n_pods, const uint8_t* state, const i
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   if (n_pods < 0 || (n_pods > 0 && (!state || !ds_idx)) || n_ds < 0 || (n_ds > 0 && !ds_desired))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
-  h->resident_n = -1;  // shares the staging arrays
-  h->outputs_resident = false;
+  drop_resident(h);  // shares the staging arrays
   UST_CUDA(h, cudaSetDevice(h->device));
   StreamDrain drain(h);
   cudaStream_t st = h->stream;
   const size_t N = (size_t)n_pods;
-  UST_CUDA(h, h->s_hot.reserve(N + 16));
-  UST_CUDA(h, h->s_ds.reserve(N + 4));
+  UST_CUDA(h, h->staged.hot.reserve(N + 16));
+  UST_CUDA(h, h->staged.ds.reserve(N + 4));
   UST_CUDA(h, h->s_dsdesired.reserve((size_t)n_ds + 1));
-  if ((size_t)n_ds + 1 > h->ds_count_cap) {
-    if (h->ds_count_dev) cudaFree(h->ds_count_dev);
-    h->ds_count_cap = (size_t)n_ds + 64;
-    UST_CUDA(h, cudaMalloc(&h->ds_count_dev, h->ds_count_cap * sizeof(unsigned long long)));
-    UST_CUDA(h, cudaMemsetAsync(h->ds_count_dev, 0, h->ds_count_cap * sizeof(unsigned long long), st));
-  }
-  if (h->ws_dirty) { UST_CUDA(h, clear_workspace(h,st)); h->ws_dirty = false; }
   if (N) {
-    UST_CUDA(h, cudaMemcpyAsync(h->s_hot.p, state, N, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, cudaMemcpyAsync(h->s_ds.p, ds_idx, N * 4, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, cudaMemcpyAsync(h->staged.hot.p, state, N, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, cudaMemcpyAsync(h->staged.ds.p, ds_idx, N * 4, cudaMemcpyHostToDevice, st));
   }
   if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsdesired.p, ds_desired, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
-  int64_t grid = (n_pods + 1023) / 1024;  // 256 threads x 4 pods per iteration
-  if (grid < 1) grid = 1;
-  if (grid > 8 * h->num_sms) grid = 8 * h->num_sms;
-  h->ws_dirty = true;
-  int e = ust_launch_build_state(n_pods, h->s_hot.p, h->s_ds.p, n_ds, h->s_dsdesired.p, h->ds_count_dev, h->ws, h->counters_dev, (int)grid, st);
-  if (e) return h->fail(UST_ERR_CUDA, "build-state kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
-  h->ws_dirty = false;
-  h->launches += 2;
+  int rc = build_state_launch(h, n_pods, n_ds, st, [&](int grid) {
+    return ust_launch_build_state(n_pods, h->staged.hot.p, h->staged.ds.p, n_ds, h->s_dsdesired.p, h->ds_count.p, h->ws,
+                                  h->counters_dev, grid, st);
+  });
+  if (rc) return rc;
   return finish_with_counters(h, st, out);
 }
 
@@ -1169,42 +1165,30 @@ int ust_build_state_uids(ust_handle* h, int64_t n_pods, const uint8_t* state, co
     }
     tab[2 * s] = x; tab[2 * s + 1] = y; tab_idx[s] = d;
   }
-  h->resident_n = -1;  // shares the staging arrays
-  h->outputs_resident = false;
+  drop_resident(h);  // shares the staging arrays
   UST_CUDA(h, cudaSetDevice(h->device));
   StreamDrain drain(h);
   cudaStream_t st = h->stream;
   const size_t N = (size_t)n_pods;
-  UST_CUDA(h, h->s_hot.reserve(N + 16));
-  UST_CUDA(h, h->s_ds.reserve(N + 4));
+  UST_CUDA(h, h->staged.hot.reserve(N + 16));
+  UST_CUDA(h, h->staged.ds.reserve(N + 4));
   UST_CUDA(h, h->s_uid.reserve(2 * N + 2));
   UST_CUDA(h, h->s_dsuid.reserve(2 * slots));
   UST_CUDA(h, h->s_dsorder.reserve(slots));
   UST_CUDA(h, h->s_dsdesired.reserve((size_t)n_ds + 1));
-  if ((size_t)n_ds + 1 > h->ds_count_cap) {
-    if (h->ds_count_dev) cudaFree(h->ds_count_dev);
-    h->ds_count_cap = (size_t)n_ds + 64;
-    UST_CUDA(h, cudaMalloc(&h->ds_count_dev, h->ds_count_cap * sizeof(unsigned long long)));
-    UST_CUDA(h, cudaMemsetAsync(h->ds_count_dev, 0, h->ds_count_cap * sizeof(unsigned long long), st));
-  }
-  if (h->ws_dirty) { UST_CUDA(h, clear_workspace(h,st)); h->ws_dirty = false; }
   if (N) {
-    UST_CUDA(h, cudaMemcpyAsync(h->s_hot.p, state, N, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, cudaMemcpyAsync(h->staged.hot.p, state, N, cudaMemcpyHostToDevice, st));
     UST_CUDA(h, cudaMemcpyAsync(h->s_uid.p, owner_uid, N * 16, cudaMemcpyHostToDevice, st));
   }
   UST_CUDA(h, cudaMemcpyAsync(h->s_dsuid.p, tab.data(), slots * 16, cudaMemcpyHostToDevice, st));
   UST_CUDA(h, cudaMemcpyAsync(h->s_dsorder.p, tab_idx.data(), slots * 4, cudaMemcpyHostToDevice, st));
   if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsdesired.p, ds_desired, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
-  int64_t grid = (n_pods + 1023) / 1024;  // 256 threads x 4 pods per iteration
-  if (grid < 1) grid = 1;
-  if (grid > 8 * h->num_sms) grid = 8 * h->num_sms;
-  h->ws_dirty = true;
-  int e = ust_launch_build_state_uids(n_pods, h->s_hot.p, h->s_uid.p, n_ds, h->s_dsuid.p, h->s_dsorder.p, (int)slots,
-                                      h->s_dsdesired.p, h->s_ds.p, h->ds_count_dev, h->ws, h->counters_dev, (int)grid, st);
-  if (e) return h->fail(UST_ERR_CUDA, "build-state kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
-  h->ws_dirty = false;
-  h->launches += 2;
-  if (N) UST_CUDA(h, cudaMemcpyAsync(ds_idx_out, h->s_ds.p, N * 4, cudaMemcpyDeviceToHost, st));
+  int rc = build_state_launch(h, n_pods, n_ds, st, [&](int grid) {
+    return ust_launch_build_state_uids(n_pods, h->staged.hot.p, h->s_uid.p, n_ds, h->s_dsuid.p, h->s_dsorder.p, (int)slots,
+                                       h->s_dsdesired.p, h->staged.ds.p, h->ds_count.p, h->ws, h->counters_dev, grid, st);
+  });
+  if (rc) return rc;
+  if (N) UST_CUDA(h, cudaMemcpyAsync(ds_idx_out, h->staged.ds.p, N * 4, cudaMemcpyDeviceToHost, st));
   return finish_with_counters(h, st, out);  // synchronises the stream: `tab` / `tab_idx` outlive their copies
 }
 
