@@ -325,6 +325,39 @@ int ust_apply_state_delta_splice(ust_handle* h, const ust_policy* policy, const 
                                  const int64_t* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
                                  const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, int64_t max_out, int64_t* out_idx,
                                  uint8_t* out_next_state, uint16_t* out_actions, int64_t* n_out, ust_counters* out);
+/* New node order of the resident snapshot of n nodes, as runs concatenated in order r = 0 .. n_runs-1:
+ *   run_src[r] >= 0   old nodes run_src[r] .. run_src[r] + run_len[r] - 1, in that order (all in [0, n))
+ *   run_src[r] == -1  the next run_len[r] of the n_insert new nodes (state / flags / pod_rev / ds_idx), in the order given
+ * run_len[r] >= 1. No old node is named by two runs; old nodes that no run names have left the snapshot. The inserted
+ * runs take exactly n_insert nodes. The new snapshot has sum(run_len) nodes (n_runs == 0: it is empty). */
+typedef struct ust_reorder {
+  int64_t n_runs;
+  const int64_t* run_src;
+  const int64_t* run_len;
+  int64_t n_insert;
+  const uint8_t* state;
+  const uint32_t* flags;
+  const int32_t* pod_rev;
+  const int32_t* ds_idx;
+} ust_reorder;
+
+/* ust_apply_state_delta_splice for any new node order: nodes that stay may also move (a driver pod re-created under a
+ * new name moves its node in BuildState's list). The reorder is applied on the device first (one gather pass over the
+ * resident columns and the previous call's outputs), then the n_changed overwrites exactly as in ust_apply_state_delta,
+ * with idx as distinct indices into the NEW snapshot, then the whole new snapshot is evaluated. Sparse outputs are in
+ * new-index order: every inserted node is reported, a node that stayed when its (next_state, actions) differ from what
+ * the previous call returned for it (wherever it moved), a node that left never. UST_ERR_TRUNCATED and
+ * ust_fetch_outputs (then with the new node count) work as in ust_apply_state_delta_splice; counters, aborts and error
+ * codes are those of ust_apply_state on the reordered arrays. reorder == NULL: exactly ust_apply_state_delta_sparse. A
+ * violated contract (a run length below 1 or run_src below -1, an old run that leaves [0, n), two runs that name the
+ * same old node, inserted runs whose total is not n_insert, NULL arrays, a new size of 2^40 nodes or more, idx outside
+ * the new snapshot, no resident snapshot or outputs, more than one rank set up by ust_comm_init) returns
+ * UST_ERR_INVALID_ARGUMENT before any device work: the resident snapshot stays as it was. The runs are checked in
+ * O(n + n_runs) host time. */
+int ust_apply_state_delta_reorder(ust_handle* h, const ust_policy* policy, const ust_reorder* reorder, int64_t n_changed,
+                                  const int64_t* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
+                                  const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, int64_t max_out, int64_t* out_idx,
+                                  uint8_t* out_next_state, uint16_t* out_actions, int64_t* n_out, ust_counters* out);
 /* The full outputs of the last call on the resident snapshot (n_nodes entries each). */
 int ust_fetch_outputs(ust_handle* h, uint8_t* next_state, uint16_t* actions);
 

@@ -49,8 +49,8 @@ def build_host(force=False):
 
 
 def build_host_tests(root):
-    """tests/host/_build/{upgrade_state_test,host_logic_test,membership_test}: the reference's specs against the mirror,
-    and the incremental path under membership changes."""
+    """tests/host/_build/{upgrade_state_test,host_logic_test,membership_test,reorder_test}: the reference's specs against
+    the mirror, and the incremental path under membership changes and nodes that move in the list."""
     tdir = os.path.join(root, "tests", "host")
     bdir = os.path.join(tdir, "_build")
     os.makedirs(bdir, exist_ok=True)
@@ -59,7 +59,8 @@ def build_host_tests(root):
     srcs = [os.path.join(tdir, f) for f in os.listdir(tdir) if f.endswith((".cpp", ".hpp"))] + [HOST_OUT, os.path.abspath(__file__)]
     out = []
     oracle = ["-L" + os.path.join(root, "oracle"), "-lust_oracle", "-Wl,-rpath," + os.path.join(root, "oracle")]
-    for name, extra in (("upgrade_state_test", []), ("host_logic_test", oracle), ("membership_test", oracle)):
+    for name, extra in (("upgrade_state_test", []), ("host_logic_test", oracle), ("membership_test", oracle),
+                        ("reorder_test", oracle)):
         exe = os.path.join(bdir, name)
         if not os.path.exists(exe) or any(os.path.getmtime(x) > os.path.getmtime(exe) for x in srcs):
             subprocess.check_call(common + [os.path.join(tdir, name + ".cpp"), "-o", exe] + link + extra)

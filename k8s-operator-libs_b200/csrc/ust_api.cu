@@ -191,12 +191,16 @@ struct ust_handle {
   DevBuf<uint64_t> s_uid, s_dsuid;   // BuildState owner join: pod owner UIDs, DaemonSet UID hash table (+ s_dsorder: slot -> index)
   DevBuf<int32_t> s_dsorder;
   IndexedColumns changed;            // delta updates: indices and values of the changed nodes
-  // membership splice: the second set the splice kernel writes (swapped with the resident columns and the previous
-  // outputs afterwards; allocated on the first splice), the removal list and the inserted nodes with their positions
+  // new node order (splice, reorder): the second set the splice / gather kernel writes (swapped with the resident columns
+  // and the previous outputs afterwards; allocated on the first such call), the removal list, the reorder's runs
+  // (run_off, then run_src: see add_run) and the inserted nodes with their positions (splice); run_seen: one bit per old
+  // node while a reorder is checked, all zero between calls
   Columns splice_cols;
   Outputs splice_outs;
-  DevBuf<long long> removed;
+  DevBuf<long long> removed, runs;
   IndexedColumns inserted;
+  std::vector<long long> run_off, run_src;
+  std::vector<uint64_t> run_seen;
   DevBuf<int32_t> sim_entered, sim_wait, sim_valid;  // timed rollout simulation: per-node clocks
 
   // multi-GPU
@@ -856,31 +860,119 @@ int ust_apply_state(ust_handle* h, const ust_policy* policy, int64_t n, const ui
                     actions, actuator_outcome, out);
 }
 
-// ust_apply_state_delta, _delta_sparse and _delta_splice: splice the resident snapshot (optional: nodes leave and join),
-// scatter the re-encoded nodes into it, evaluate everything, return all outputs (dense) or the outputs that differ from
-// the previous call's (sparse).
-static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splice* sp, int64_t n_changed, const int64_t* idx,
-                        const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds,
-                        const int32_t* ds_rev, bool sparse, uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome,
-                        int64_t max_out, int64_t* out_idx, int64_t* n_out, ust_counters* out) {
+// The runs of a reorder as the gather kernel reads them (ust_launch_reorder): h->run_off holds the exclusive prefix of
+// the run lengths (one entry more than there are runs), h->run_src per run the old start, or -1 - offset into the
+// inserted nodes. Adjacent runs that continue each other are merged.
+static void clear_runs(ust_handle* h) {
+  h->run_off.assign(1, 0);
+  h->run_src.clear();
+}
+static void add_run(ust_handle* h, long long src, long long len) {
+  if (!h->run_src.empty()) {
+    const long long last = h->run_src.back(), last_len = h->run_off.back() - h->run_off[h->run_off.size() - 2];
+    if ((last >= 0) == (src >= 0) && (src >= 0 ? last + last_len == src : last - last_len == src)) {
+      h->run_off.back() += len;
+      return;
+    }
+  }
+  h->run_src.push_back(src);
+  h->run_off.push_back(h->run_off.back() + len);
+}
+
+// Bits [a, a + len) of the bitmap: set (false when one of them was set already) or cleared.
+static bool mark_bits(uint64_t* w, long long a, long long len, bool set) {
+  const long long e = a + len;
+  for (long long i = a >> 6; i <= (e - 1) >> 6; i++) {
+    const long long lo = std::max(a, i << 6), hi = std::min(e, (i + 1) << 6);
+    const uint64_t m = hi - lo == 64 ? ~0ull : ((1ull << (hi - lo)) - 1) << (lo & 63);
+    if (!set) { w[i] &= ~m; continue; }
+    if (w[i] & m) return false;
+    w[i] |= m;
+  }
+  return true;
+}
+
+// A reorder checked in full and turned into runs, O(n + n_runs): a bitmap over the old snapshot finds old nodes that two
+// runs name. Sets *n_new to the new snapshot's size.
+static int reorder_runs(ust_handle* h, const ust_reorder* ro, int64_t n_old, int64_t* n_new) {
+  if (ro->n_runs < 0 || ro->n_insert < 0 || (ro->n_runs > 0 && (!ro->run_src || !ro->run_len)) ||
+      (ro->n_insert > 0 && (!ro->state || !ro->flags || !ro->pod_rev || !ro->ds_idx)))
+    return h->fail(UST_ERR_INVALID_ARGUMENT, "bad reorder");
+  const size_t words = ((size_t)n_old + 63) / 64;
+  if (h->run_seen.size() < words) h->run_seen.resize(words, 0);
+  clear_runs(h);
+  int rc = UST_OK;
+  int64_t marked = 0, ins = 0;  // runs whose old nodes are marked; inserted nodes taken
+  for (int64_t r = 0; r < ro->n_runs && rc == UST_OK; r++) {
+    const long long src = ro->run_src[r], len = ro->run_len[r];
+    if (len < 1 || src < -1)
+      rc = h->fail(UST_ERR_INVALID_ARGUMENT, "reorder: run %lld has source %lld and length %lld", (long long)r, src, len);
+    else if (len >= (1LL << 40) - h->run_off.back())
+      rc = h->fail(UST_ERR_INVALID_ARGUMENT, "too many nodes");
+    else if (src < 0 && len > ro->n_insert - ins)
+      rc = h->fail(UST_ERR_INVALID_ARGUMENT, "reorder: the inserted runs take more than the %lld inserted nodes", (long long)ro->n_insert);
+    else if (src >= 0 && (src >= n_old || len > n_old - src))
+      rc = h->fail(UST_ERR_INVALID_ARGUMENT, "reorder: run %lld (old nodes %lld + %lld) leaves the snapshot of %lld nodes", (long long)r, src,
+                   len, (long long)n_old);
+    else if (src >= 0 && (marked = r + 1, !mark_bits(h->run_seen.data(), src, len, true)))
+      rc = h->fail(UST_ERR_INVALID_ARGUMENT, "reorder: run %lld names an old node that an earlier run names", (long long)r);
+    else if (src < 0) {
+      add_run(h, -1 - ins, len);
+      ins += len;
+    } else {
+      add_run(h, src, len);
+    }
+  }
+  for (int64_t r = 0; r < marked; r++)  // the bitmap is all zero again
+    if (ro->run_src[r] >= 0) mark_bits(h->run_seen.data(), ro->run_src[r], ro->run_len[r], false);
+  if (rc == UST_OK && ins != ro->n_insert)
+    rc = h->fail(UST_ERR_INVALID_ARGUMENT, "reorder: the inserted runs take %lld of the %lld inserted nodes", (long long)ins, (long long)ro->n_insert);
+  *n_new = h->run_off.back();
+  return rc;
+}
+
+// ust_apply_state_delta, _delta_sparse, _delta_splice and _delta_reorder: bring the resident snapshot into a new node
+// order (optional: nodes leave, join and move), scatter the re-encoded nodes into it, evaluate everything, return all
+// outputs (dense) or the outputs that differ from the previous call's (sparse).
+static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splice* sp, const ust_reorder* ro, int64_t n_changed,
+                        const int64_t* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx,
+                        int32_t n_ds, const int32_t* ds_rev, bool sparse, uint8_t* next_state, uint16_t* actions,
+                        uint8_t* actuator_outcome, int64_t max_out, int64_t* out_idx, int64_t* n_out, ust_counters* out) {
   const int64_t n_old = h->resident_n;
   if (n_old < 0) return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident snapshot: call ust_apply_state (without pod lists) first");
   if (sparse && !h->outputs_resident)
     return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident outputs to compare with: the previous call must be an ApplyState on this snapshot");
-  // the splice, checked in full before anything is touched
-  const int64_t n_rm = sp ? sp->n_remove : 0, n_ins = sp ? sp->n_insert : 0;
-  if (n_rm < 0 || n_ins < 0 || n_rm > n_old || (n_rm > 0 && !sp->remove_idx) ||
-      (n_ins > 0 && (!sp->insert_before || !sp->state || !sp->flags || !sp->pod_rev || !sp->ds_idx)))
-    return h->fail(UST_ERR_INVALID_ARGUMENT, "bad splice");
-  for (int64_t k = 0; k < n_rm; k++)
-    if (sp->remove_idx[k] < (k ? sp->remove_idx[k - 1] + 1 : 0) || sp->remove_idx[k] >= n_old)
-      return h->fail(UST_ERR_INVALID_ARGUMENT, "splice: remove_idx[%lld] = %lld is not strictly increasing in [0, %lld)", (long long)k,
-                     (long long)sp->remove_idx[k], (long long)n_old);
-  for (int64_t k = 0; k < n_ins; k++)
-    if (sp->insert_before[k] < (k ? sp->insert_before[k - 1] : 0) || sp->insert_before[k] > n_old)
-      return h->fail(UST_ERR_INVALID_ARGUMENT, "splice: insert_before[%lld] = %lld is not non-decreasing in [0, %lld]", (long long)k,
-                     (long long)sp->insert_before[k], (long long)n_old);
-  const int64_t n = n_old - n_rm + n_ins;
+  // the new node order, checked in full before anything is touched
+  int64_t n = n_old, n_ins = 0;
+  const uint8_t* ins_state = nullptr;
+  const uint32_t* ins_flags = nullptr;
+  const int32_t *ins_rev = nullptr, *ins_ds = nullptr;
+  bool gather = false;
+  if (ro) {
+    if (int rc = reorder_runs(h, ro, n_old, &n)) return rc;
+    gather = true;
+    n_ins = ro->n_insert;
+    ins_state = ro->state; ins_flags = ro->flags; ins_rev = ro->pod_rev; ins_ds = ro->ds_idx;
+  } else {
+    const int64_t n_rm = sp ? sp->n_remove : 0;
+    n_ins = sp ? sp->n_insert : 0;
+    if (n_rm < 0 || n_ins < 0 || n_rm > n_old || (n_rm > 0 && !sp->remove_idx) ||
+        (n_ins > 0 && (!sp->insert_before || !sp->state || !sp->flags || !sp->pod_rev || !sp->ds_idx)))
+      return h->fail(UST_ERR_INVALID_ARGUMENT, "bad splice");
+    for (int64_t k = 0; k < n_rm; k++)
+      if (sp->remove_idx[k] < (k ? sp->remove_idx[k - 1] + 1 : 0) || sp->remove_idx[k] >= n_old)
+        return h->fail(UST_ERR_INVALID_ARGUMENT, "splice: remove_idx[%lld] = %lld is not strictly increasing in [0, %lld)", (long long)k,
+                       (long long)sp->remove_idx[k], (long long)n_old);
+    for (int64_t k = 0; k < n_ins; k++)
+      if (sp->insert_before[k] < (k ? sp->insert_before[k - 1] : 0) || sp->insert_before[k] > n_old)
+        return h->fail(UST_ERR_INVALID_ARGUMENT, "splice: insert_before[%lld] = %lld is not non-decreasing in [0, %lld]", (long long)k,
+                       (long long)sp->insert_before[k], (long long)n_old);
+    n = n_old - n_rm + n_ins;
+    gather = n_rm || n_ins;
+    if (gather) {
+      ins_state = sp->state; ins_flags = sp->flags; ins_rev = sp->pod_rev; ins_ds = sp->ds_idx;
+    }
+  }
   if (n >= (1LL << 40)) return h->fail(UST_ERR_INVALID_ARGUMENT, "too many nodes");
   if (n_changed < 0 || (n_changed > 0 && (!idx || !state || !flags || !pod_rev || !ds_idx)))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
@@ -893,12 +985,14 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
   UST_CUDA(h, cudaSetDevice(h->device));
   StreamDrain drain(h);
   cudaStream_t st = h->stream;
-  const size_t N = (size_t)n, M = (size_t)n_changed, R = (size_t)n_rm, I = (size_t)n_ins;
-  if (R || I) {  // the previous outputs travel with the snapshot
+  const size_t N = (size_t)n, M = (size_t)n_changed, I = (size_t)n_ins, NR = h->run_src.size();
+  const size_t R = !ro && gather ? (size_t)sp->n_remove : 0;
+  if (gather) {  // the previous outputs travel with the snapshot
     UST_CUDA(h, h->splice_cols.reserve(N));
     UST_CUDA(h, h->splice_outs.reserve(N));
-    UST_CUDA(h, h->removed.reserve(R + 1));
-    UST_CUDA(h, h->inserted.idx.reserve(I + 1));
+    if (ro) UST_CUDA(h, h->runs.reserve(2 * NR + 2));
+    else UST_CUDA(h, h->removed.reserve(R + 1));
+    if (!ro) UST_CUDA(h, h->inserted.idx.reserve(I + 1));
     UST_CUDA(h, h->inserted.cols.reserve(I));
   }
   UST_CUDA(h, h->s_dsrev.reserve((size_t)n_ds + 1));
@@ -913,17 +1007,30 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
   }
   drop_resident(h);  // until the patched snapshot has been evaluated
   if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsrev.p, ds_rev, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
-  if (R || I) {
-    if (R) UST_CUDA(h, cudaMemcpyAsync(h->removed.p, sp->remove_idx, R * 8, cudaMemcpyHostToDevice, st));
-    if (I) UST_CUDA(h, cudaMemcpyAsync(h->inserted.idx.p, sp->insert_before, I * 8, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, h->inserted.cols.upload(sp->state, sp->flags, sp->pod_rev, sp->ds_idx, 0, I, st));
+  if (gather) {
+    UST_CUDA(h, h->inserted.cols.upload(ins_state, ins_flags, ins_rev, ins_ds, 0, I, st));
     const Columns &in = h->inserted.cols, &s = h->staged, &x = h->splice_cols;
-    int e = ust_launch_splice((long long)n_old, (long long)n_rm, h->removed.p, (long long)n_ins, h->inserted.idx.p, in.hot.p, in.flags.p,
-                              in.rev.p, in.ds.p, s.hot.p, s.flags.p, s.rev.p, s.ds.p, h->outs.next.p, h->outs.actions.p,
-                              x.hot.p, x.flags.p, x.rev.p, x.ds.p, h->splice_outs.next.p, h->splice_outs.actions.p, st);
-    if (e) return h->fail(UST_ERR_CUDA, "splice kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    int e;
+    if (ro) {
+      long long* off = h->runs.p;
+      long long* src = h->runs.p + NR + 1;
+      UST_CUDA(h, cudaMemcpyAsync(off, h->run_off.data(), (NR + 1) * 8, cudaMemcpyHostToDevice, st));
+      if (NR) UST_CUDA(h, cudaMemcpyAsync(src, h->run_src.data(), NR * 8, cudaMemcpyHostToDevice, st));
+      e = ust_launch_reorder((long long)n, (long long)NR, off, src, in.hot.p, in.flags.p, in.rev.p, in.ds.p, s.hot.p, s.flags.p, s.rev.p,
+                             s.ds.p, h->outs.next.p, h->outs.actions.p, x.hot.p, x.flags.p, x.rev.p, x.ds.p, h->splice_outs.next.p,
+                             h->splice_outs.actions.p, st);
+      if (e) return h->fail(UST_ERR_CUDA, "reorder kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    } else {
+      // a splice keeps its own kernel: the gather kernel measured slower on splices (DESIGN.md §3.4)
+      if (R) UST_CUDA(h, cudaMemcpyAsync(h->removed.p, sp->remove_idx, R * 8, cudaMemcpyHostToDevice, st));
+      if (I) UST_CUDA(h, cudaMemcpyAsync(h->inserted.idx.p, sp->insert_before, I * 8, cudaMemcpyHostToDevice, st));
+      e = ust_launch_splice((long long)n_old, (long long)R, h->removed.p, (long long)n_ins, h->inserted.idx.p, in.hot.p, in.flags.p,
+                            in.rev.p, in.ds.p, s.hot.p, s.flags.p, s.rev.p, s.ds.p, h->outs.next.p, h->outs.actions.p,
+                            x.hot.p, x.flags.p, x.rev.p, x.ds.p, h->splice_outs.next.p, h->splice_outs.actions.p, st);
+      if (e) return h->fail(UST_ERR_CUDA, "splice kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    }
     h->launches += 1;
-    // the spliced set becomes the resident one (the previous outputs in `outs`, as after any call)
+    // the new set becomes the resident one (the previous outputs in `outs`, as after any call)
     std::swap(h->staged, h->splice_cols);
     std::swap(h->outs, h->splice_outs);
   }
@@ -977,7 +1084,7 @@ int ust_apply_state_delta(ust_handle* h, const ust_policy* policy, int64_t n_cha
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  return delta_common(h, policy, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, false, next_state, actions,
+  return delta_common(h, policy, nullptr, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, false, next_state, actions,
                       actuator_outcome, 0, nullptr, nullptr, out);
 }
 
@@ -988,7 +1095,7 @@ int ust_apply_state_delta_sparse(ust_handle* h, const ust_policy* policy, int64_
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  return delta_common(h, policy, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
+  return delta_common(h, policy, nullptr, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
                       nullptr, max_out, out_idx, n_out, out);
 }
 
@@ -1001,8 +1108,21 @@ int ust_apply_state_delta_splice(ust_handle* h, const ust_policy* policy, const 
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   // node indices of a shard are global ranges (ust_comm_init): a splice would have to move them on every rank
   if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_splice runs on one GPU");
-  return delta_common(h, policy, splice, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
+  return delta_common(h, policy, splice, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
                       nullptr, max_out, out_idx, n_out, out);
+}
+
+int ust_apply_state_delta_reorder(ust_handle* h, const ust_policy* policy, const ust_reorder* reorder, int64_t n_changed,
+                                  const int64_t* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
+                                  const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, int64_t max_out, int64_t* out_idx,
+                                  uint8_t* out_next_state, uint16_t* out_actions, int64_t* n_out, ust_counters* out) {
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
+  // node indices of a shard are global ranges (ust_comm_init): a reorder would have to move them on every rank
+  if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_reorder runs on one GPU");
+  return delta_common(h, policy, nullptr, reorder, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state,
+                      out_actions, nullptr, max_out, out_idx, n_out, out);
 }
 
 int ust_fetch_outputs(ust_handle* h, uint8_t* next_state, uint16_t* actions) {

@@ -181,6 +181,13 @@ int ust_launch_splice(long long n, long long n_rm, const long long* rm, long lon
                       const uint32_t* ins_flags, const int32_t* ins_rev, const int32_t* ins_ds, const uint8_t* hot, const uint32_t* flags,
                       const int32_t* rev, const int32_t* ds, const uint8_t* next, const uint16_t* act, uint8_t* o_hot, uint32_t* o_flags,
                       int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, void* stream);
+// new node order of the resident snapshot (ust_apply_state_delta_reorder): the resident columns and the previous
+// outputs, gathered into the o_* arrays (n entries). Run r covers new positions [run_off[r], run_off[r + 1]) and reads old
+// nodes from run_src[r] on, or inserted nodes from -1 - run_src[r] on (run_src[r] < 0); checked by the caller
+int ust_launch_reorder(long long n, long long n_runs, const long long* run_off, const long long* run_src, const uint8_t* ins_hot,
+                       const uint32_t* ins_flags, const int32_t* ins_rev, const int32_t* ins_ds, const uint8_t* hot, const uint32_t* flags,
+                       const int32_t* rev, const int32_t* ds, const uint8_t* next, const uint16_t* act, uint8_t* o_hot, uint32_t* o_flags,
+                       int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, void* stream);
 // rollout simulation: the clock of the feedback between two reconciles (include/ust.h, ust_sim_options)
 struct UstSimParams {
   int timed;            // 0: whatever a node waits for has happened by the next reconcile

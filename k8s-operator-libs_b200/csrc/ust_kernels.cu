@@ -12,7 +12,8 @@
 // every tile with the reference's abort semantics (nodes the sequential passes had not reached stay untouched,
 // common_manager.go:462-523).
 // Around it: ust_pod_summary_kernel (pod lists -> one byte per node), ust_build_state*_kernel (BuildState),
-// ust_patch_kernel / ust_splice_kernel / ust_feedback_kernel (delta updates, membership changes, rollout simulation),
+// ust_patch_kernel / ust_splice_kernel / ust_reorder_kernel / ust_feedback_kernel (delta updates, membership changes,
+// new node orders, rollout simulation),
 // ust_widen_kernel (packed host format).
 #include <climits>
 
@@ -876,6 +877,70 @@ __global__ void __launch_bounds__(kThreads) ust_splice_kernel(long long n, long 
   }
 }
 
+// New node order of the resident snapshot (ust_apply_state_delta_reorder): one pass that writes every node of the new
+// snapshot at its new index in a second buffer set. The new order is a list of runs: run r covers new positions [run_off[r], run_off[r + 1]) and reads them from old nodes
+// run_src[r], run_src[r] + 1, ... (run_src >= 0), or from inserted nodes -1 - run_src, ... (run_src < 0), whose previous
+// output next_state is 0xFF (no state code equals it, so the diff reports them). A CTA owns kGatherTile new positions;
+// it finds the runs that cover them once, by binary search, and stages their offsets and sources in shared memory
+// (every run is at least one position long, so at most kGatherTile of them meet a tile). Each thread then finds its
+// positions' runs in that range, walking forward from the run of its previous position.
+// 16 B read + 16 B written per node, 16 B per run; a run is read contiguously.
+constexpr int kGatherTile = 2048;
+
+__global__ void __launch_bounds__(kThreads) ust_reorder_kernel(long long n, long long n_runs, const long long* __restrict__ run_off,
+                                                               const long long* __restrict__ run_src,
+                                                               const uint8_t* __restrict__ ins_hot, const uint32_t* __restrict__ ins_flags,
+                                                               const int32_t* __restrict__ ins_rev, const int32_t* __restrict__ ins_ds,
+                                                               const uint8_t* __restrict__ hot, const uint32_t* __restrict__ flags,
+                                                               const int32_t* __restrict__ rev, const int32_t* __restrict__ ds,
+                                                               const uint8_t* __restrict__ next, const uint16_t* __restrict__ act,
+                                                               uint8_t* __restrict__ o_hot, uint32_t* __restrict__ o_flags,
+                                                               int32_t* __restrict__ o_rev, int32_t* __restrict__ o_ds,
+                                                               uint8_t* __restrict__ o_next, uint16_t* __restrict__ o_act) {
+  __shared__ long long s_off[kGatherTile];
+  __shared__ long long s_src[kGatherTile];
+  __shared__ long long s_runs[2];
+  const int t = threadIdx.x;
+  const long long b0 = (long long)blockIdx.x * kGatherTile;
+  if (b0 >= n) return;  // n == 0: the one CTA of the launch has nothing to do
+  const long long b1 = b0 + kGatherTile < n ? b0 + kGatherTile : n;
+  if (t < 2) {  // the last run that starts at or before b0 (t = 0) / b1 - 1 (t = 1)
+    const long long v = t ? b1 - 1 : b0;
+    long long lo = 0, hi = n_runs;
+    while (hi - lo > 1) {
+      const long long mid = (lo + hi) >> 1;
+      if (__ldg(run_off + mid) <= v) lo = mid; else hi = mid;
+    }
+    s_runs[t] = lo;
+  }
+  __syncthreads();
+  const long long r0 = s_runs[0];
+  const int nr = (int)(s_runs[1] - r0 + 1);
+  for (int j = t; j < nr; j += kThreads) { s_off[j] = __ldg(run_off + r0 + j); s_src[j] = __ldg(run_src + r0 + j); }
+  __syncthreads();
+  const int len = (int)(b1 - b0);
+  int r = 0;
+#pragma unroll 4
+  for (int j = t; j < len; j += kThreads) {
+    const long long p = b0 + j;
+    int hi = nr;
+    while (hi - r > 1) {
+      const int mid = (r + hi) >> 1;
+      if (s_off[mid] <= p) r = mid; else hi = mid;
+    }
+    const long long src = s_src[r], k = p - s_off[r];
+    if (src >= 0) {
+      const long long i = src + k;
+      o_hot[p] = __ldcs(hot + i); o_flags[p] = __ldcs(flags + i); o_rev[p] = __ldcs(rev + i); o_ds[p] = __ldcs(ds + i);
+      o_next[p] = __ldcs(next + i); o_act[p] = __ldcs(act + i);
+    } else {
+      const long long i = -1 - src + k;
+      o_hot[p] = __ldg(ins_hot + i); o_flags[p] = __ldg(ins_flags + i); o_rev[p] = __ldg(ins_rev + i); o_ds[p] = __ldg(ins_ds + i);
+      o_next[p] = 0xFF; o_act[p] = 0;
+    }
+  }
+}
+
 // Rollout simulation (SURVEY 8f.3): the state feedback between two reconciles. Untimed (sp.timed == 0): "ideal actuators" - every call
 // the reference makes through its providers takes effect, every asynchronous actuator succeeds, and whatever a node
 // is waiting for (jobs, pod readiness, validation) has happened by the next reconcile. One streaming pass, in place:
@@ -1157,6 +1222,16 @@ int ust_launch_splice(long long n, long long n_rm, const long long* rm, long lon
   const long long grid = n / kSpliceTile + 1;  // positions 0..n
   ust_splice_kernel<<<(unsigned)grid, kThreads, 0, (cudaStream_t)stream>>>(n, n_rm, rm, n_ins, ib, ins_hot, ins_flags, ins_rev, ins_ds, hot,
                                                                            flags, rev, ds, next, act, o_hot, o_flags, o_rev, o_ds, o_next, o_act);
+  return (int)cudaGetLastError();
+}
+int ust_launch_reorder(long long n, long long n_runs, const long long* run_off, const long long* run_src, const uint8_t* ins_hot,
+                       const uint32_t* ins_flags, const int32_t* ins_rev, const int32_t* ins_ds, const uint8_t* hot, const uint32_t* flags,
+                       const int32_t* rev, const int32_t* ds, const uint8_t* next, const uint16_t* act, uint8_t* o_hot, uint32_t* o_flags,
+                       int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, void* stream) {
+  const long long grid = n > 0 ? (n + kGatherTile - 1) / kGatherTile : 1;  // one launch also for the empty snapshot
+  ust_reorder_kernel<<<(unsigned)grid, kThreads, 0, (cudaStream_t)stream>>>(n, n_runs, run_off, run_src, ins_hot, ins_flags, ins_rev,
+                                                                            ins_ds, hot, flags, rev, ds, next, act, o_hot, o_flags,
+                                                                            o_rev, o_ds, o_next, o_act);
   return (int)cudaGetLastError();
 }
 int ust_launch_feedback(long long n, uint8_t* hot, uint32_t* flags, int32_t* pod_rev, const int32_t* ds_idx, int n_ds,

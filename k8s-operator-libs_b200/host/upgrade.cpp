@@ -633,7 +633,7 @@ int ClusterUpgradeStateManagerImpl::EvaluateCached(const ust_policy& policy, boo
     const size_t i = (size_t)changed[j];
     st[j] = k.state[i]; fl[j] = k.flags[i]; rv[j] = k.pod_rev[i]; di[j] = k.ds_idx[i];
   }
-  // nodes that joined: their columns from the cache, at the positions the splice gives them
+  // nodes that joined: their columns from the cache, at the positions the splice / reorder gives them
   const Cache::Splice& ps = k.pending;
   const size_t ni = ps.insert_at.size();
   std::vector<uint8_t> ist(ni + 1);
@@ -645,14 +645,20 @@ int ClusterUpgradeStateManagerImpl::EvaluateCached(const ust_policy& policy, boo
   }
   const ust_splice splice = {(int64_t)ps.remove_idx.size(), ps.remove_idx.data(), (int64_t)ni, ps.insert_before.data(),
                              ist.data(), ifl.data(), irv.data(), idi.data()};
+  const ust_reorder reorder = {(int64_t)ps.run_src.size(), ps.run_src.data(), ps.run_len.data(), (int64_t)ni,
+                               ist.data(), ifl.data(), irv.data(), idi.data()};
   const int64_t cap = (int64_t)(n / 4 + 1024);
   std::vector<int64_t> oi((size_t)cap + 1);
   std::vector<uint8_t> on((size_t)cap + 1);
   std::vector<uint16_t> oa((size_t)cap + 1);
   int64_t n_out = 0;
-  int rc = ust_apply_state_delta_splice(handle_, &policy, ps.empty() ? nullptr : &splice, (int64_t)m, ix.data(), st.data(), fl.data(),
-                                        rv.data(), di.data(), (int32_t)k.ds_rev.size(), dsrev.data(), cap, oi.data(), on.data(), oa.data(),
-                                        &n_out, c);
+  int rc = ps.run_src.empty()
+               ? ust_apply_state_delta_splice(handle_, &policy, ps.empty() ? nullptr : &splice, (int64_t)m, ix.data(), st.data(), fl.data(),
+                                              rv.data(), di.data(), (int32_t)k.ds_rev.size(), dsrev.data(), cap, oi.data(), on.data(),
+                                              oa.data(), &n_out, c)
+               : ust_apply_state_delta_reorder(handle_, &policy, &reorder, (int64_t)m, ix.data(), st.data(), fl.data(), rv.data(),
+                                               di.data(), (int32_t)k.ds_rev.size(), dsrev.data(), cap, oi.data(), on.data(), oa.data(),
+                                               &n_out, c);
   if (rc == UST_ERR_CUDA || rc == UST_ERR_INVALID_ARGUMENT || rc == UST_ERR_COMM) return rc;
   if (n_out > cap) {
     // More changed outputs than the arrays hold: nothing was written to them. That is UST_ERR_TRUNCATED, or a
@@ -672,197 +678,211 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
   if (upgradePolicy == nullptr || !upgradePolicy->AutoUpgrade) return std::nullopt;  // upgrade_state.go:179-182
   ust_policy pol;
   flatten_policy(*upgradePolicy, podDeletionStateEnabled_, validationStateEnabled_, opts_.Requestor.UseMaintenanceOperator, &pol);
-  for (int attempt = 0; attempt < 2; attempt++) {
-    Cache& k = cache_;
-    stats_.reconciles += attempt == 0 ? 1 : 0;
-    bool full = !k.valid;
-    for (auto& sl : k.slots) sl.seen = false;
-    // the DaemonSet table: identities are cached by UID, revision hashes are looked up once per DaemonSet per reconcile
-    std::map<const DaemonSet*, int32_t> dsOf;
-    auto dsIndexOf = [&](const DaemonSet* d) -> int32_t {
-      auto it = dsOf.find(d);
-      if (it != dsOf.end()) return it->second;
-      auto ins = k.dsIndexByUID.emplace(d->UID, (int32_t)k.dsIndexByUID.size());
-      const int32_t idx = ins.first->second;
-      if ((size_t)idx >= k.ds_rev.size()) { k.ds_rev.resize((size_t)idx + 1, 0); k.dsHashError.resize((size_t)idx + 1, false); }
-      std::string dsHash;
-      const bool bad = (bool)PodManager->GetDaemonsetControllerRevisionHash(d, &dsHash);
-      k.ds_rev[(size_t)idx] = bad ? 0 : k.intern.emplace(dsHash, (int32_t)k.intern.size() + 1).first->second;
-      k.dsHashError[(size_t)idx] = bad;
-      dsOf.emplace(d, idx);
-      return idx;
+  Cache& k = cache_;
+  stats_.reconciles++;
+  const bool full = !k.valid;
+  for (auto& sl : k.slots) sl.seen = false;
+  // the DaemonSet table: identities are cached by UID, revision hashes are looked up once per DaemonSet per reconcile
+  std::map<const DaemonSet*, int32_t> dsOf;
+  auto dsIndexOf = [&](const DaemonSet* d) -> int32_t {
+    auto it = dsOf.find(d);
+    if (it != dsOf.end()) return it->second;
+    auto ins = k.dsIndexByUID.emplace(d->UID, (int32_t)k.dsIndexByUID.size());
+    const int32_t idx = ins.first->second;
+    if ((size_t)idx >= k.ds_rev.size()) { k.ds_rev.resize((size_t)idx + 1, 0); k.dsHashError.resize((size_t)idx + 1, false); }
+    std::string dsHash;
+    const bool bad = (bool)PodManager->GetDaemonsetControllerRevisionHash(d, &dsHash);
+    k.ds_rev[(size_t)idx] = bad ? 0 : k.intern.emplace(dsHash, (int32_t)k.intern.size() + 1).first->second;
+    k.dsHashError[(size_t)idx] = bad;
+    dsOf.emplace(d, idx);
+    return idx;
+  };
+  std::vector<int64_t> changed;
+  // Slots follow BuildState's list order (NodeUpgradeState::ListIndex), of which every bucket's slice order is a
+  // subsequence; entries without a ListIndex take their position in the bucket walk instead. The slots move to this
+  // reconcile's order: a node the cache has not seen joins at its position, a cached slot no entry names has left, and a
+  // cached node that changed its position moves with its slot (a driver pod re-created under a new name moves its node
+  // in a list sorted by name).
+  std::vector<const NodeUpgradeState*> order;
+  {
+    std::vector<std::pair<int64_t, const NodeUpgradeState*>> listed;
+    bool haveIndex = true;
+    auto collect = [&](const std::vector<NodeUpgradeState*>& v) {
+      for (const NodeUpgradeState* ns : v) { haveIndex = haveIndex && ns->ListIndex >= 0; listed.emplace_back(ns->ListIndex, ns); }
     };
-    std::vector<int64_t> changed;
-    // Slots follow BuildState's list order (NodeUpgradeState::ListIndex), of which every bucket's slice order is a
-    // subsequence: walk the entries in that order and check that the cached slots still increase along it. A node the
-    // cache has not seen joins right after the last cached slot before it; a cached slot no entry names has left.
-    // Entries without a ListIndex take their position in the bucket walk instead.
-    bool orderBroken = false;
-    std::vector<std::pair<int64_t, const NodeUpgradeState*>> joins;  // (insert before old slot, entry), in list order
-    std::vector<char> present(k.slots.size(), 0);
-    {
-      std::vector<std::pair<int64_t, const NodeUpgradeState*>> order;
-      int64_t pos = 0;
-      bool haveIndex = true;
-      auto collect = [&](const std::vector<NodeUpgradeState*>& v) {
-        for (const NodeUpgradeState* ns : v) { haveIndex = haveIndex && ns->ListIndex >= 0; order.emplace_back(ns->ListIndex, ns); pos++; }
-      };
-      for (int code : kPassOrder) {
-        auto it = currentState->NodeStates.find(kStateNames[code]);
-        if (it != currentState->NodeStates.end()) collect(it->second);
-      }
-      for (const auto& kv : currentState->NodeStates) {
-        const int code = StateCodeOfLabel(kv.first);
-        if (code == UST_STATE_OTHER || code == UST_STATE_POST_MAINTENANCE_REQUIRED) collect(kv.second);
-      }
-      if (haveIndex) std::stable_sort(order.begin(), order.end(), [](const auto& x, const auto& y) { return x.first < y.first; });
-      long long lastSlot = -1;
-      for (const auto& o : order) {
-        auto it = k.idOf.find(o.second->Node->Name);
-        if (it == k.idOf.end()) { joins.emplace_back(lastSlot + 1, o.second); continue; }
-        const long long slot = (long long)k.slotOfId[it->second];
-        if (slot < lastSlot) orderBroken = true;
-        present[(size_t)slot] = 1;
-        lastSlot = slot;
-      }
-    }
-    if (orderBroken && attempt == 0) { ResetIncremental(); continue; }  // re-encode in this snapshot's order
-    // The splice: the host arrays move to the new node order (linear), the same change is kept for the device
-    // (Cache::pending). Joined slots start empty and are encoded by the walk below.
-    Cache::Splice sp;
-    for (size_t i = 0; i < k.slots.size(); i++)
-      if (!present[i]) sp.remove_idx.push_back((int64_t)i);
-    std::vector<char> joined;
-    if (!sp.remove_idx.empty() || !joins.empty()) {
-      const size_t nOld = k.slots.size(), nNew = nOld - sp.remove_idx.size() + joins.size();
-      Cache nk;
-      nk.slots.reserve(nNew); nk.state.reserve(nNew); nk.flags.reserve(nNew); nk.pod_rev.reserve(nNew); nk.ds_idx.reserve(nNew);
-      nk.next.reserve(nNew); nk.actions.reserve(nNew); nk.deferredMsg.reserve(nNew);
-      joined.assign(nNew, 0);
-      size_t j = 0;
-      Error dup;
-      for (size_t p = 0; p <= nOld; p++) {
-        for (; j < joins.size() && joins[j].first == (int64_t)p; j++) {
-          const std::string& name = joins[j].second->Node->Name;
-          size_t id = k.slotOfId.size();
-          if (!k.freeIds.empty()) { id = k.freeIds.back(); k.freeIds.pop_back(); } else k.slotOfId.push_back(0);
-          if (!k.idOf.emplace(name, id).second) { dup = Errorf("node " + name + " appears twice in the snapshot"); k.freeIds.push_back(id); continue; }
-          sp.insert_before.push_back((int64_t)p);
-          sp.insert_at.push_back((int64_t)nk.slots.size());
-          joined[nk.slots.size()] = 1;
-          nk.slots.emplace_back();
-          nk.slots.back().name = name;
-          nk.slots.back().id = id;
-          nk.state.push_back(UST_STATE_EXCLUDED); nk.flags.push_back(0); nk.pod_rev.push_back(0); nk.ds_idx.push_back(-1);
-          nk.next.push_back(0); nk.actions.push_back(0); nk.deferredMsg.emplace_back();
-        }
-        if (p == nOld) break;
-        if (!present[p]) {  // the node left: its name and id go, its entries are not carried over
-          k.idOf.erase(k.slots[p].name);
-          k.freeIds.push_back(k.slots[p].id);
-          continue;
-        }
-        nk.slots.push_back(std::move(k.slots[p]));
-        nk.state.push_back(k.state[p]); nk.flags.push_back(k.flags[p]); nk.pod_rev.push_back(k.pod_rev[p]); nk.ds_idx.push_back(k.ds_idx[p]);
-        nk.next.push_back(p < k.next.size() ? k.next[p] : 0); nk.actions.push_back(p < k.actions.size() ? k.actions[p] : 0);
-        nk.deferredMsg.push_back(std::move(k.deferredMsg[p]));
-      }
-      if (dup) { ResetIncremental(); return dup; }
-      k.slots.swap(nk.slots); k.state.swap(nk.state); k.flags.swap(nk.flags); k.pod_rev.swap(nk.pod_rev); k.ds_idx.swap(nk.ds_idx);
-      k.next.swap(nk.next); k.actions.swap(nk.actions); k.deferredMsg.swap(nk.deferredMsg);
-      for (size_t i = 0; i < k.slots.size(); i++) k.slotOfId[k.slots[i].id] = i;
-    }
-    if (!full) {
-      stats_.inserted += (int64_t)sp.insert_at.size();
-      stats_.removed += (int64_t)sp.remove_idx.size();
-    }
-    k.pending = full ? Cache::Splice() : std::move(sp);
-    stats_.slots = (int64_t)k.slots.size();
-    // this reconcile's view in pass order (what Replay walks): entry, its slot
-    EncodedSnapshot view;
-    view.policy = pol;
-    std::vector<size_t> slotOfView;
-    auto visit = [&](NodeUpgradeState* ns, int code) -> Error {
-      const Node& n = *ns->Node;
-      const size_t i = k.slotOfId[k.idOf.at(n.Name)];
-      Cache::Slot& sl = k.slots[i];
-      if (sl.seen) return Errorf("node " + n.Name + " appears twice in the snapshot");
-      sl.seen = true;
-      int32_t ds = -1;
-      bool dsErr = false;
-      if (!ns->IsOrphanedPod()) { ds = dsIndexOf(ns->DriverDaemonSet); dsErr = k.dsHashError[(size_t)ds]; }
-      // everything the encoding of the entry depends on
-      const bool versioned = !n.ResourceVersion.empty() && (ns->DriverPod == nullptr || !ns->DriverPod->ResourceVersion.empty());
-      std::string sig = std::to_string(code) + "|" + n.ResourceVersion + "|" + (ns->DriverPod ? ns->DriverPod->ResourceVersion : "-") + "|" +
-                        std::to_string(ds) + (dsErr ? "!" : "") + "|" + std::to_string(ds >= 0 ? k.ds_rev[(size_t)ds] : 0) + "|" +
-                        (ns->NodeMaintenance ? (ns->NodeMaintenance->ReadyConditionWithReasonReady ? "R" : "P") : "-");
-      if (!versioned || sig != sl.sig || sl.code != code) {
-        uint8_t hot; uint32_t f; int32_t rev; std::string deferred;
-        if (Error err = encodeOne(ns, code, ds, dsErr, &k.intern, k.ds_rev, &hot, &f, &rev, &deferred)) return err;
-        stats_.encoded++;
-        if (hot != k.state[i] || f != k.flags[i] || rev != k.pod_rev[i] || ds != k.ds_idx[i]) {
-          k.state[i] = hot; k.flags[i] = f; k.pod_rev[i] = rev; k.ds_idx[i] = ds;
-          if (joined.empty() || !joined[i]) changed.push_back((int64_t)i);  // a joined node travels with the splice
-        }
-        k.deferredMsg[i] = deferred;
-        sl.sig = versioned ? sig : std::string();
-        sl.code = code;
-      } else {
-        stats_.reused++;
-      }
-      if (!slotOfView.empty() && (int)(view.state.back() & UST_HOT_STATE_MASK) == code && slotOfView.back() > i)
-        orderBroken = true;  // within a bucket, slot order must be the slice order: slots are handed out in it
-                             // (upgrade_inplace.go:71) and the first error in it ends the pass
-      view.entries.push_back(ns);
-      view.state.push_back(k.state[i]);
-      slotOfView.push_back(i);
-      return std::nullopt;
-    };
-    Error walkErr;
     for (int code : kPassOrder) {
       auto it = currentState->NodeStates.find(kStateNames[code]);
-      if (it == currentState->NodeStates.end()) continue;
-      for (NodeUpgradeState* ns : it->second)
+      if (it != currentState->NodeStates.end()) collect(it->second);
+    }
+    for (const auto& kv : currentState->NodeStates) {
+      const int code = StateCodeOfLabel(kv.first);
+      if (code == UST_STATE_OTHER || code == UST_STATE_POST_MAINTENANCE_REQUIRED) collect(kv.second);
+    }
+    if (haveIndex) std::stable_sort(listed.begin(), listed.end(), [](const auto& x, const auto& y) { return x.first < y.first; });
+    order.reserve(listed.size());
+    for (const auto& l : listed) order.push_back(l.second);
+  }
+  // The new slot order: per position the old slot it takes, or -1 for a node that joins. The same change is kept for the
+  // device (Cache::pending): a splice while the surviving slots keep their relative order, else runs of a reorder.
+  const size_t nOld = k.slots.size();
+  std::vector<int64_t> from;
+  from.reserve(order.size());
+  std::vector<char> present(nOld, 0);
+  Cache::Splice sp;
+  bool moved = false;
+  long long lastSlot = -1;
+  for (const NodeUpgradeState* ns : order) {
+    auto it = k.idOf.find(ns->Node->Name);
+    if (it == k.idOf.end()) {  // joins right after the last cached slot before it
+      sp.insert_before.push_back(lastSlot + 1);
+      sp.insert_at.push_back((int64_t)from.size());
+      from.push_back(-1);
+      continue;
+    }
+    const size_t slot = k.slotOfId[it->second];
+    if (present[slot]) { ResetIncremental(); return Errorf("node " + ns->Node->Name + " appears twice in the snapshot"); }
+    present[slot] = 1;
+    moved = moved || (long long)slot < lastSlot;
+    lastSlot = (long long)slot;
+    from.push_back((int64_t)slot);
+  }
+  for (size_t i = 0; i < nOld; i++)
+    if (!present[i]) sp.remove_idx.push_back((int64_t)i);
+  if (moved) {  // maximal runs of consecutive old slots, joins as inserted runs
+    sp.insert_before.clear();
+    for (size_t p = 0; p < from.size(); p++) {
+      const bool cont = p > 0 && ((from[p] < 0 && from[p - 1] < 0) || (from[p] >= 0 && from[p - 1] >= 0 && from[p] == from[p - 1] + 1));
+      if (cont) { sp.run_len.back()++; continue; }
+      sp.run_src.push_back(from[p] < 0 ? -1 : from[p]);
+      sp.run_len.push_back(1);
+    }
+  }
+  // The host arrays move to the new order (linear). Joined slots start empty and are encoded by the walk below.
+  std::vector<char> joined;
+  if (!sp.empty()) {
+    for (int64_t i : sp.remove_idx) {  // the node left: its name and id go, its entries are not carried over
+      k.idOf.erase(k.slots[(size_t)i].name);
+      k.freeIds.push_back(k.slots[(size_t)i].id);
+    }
+    const size_t nNew = from.size();
+    Cache nk;
+    nk.slots.reserve(nNew); nk.state.reserve(nNew); nk.flags.reserve(nNew); nk.pod_rev.reserve(nNew); nk.ds_idx.reserve(nNew);
+    nk.next.reserve(nNew); nk.actions.reserve(nNew); nk.deferredMsg.reserve(nNew);
+    joined.assign(nNew, 0);
+    for (size_t p = 0; p < nNew; p++) {
+      if (from[p] < 0) {
+        const std::string& name = order[p]->Node->Name;
+        size_t id = k.slotOfId.size();
+        if (!k.freeIds.empty()) { id = k.freeIds.back(); k.freeIds.pop_back(); } else k.slotOfId.push_back(0);
+        if (!k.idOf.emplace(name, id).second) { ResetIncremental(); return Errorf("node " + name + " appears twice in the snapshot"); }
+        joined[p] = 1;
+        nk.slots.emplace_back();
+        nk.slots.back().name = name;
+        nk.slots.back().id = id;
+        nk.state.push_back(UST_STATE_EXCLUDED); nk.flags.push_back(0); nk.pod_rev.push_back(0); nk.ds_idx.push_back(-1);
+        nk.next.push_back(0); nk.actions.push_back(0); nk.deferredMsg.emplace_back();
+        continue;
+      }
+      const size_t q = (size_t)from[p];
+      nk.slots.push_back(std::move(k.slots[q]));
+      nk.state.push_back(k.state[q]); nk.flags.push_back(k.flags[q]); nk.pod_rev.push_back(k.pod_rev[q]); nk.ds_idx.push_back(k.ds_idx[q]);
+      nk.next.push_back(q < k.next.size() ? k.next[q] : 0); nk.actions.push_back(q < k.actions.size() ? k.actions[q] : 0);
+      nk.deferredMsg.push_back(std::move(k.deferredMsg[q]));
+    }
+    k.slots.swap(nk.slots); k.state.swap(nk.state); k.flags.swap(nk.flags); k.pod_rev.swap(nk.pod_rev); k.ds_idx.swap(nk.ds_idx);
+    k.next.swap(nk.next); k.actions.swap(nk.actions); k.deferredMsg.swap(nk.deferredMsg);
+    for (size_t i = 0; i < k.slots.size(); i++) k.slotOfId[k.slots[i].id] = i;
+  }
+  if (!full) {
+    stats_.inserted += (int64_t)sp.insert_at.size();
+    stats_.removed += (int64_t)sp.remove_idx.size();
+    stats_.reorders += moved ? 1 : 0;
+  }
+  k.pending = full ? Cache::Splice() : std::move(sp);
+  stats_.slots = (int64_t)k.slots.size();
+  // this reconcile's view in pass order (what Replay walks): entry, its slot
+  EncodedSnapshot view;
+  view.policy = pol;
+  std::vector<size_t> slotOfView;
+  bool orderBroken = false;
+  auto visit = [&](NodeUpgradeState* ns, int code) -> Error {
+    const Node& n = *ns->Node;
+    const size_t i = k.slotOfId[k.idOf.at(n.Name)];
+    Cache::Slot& sl = k.slots[i];
+    if (sl.seen) return Errorf("node " + n.Name + " appears twice in the snapshot");
+    sl.seen = true;
+    int32_t ds = -1;
+    bool dsErr = false;
+    if (!ns->IsOrphanedPod()) { ds = dsIndexOf(ns->DriverDaemonSet); dsErr = k.dsHashError[(size_t)ds]; }
+    // everything the encoding of the entry depends on
+    const bool versioned = !n.ResourceVersion.empty() && (ns->DriverPod == nullptr || !ns->DriverPod->ResourceVersion.empty());
+    std::string sig = std::to_string(code) + "|" + n.ResourceVersion + "|" + (ns->DriverPod ? ns->DriverPod->ResourceVersion : "-") + "|" +
+                      std::to_string(ds) + (dsErr ? "!" : "") + "|" + std::to_string(ds >= 0 ? k.ds_rev[(size_t)ds] : 0) + "|" +
+                      (ns->NodeMaintenance ? (ns->NodeMaintenance->ReadyConditionWithReasonReady ? "R" : "P") : "-");
+    if (!versioned || sig != sl.sig || sl.code != code) {
+      uint8_t hot; uint32_t f; int32_t rev; std::string deferred;
+      if (Error err = encodeOne(ns, code, ds, dsErr, &k.intern, k.ds_rev, &hot, &f, &rev, &deferred)) return err;
+      stats_.encoded++;
+      if (hot != k.state[i] || f != k.flags[i] || rev != k.pod_rev[i] || ds != k.ds_idx[i]) {
+        k.state[i] = hot; k.flags[i] = f; k.pod_rev[i] = rev; k.ds_idx[i] = ds;
+        if (joined.empty() || !joined[i]) changed.push_back((int64_t)i);  // a joined node travels with the splice / reorder
+      }
+      k.deferredMsg[i] = deferred;
+      sl.sig = versioned ? sig : std::string();
+      sl.code = code;
+    } else {
+      stats_.reused++;
+    }
+    if (!slotOfView.empty() && (int)(view.state.back() & UST_HOT_STATE_MASK) == code && slotOfView.back() > i)
+      orderBroken = true;  // within a bucket, slot order must be the slice order: slots are handed out in it
+                           // (upgrade_inplace.go:71) and the first error in it ends the pass
+    view.entries.push_back(ns);
+    view.state.push_back(k.state[i]);
+    slotOfView.push_back(i);
+    return std::nullopt;
+  };
+  Error walkErr;
+  for (int code : kPassOrder) {
+    auto it = currentState->NodeStates.find(kStateNames[code]);
+    if (it == currentState->NodeStates.end()) continue;
+    for (NodeUpgradeState* ns : it->second)
+      if ((walkErr = visit(ns, code))) break;
+    if (walkErr) break;
+  }
+  if (!walkErr)
+    for (const auto& kv : currentState->NodeStates) {
+      const int code = StateCodeOfLabel(kv.first);
+      if (code != UST_STATE_OTHER && code != UST_STATE_POST_MAINTENANCE_REQUIRED) continue;
+      for (NodeUpgradeState* ns : kv.second)
         if ((walkErr = visit(ns, code))) break;
       if (walkErr) break;
     }
-    if (!walkErr)
-      for (const auto& kv : currentState->NodeStates) {
-        const int code = StateCodeOfLabel(kv.first);
-        if (code != UST_STATE_OTHER && code != UST_STATE_POST_MAINTENANCE_REQUIRED) continue;
-        for (NodeUpgradeState* ns : kv.second)
-          if ((walkErr = visit(ns, code))) break;
-        if (walkErr) break;
-      }
-    if (walkErr) { ResetIncremental(); return walkErr; }
-    if (orderBroken) {  // a bucket's slice order contradicts the cached order (entries without a ListIndex): start over
-      ResetIncremental();
-      if (attempt == 0) continue;
-      return Errorf("incremental ApplyState: a bucket's slice order contradicts the list order");
-    }
-    std::sort(changed.begin(), changed.end());
-    if (full) stats_.full_uploads++;
-    const int rc = EvaluateCached(pol, full, changed, &k, &last_);
-    if (rc == UST_ERR_CUDA || rc == UST_ERR_INVALID_ARGUMENT || rc == UST_ERR_NIL_STATE || rc == UST_ERR_COMM) {
-      ResetIncremental();
-      return Errorf(handle_ ? ust_last_error(handle_) : "no H100 device bound to this manager: ApplyState has no CPU path");
-    }
-    k.valid = true;
-    // Replay walks this reconcile's view: gather its outputs, translate the abort position
-    const size_t nv = view.entries.size();
-    std::vector<uint8_t> next(nv + 1);
-    std::vector<uint16_t> actions(nv + 1);
-    ust_counters c = last_;
-    for (size_t v = 0; v < nv; v++) {
-      const size_t i = slotOfView[v];
-      next[v] = k.next[i];
-      actions[v] = k.actions[i];
-      if (!k.deferredMsg[i].empty()) view.deferred[v] = k.deferredMsg[i];
-      if (last_.error_index == (int64_t)i) c.error_index = (int64_t)v;
-    }
-    return Replay(view, *upgradePolicy, next.data(), actions.data(), rc, c);
+  if (walkErr) { ResetIncremental(); return walkErr; }
+  if (orderBroken) {  // the slots follow the list order: a bucket whose slice order contradicts it is inconsistent input
+    ResetIncremental();
+    return Errorf("incremental ApplyState: a bucket's slice order contradicts the list order");
   }
-  return Errorf("incremental ApplyState could not settle on a node order");
+  std::sort(changed.begin(), changed.end());
+  if (full) stats_.full_uploads++;
+  const int rc = EvaluateCached(pol, full, changed, &k, &last_);
+  if (rc == UST_ERR_CUDA || rc == UST_ERR_INVALID_ARGUMENT || rc == UST_ERR_NIL_STATE || rc == UST_ERR_COMM) {
+    ResetIncremental();
+    return Errorf(handle_ ? ust_last_error(handle_) : "no H100 device bound to this manager: ApplyState has no CPU path");
+  }
+  k.valid = true;
+  // Replay walks this reconcile's view: gather its outputs, translate the abort position
+  const size_t nv = view.entries.size();
+  std::vector<uint8_t> next(nv + 1);
+  std::vector<uint16_t> actions(nv + 1);
+  ust_counters c = last_;
+  for (size_t v = 0; v < nv; v++) {
+    const size_t i = slotOfView[v];
+    next[v] = k.next[i];
+    actions[v] = k.actions[i];
+    if (!k.deferredMsg[i].empty()) view.deferred[v] = k.deferredMsg[i];
+    if (last_.error_index == (int64_t)i) c.error_index = (int64_t)v;
+  }
+  return Replay(view, *upgradePolicy, next.data(), actions.data(), rc, c);
 }
 
 }  // namespace upgrade

@@ -284,14 +284,17 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
   // (upgrade_state.go:140-161, common_manager.go:229-604); the provider calls skipped for an unchanged object are
   // GetPodControllerRevisionHash and IsWaitingForSafeDriverLoad, both pure functions of the object in the reference's
   // own implementations (pod_manager.go:84-89, safe_driver_load_manager.go:51-53).
-  // Nodes that join the cluster are inserted at their list position among the cached slots and encoded on their own;
-  // nodes that leave are removed with their slot. Both travel to the device as one splice of the resident snapshot
-  // (ust_apply_state_delta_splice). Falls back to a full encode + upload on the first call and when the surviving nodes'
-  // list order no longer follows the cached order (slots are handed out in slice order, upgrade_inplace.go:71).
+  // The cached slots follow the list order (slots are handed out in slice order, upgrade_inplace.go:71). Nodes that join
+  // the cluster are inserted at their list position and encoded on their own; nodes that leave are removed with their
+  // slot; nodes that move in the list (a driver pod re-created under a new name, DaemonSets listed in another order)
+  // move with their slot and are not re-encoded. Joins and leaves alone travel to the device as one splice of the
+  // resident snapshot (ust_apply_state_delta_splice); with moves, as one reorder (ust_apply_state_delta_reorder). A full
+  // encode + upload happens on the first call only.
   Error ApplyStateIncremental(ClusterUpgradeState* currentState, const DriverUpgradePolicySpec* upgradePolicy);
   struct IncrementalStats {
     int64_t reconciles = 0, full_uploads = 0, encoded = 0, reused = 0, outputs_received = 0;
-    int64_t inserted = 0, removed = 0;  // nodes that joined / left the cached snapshot by a splice
+    int64_t inserted = 0, removed = 0;  // nodes that joined / left the cached snapshot by a splice or reorder
+    int64_t reorders = 0;               // reconciles that went to the device as a reorder (a surviving node moved)
     int64_t slots = 0;                  // size of the cached snapshot after the last reconcile
   };
   const IncrementalStats& Stats() const { return stats_; }
@@ -309,12 +312,15 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
     std::unordered_map<std::string, size_t> idOf;
     std::vector<size_t> slotOfId;
     std::vector<size_t> freeIds;
-    // The membership change the host arrays went through since the device last saw them, in the terms of ust_splice
-    // (indices into the previous snapshot); insert_at[k] is the new index of inserted node k, whose columns are
-    // state[insert_at[k]] etc. Empty after a full upload.
+    // The change of node order the host arrays went through since the device last saw them (indices into the previous
+    // snapshot): remove_idx are the slots that left; insert_at[k] is the new index of inserted node k, whose columns are
+    // state[insert_at[k]] etc. While the surviving slots keep their order it is a ust_splice (insert_before); when one
+    // of them moved, the new order as ust_reorder runs (run_src / run_len) instead, and insert_before is empty.
+    // Empty after a full upload.
     struct Splice {
       std::vector<int64_t> remove_idx, insert_before, insert_at;
-      bool empty() const { return remove_idx.empty() && insert_before.empty(); }
+      std::vector<int64_t> run_src, run_len;
+      bool empty() const { return remove_idx.empty() && insert_before.empty() && run_src.empty(); }
     };
     Splice pending;
     std::vector<Slot> slots;

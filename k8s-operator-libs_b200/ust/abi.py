@@ -93,6 +93,12 @@ class Splice(C.Structure):
                 ("state", C.c_void_p), ("flags", C.c_void_p), ("pod_rev", C.c_void_p), ("ds_idx", C.c_void_p)]
 
 
+class Reorder(C.Structure):
+    """ust_reorder: a new node order of the resident snapshot as runs of old and inserted nodes (raw host addresses)."""
+    _fields_ = [("n_runs", C.c_int64), ("run_src", C.c_void_p), ("run_len", C.c_void_p), ("n_insert", C.c_int64),
+                ("state", C.c_void_p), ("flags", C.c_void_p), ("pod_rev", C.c_void_p), ("ds_idx", C.c_void_p)]
+
+
 def make_policy(auto_upgrade=True, max_parallel_upgrades=0, max_unavailable=None, pod_deletion_enabled=False,
                 validation_enabled=False, pod_deletion=None, drain=None, wait_for_completion=None,
                 use_maintenance_operator=False, evaluate_actuators=False):
