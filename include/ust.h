@@ -361,6 +361,50 @@ int ust_apply_state_delta_reorder(ust_handle* h, const ust_policy* policy, const
 /* The full outputs of the last call on the resident snapshot (n_nodes entries each). */
 int ust_fetch_outputs(ust_handle* h, uint8_t* next_state, uint16_t* actions);
 
+/* Replacement workload pod lists for some nodes of the resident pod-list snapshot of n nodes:
+ *   node_idx[n_lists]     strictly increasing, each in [0, n)
+ *   pod_off[n_lists + 1]  list k is pod_flags[pod_off[k] .. pod_off[k+1]); pod_off[0] == 0, non-decreasing,
+ *                         pod_off[n_lists] == n_pods (lists may be empty, or shorter or longer than before)
+ *   pod_flags[n_pods]     UST_POD_* bits as in ust_pods */
+typedef struct ust_pod_lists {
+  int64_t n_lists;
+  const int64_t* node_idx;
+  const int32_t* pod_off;
+  const uint16_t* pod_flags;
+  int64_t n_pods;
+} ust_pod_lists;
+
+/* Delta form of ust_apply_state with pod lists (actuator evaluation, evaluate_actuators): the pod lists stay resident
+ * too, and a reconcile sends only the lists that changed (a pod changed phase, a job pod appeared or finished).
+ * The resident pod-list snapshot is left by
+ *   - a ust_apply_state call with pods != NULL and actuator_outcome != NULL that produced counters (a reference-level
+ *     abort counts),
+ *   - a ust_apply_state_delta_pods call that produced counters (UST_ERR_TRUNCATED counts).
+ * Only ust_apply_state_delta_pods and ust_fetch_outputs_pods use it: after a call with pod lists, ust_apply_state_delta,
+ * _sparse, _splice, _reorder, ust_fetch_outputs and the simulations find nothing resident, as before. Every call that
+ * drops the resident snapshot drops the pod-list snapshot too: ust_apply_state without pods, _packed, both BuildStates,
+ * the simulations, the node delta calls and any call that fails once its arguments were accepted.
+ * ust_apply_state_device leaves it alone.
+ * One call (1) replaces the lists of lists->node_idx (every other node keeps its list), (2) applies the n_changed node
+ * overwrites exactly as ust_apply_state_delta, (3) evaluates the whole snapshot with its pod lists. Sparse outputs in node
+ * order: out_idx[k], out_next_state[k], out_actions[k], out_outcome[k] for k < *n_out, for every node whose next_state,
+ * actions or actuator_outcome differs from what the previous call returned for it (out_outcome is required when
+ * max_out > 0). Counters, aborts and error codes are those of ust_apply_state with pods on the updated arrays;
+ * UST_ERR_TRUNCATED works as in ust_apply_state_delta_sparse (a reference-level abort keeps its own code), and
+ * ust_fetch_outputs_pods then returns the full outputs. lists == NULL or n_lists == 0: no list changes.
+ * A violated contract (node_idx unsorted, duplicated or out of range, malformed replacement offsets, a new pod total of
+ * 2^31 or more, NULL arrays, idx outside the snapshot, no resident pod-list snapshot, more than one rank set up by
+ * ust_comm_init) returns UST_ERR_INVALID_ARGUMENT before any device work: the resident snapshot stays as it was. The
+ * checks cost O(n_lists + n_pods + n_changed) host time. When every replaced list keeps its length the new lists are
+ * copied in place; otherwise the resident CSR is laid out anew on the device in one pass. */
+int ust_apply_state_delta_pods(ust_handle* h, const ust_policy* policy, const ust_pod_lists* lists /* nullable */,
+                               int64_t n_changed, const int64_t* idx, const uint8_t* state, const uint32_t* flags,
+                               const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev,
+                               int64_t max_out, int64_t* out_idx, uint8_t* out_next_state, uint16_t* out_actions,
+                               uint8_t* out_outcome, int64_t* n_out, ust_counters* out);
+/* The full outputs of the last call on the resident pod-list snapshot (n_nodes entries each). */
+int ust_fetch_outputs_pods(ust_handle* h, uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome);
+
 /* Rollout simulation (SURVEY 8f.3) on the resident snapshot (see ust_apply_state_delta): `steps` reconciles in a row,
  * entirely on the device. After each ApplyState the decisions are fed back into the snapshot under "ideal
  * actuators": every provider call takes effect (state label, annotations, cordon / uncordon), every scheduled

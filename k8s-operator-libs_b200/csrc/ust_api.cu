@@ -155,6 +155,10 @@ struct ust_handle {
   int64_t resident_n = -1;  // nodes of the snapshot the last ust_apply_state left in the staging arrays (-1 = none)
   int32_t resident_n_ds = 0;  // ... and the size of its DaemonSet table
   bool outputs_resident = false;  // `outs` holds the outputs of the last call on the resident snapshot
+  // the resident pod-list snapshot (ust_apply_state_delta_pods): nodes in `staged`, pod lists in s_podoff / s_podflags,
+  // outputs in `outs` and s_outcome. Only the pod-list entry points see it.
+  int64_t pods_n = -1;      // its nodes (-1 = none)
+  int64_t pods_total = 0;   // its pods
   DevBuf<ust_counters> sim_hist;  // rollout simulation: one ust_counters per simulated reconcile
   int segments = 6;      // upload / compute / download pipeline depth of the host path (UST_SEGMENTS, tuning)
   bool no_hint = false;  // UST_NO_HINT=1 (tuning): every call speculates from the policy default, never from the previous call
@@ -174,7 +178,7 @@ struct ust_handle {
   // staging for the host-pointer API; `staged` and `outs` hold the resident snapshot and its outputs
   Columns staged;
   Outputs outs;
-  DevBuf<uint8_t> s_outcome;
+  DevBuf<uint8_t> s_outcome, s_outcome_prev;  // actuator_outcome; the previous call's (pod-list deltas: swapped like outs / outs_prev)
   DevBuf<int32_t> s_dsrev, s_podoff, s_dsdesired;
   DevBuf<uint16_t> s_rev16;          // packed host format: interned pod revisions / DaemonSet indices as uploaded
   DevBuf<int8_t> s_ds8;
@@ -191,6 +195,15 @@ struct ust_handle {
   DevBuf<uint64_t> s_uid, s_dsuid;   // BuildState owner join: pod owner UIDs, DaemonSet UID hash table (+ s_dsorder: slot -> index)
   DevBuf<int32_t> s_dsorder;
   IndexedColumns changed;            // delta updates: indices and values of the changed nodes
+  // pod-list deltas: the replaced lists as uploaded (node indices, offsets, pods, length-change prefix), the run table of a
+  // relayout, the second CSR pair a relayout writes (swapped with s_podoff / s_podflags; allocated on the first relayout),
+  // the sparse outcomes; on the host the list length of every node of the pod-list snapshot, and the lengths the
+  // checks of a pod-list ust_apply_state fill (swapped in when that call leaves its snapshot resident)
+  DevBuf<long long> pl_idx;
+  DevBuf<int32_t> pl_off, pl_shift, pl_runs, s_podoff2;
+  DevBuf<uint16_t> pl_flags, s_podflags2;
+  DevBuf<uint8_t> sp_outcome;
+  std::vector<int32_t> pod_len, pod_len_next, pl_shift_host;
   // new node order (splice, reorder): the second set the splice / gather kernel writes (swapped with the resident columns
   // and the previous outputs afterwards; allocated on the first such call), the removal list, the reorder's runs
   // (run_off, then run_src: see add_run) and the inserted nodes with their positions (splice); run_seen: one bit per old
@@ -396,11 +409,14 @@ static int launch_verify(ust_handle* h, UstParams& P, cudaStream_t st, bool pdl)
 }
 
 // The pod CSR must be well-formed before a kernel walks it: pod_off[0] == 0, non-decreasing, pod_off[n] == n_pods.
-static int check_pod_offsets_host(ust_handle* h, int64_t n, const int32_t* pod_off, int64_t n_pods) {
+// `lens` (nullable, n entries) receives the list lengths on the way.
+static int check_pod_offsets_host(ust_handle* h, int64_t n, const int32_t* pod_off, int64_t n_pods, int32_t* lens = nullptr) {
   if (n == 0) return UST_OK;
   if (pod_off[0] != 0) return h->fail(UST_ERR_INVALID_ARGUMENT, "pod_off[0] must be 0");
-  for (int64_t i = 0; i < n; i++)
+  for (int64_t i = 0; i < n; i++) {
     if (pod_off[i + 1] < pod_off[i]) return h->fail(UST_ERR_INVALID_ARGUMENT, "pod_off must not decrease (node %lld)", (long long)i);
+    if (lens) lens[i] = pod_off[i + 1] - pod_off[i];
+  }
   if ((int64_t)pod_off[n] != n_pods) return h->fail(UST_ERR_INVALID_ARGUMENT, "pod_off[n_nodes] must equal n_pods");
   return UST_OK;
 }
@@ -553,12 +569,20 @@ static int widen_nodes(ust_handle* h, size_t first, size_t count, cudaStream_t s
 static void drop_resident(ust_handle* h) {
   h->resident_n = -1;
   h->outputs_resident = false;
+  h->pods_n = -1;
 }
 
 // The snapshot in `staged` stays resident after a call that produced counters (a reference-level abort and
 // UST_ERR_TRUNCATED included), with the call's outputs unless `outputs` is false. A call that failed keeps nothing.
-static int adopt_resident(ust_handle* h, int rc, int64_t n, int32_t n_ds, bool outputs = true) {
+// n_pods >= 0: the call evaluated pod lists of that many pods and their actuator outcomes; its snapshot is the pod-list
+// snapshot, which only ust_apply_state_delta_pods and ust_fetch_outputs_pods use.
+static int adopt_resident(ust_handle* h, int rc, int64_t n, int32_t n_ds, bool outputs = true, int64_t n_pods = -1) {
   if (rc != UST_ERR_CUDA && rc != UST_ERR_INVALID_ARGUMENT && rc != UST_ERR_COMM && rc != UST_ERR_NIL_STATE) {
+    if (n_pods >= 0) {
+      h->pods_n = n;
+      h->pods_total = n_pods;
+      return rc;
+    }
     h->resident_n = n;
     h->resident_n_ds = n_ds;
     h->outputs_resident = outputs;
@@ -639,7 +663,9 @@ static int apply_pipelined(ust_handle* h, const ust_policy* policy, int64_t n, c
 }
 
 // ust_apply_state and ust_apply_state_packed after their argument checks: upload, evaluate, download. Snapshots of
-// 2^19 nodes or more take the pipelined path unless they come with pod lists; a call with pod lists is never resident.
+// 2^19 nodes or more take the pipelined path unless they come with pod lists. A call with pod lists and actuator_outcome
+// leaves the pod-list snapshot (its list lengths are in h->pod_len_next, filled by the offset check); one with pod lists
+// but no outcome leaves nothing resident.
 static int apply_host(ust_handle* h, const ust_policy* policy, int64_t n, const HostNodes& in, int32_t n_ds,
                       const int32_t* ds_rev, const ust_pods* pods, uint8_t* next_state, uint16_t* actions,
                       uint8_t* outcome, ust_counters* out) {
@@ -683,7 +709,10 @@ static int apply_host(ust_handle* h, const ust_policy* policy, int64_t n, const 
     if (outcome) UST_CUDA(h, cudaMemcpyAsync(outcome, h->s_outcome.p, N, cudaMemcpyDeviceToHost, st));
   }
   rc = finish_with_counters(h, st, out);
-  return pods ? rc : adopt_resident(h, rc, n, n_ds);
+  if (!pods) return adopt_resident(h, rc, n, n_ds);
+  if (!outcome) return rc;
+  std::swap(h->pod_len, h->pod_len_next);
+  return adopt_resident(h, rc, n, n_ds, true, pods->n_pods);
 }
 
 // The launch of ust_build_state / _uids once their inputs are enqueued: `launch(grid)` starts the counting kernel and
@@ -855,7 +884,16 @@ int ust_apply_state(ust_handle* h, const ust_policy* policy, int64_t n, const ui
   if (n_ds < 0 || (n_ds > 0 && !ds_rev)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad DaemonSet table");
   if (pods && (!pods->pod_off || pods->n_pods < 0 || (pods->n_pods > 0 && !pods->pod_flags)))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad pod lists");
-  if (pods) { int prc = check_pod_offsets_host(h, n, pods->pod_off, pods->n_pods); if (prc) return prc; }
+  if (pods) {
+    // a call that may leave the pod-list snapshot notes its list lengths for the checks of ust_apply_state_delta_pods
+    int32_t* lens = nullptr;
+    if (actuator_outcome) {
+      h->pod_len_next.resize((size_t)n);
+      lens = h->pod_len_next.data();
+    }
+    int prc = check_pod_offsets_host(h, n, pods->pod_off, pods->n_pods, lens);
+    if (prc) return prc;
+  }
   return apply_host(h, policy, n, HostNodes{state, flags, pod_rev, ds_idx, nullptr, nullptr}, n_ds, ds_rev, pods, next_state,
                     actions, actuator_outcome, out);
 }
@@ -931,16 +969,20 @@ static int reorder_runs(ust_handle* h, const ust_reorder* ro, int64_t n_old, int
   return rc;
 }
 
-// ust_apply_state_delta, _delta_sparse, _delta_splice and _delta_reorder: bring the resident snapshot into a new node
-// order (optional: nodes leave, join and move), scatter the re-encoded nodes into it, evaluate everything, return all
-// outputs (dense) or the outputs that differ from the previous call's (sparse).
-static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splice* sp, const ust_reorder* ro, int64_t n_changed,
-                        const int64_t* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx,
-                        int32_t n_ds, const int32_t* ds_rev, bool sparse, uint8_t* next_state, uint16_t* actions,
-                        uint8_t* actuator_outcome, int64_t max_out, int64_t* out_idx, int64_t* n_out, ust_counters* out) {
-  const int64_t n_old = h->resident_n;
+// ust_apply_state_delta, _delta_sparse, _delta_splice, _delta_reorder and _delta_pods: bring the resident snapshot into a
+// new node order (optional: nodes leave, join and move), scatter the re-encoded nodes into it, evaluate everything, return
+// all outputs (dense) or the outputs that differ from the previous call's (sparse). `pods`: the pod-list snapshot, whose
+// lists `pl` (nullable) replaces first; its sparse outputs include actuator_outcome (written to `actuator_outcome`).
+static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splice* sp, const ust_reorder* ro, bool pods,
+                        const ust_pod_lists* pl, int64_t n_changed, const int64_t* idx, const uint8_t* state, const uint32_t* flags,
+                        const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, bool sparse,
+                        uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome, int64_t max_out, int64_t* out_idx,
+                        int64_t* n_out, ust_counters* out) {
+  const int64_t n_old = pods ? h->pods_n : h->resident_n;
+  if (n_old < 0 && pods)
+    return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident pod-list snapshot: call ust_apply_state with pod lists and actuator_outcome first");
   if (n_old < 0) return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident snapshot: call ust_apply_state (without pod lists) first");
-  if (sparse && !h->outputs_resident)
+  if (sparse && !pods && !h->outputs_resident)
     return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident outputs to compare with: the previous call must be an ApplyState on this snapshot");
   // the new node order, checked in full before anything is touched
   int64_t n = n_old, n_ins = 0;
@@ -977,11 +1019,36 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
   if (n_changed < 0 || (n_changed > 0 && (!idx || !state || !flags || !pod_rev || !ds_idx)))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
   if (!sparse && n > 0 && (!next_state || !actions)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
-  if (sparse && (max_out < 0 || !n_out || (max_out > 0 && (!out_idx || !next_state || !actions))))
+  if (sparse && (max_out < 0 || !n_out || (max_out > 0 && (!out_idx || !next_state || !actions || (pods && !actuator_outcome)))))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
   if (n_ds < 0 || (n_ds > 0 && !ds_rev)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad DaemonSet table");
   for (int64_t k = 0; k < n_changed; k++)
     if (idx[k] < 0 || idx[k] >= n) return h->fail(UST_ERR_INVALID_ARGUMENT, "changed node %lld has index %lld outside the snapshot of %lld nodes", (long long)k, (long long)idx[k], (long long)n);
+  // replacement pod lists, checked in O(n_lists + n_pods) against the host copy of the resident list lengths; with every
+  // length kept they are copied in place, otherwise the CSR is laid out anew (pl_shift_host: prefix of the length changes)
+  const int64_t L = pods && pl ? pl->n_lists : 0;
+  int64_t new_total = pods ? h->pods_total : 0;
+  bool same_len = true;
+  if (L != 0) {
+    if (L < 0 || !pl->node_idx || !pl->pod_off || pl->n_pods < 0 || (pl->n_pods > 0 && !pl->pod_flags))
+      return h->fail(UST_ERR_INVALID_ARGUMENT, "bad pod lists");
+    for (int64_t k = 0; k < L; k++)
+      if (pl->node_idx[k] < (k ? pl->node_idx[k - 1] + 1 : 0) || pl->node_idx[k] >= n)
+        return h->fail(UST_ERR_INVALID_ARGUMENT, "pod lists: node_idx[%lld] = %lld is not strictly increasing in [0, %lld)", (long long)k,
+                       (long long)pl->node_idx[k], (long long)n);
+    if (int rc = check_pod_offsets_host(h, L, pl->pod_off, pl->n_pods)) return rc;
+    h->pl_shift_host.resize((size_t)L + 1);
+    int64_t d = 0;
+    for (int64_t k = 0; k < L; k++) {
+      h->pl_shift_host[(size_t)k] = (int32_t)d;  // |d| stays below 2^31 when the new total does (checked below)
+      const int32_t len = pl->pod_off[k + 1] - pl->pod_off[k];
+      same_len = same_len && len == h->pod_len[(size_t)pl->node_idx[k]];
+      d += (int64_t)len - h->pod_len[(size_t)pl->node_idx[k]];
+    }
+    h->pl_shift_host[(size_t)L] = (int32_t)d;
+    new_total += d;
+    if (new_total >= (1LL << 31)) return h->fail(UST_ERR_INVALID_ARGUMENT, "pod lists: %lld pods in all, pod_off is int32", (long long)new_total);
+  }
   UST_CUDA(h, cudaSetDevice(h->device));
   StreamDrain drain(h);
   cudaStream_t st = h->stream;
@@ -996,7 +1063,22 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
     UST_CUDA(h, h->inserted.cols.reserve(I));
   }
   UST_CUDA(h, h->s_dsrev.reserve((size_t)n_ds + 1));
-  if (actuator_outcome) UST_CUDA(h, h->s_outcome.reserve(N + 16));
+  if (actuator_outcome || pods) UST_CUDA(h, h->s_outcome.reserve(N + 16));
+  if (pods && sparse) {
+    UST_CUDA(h, h->s_outcome_prev.reserve(N + 16));
+    UST_CUDA(h, h->sp_outcome.reserve((size_t)max_out + 1));
+  }
+  if (L) {  // the new lists carry 8 pods of padding for the relayout's 16-byte loads, the new CSR too
+    UST_CUDA(h, h->pl_idx.reserve((size_t)L));
+    UST_CUDA(h, h->pl_off.reserve((size_t)L + 1));
+    UST_CUDA(h, h->pl_flags.reserve((size_t)pl->n_pods + 16));
+    if (!same_len) {
+      UST_CUDA(h, h->pl_shift.reserve((size_t)L + 1));
+      UST_CUDA(h, h->pl_runs.reserve(4 * (size_t)L + 3));
+      UST_CUDA(h, h->s_podoff2.reserve(N + 1));
+      UST_CUDA(h, h->s_podflags2.reserve((size_t)new_total + 16));
+    }
+  }
   UST_CUDA(h, h->changed.idx.reserve(M + 1));
   UST_CUDA(h, h->changed.cols.reserve(M));
   if (sparse) {  // the pair this call writes holds the new size as well
@@ -1006,7 +1088,26 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
     UST_CUDA(h, h->outs_sparse.reserve((size_t)max_out));
   }
   drop_resident(h);  // until the patched snapshot has been evaluated
+  for (int64_t k = 0; k < L; k++) h->pod_len[(size_t)pl->node_idx[k]] = pl->pod_off[k + 1] - pl->pod_off[k];
   if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsrev.p, ds_rev, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
+  if (L) {
+    UST_CUDA(h, cudaMemcpyAsync(h->pl_idx.p, pl->node_idx, (size_t)L * 8, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, cudaMemcpyAsync(h->pl_off.p, pl->pod_off, ((size_t)L + 1) * 4, cudaMemcpyHostToDevice, st));
+    if (pl->n_pods) UST_CUDA(h, cudaMemcpyAsync(h->pl_flags.p, pl->pod_flags, (size_t)pl->n_pods * 2, cudaMemcpyHostToDevice, st));
+    int e;
+    if (same_len) {
+      e = ust_launch_pods_scatter((long long)L, h->pl_idx.p, h->pl_off.p, h->pl_flags.p, h->s_podoff.p, h->s_podflags.p, 8 * h->num_sms, st);
+      h->launches += 1;
+    } else {
+      UST_CUDA(h, cudaMemcpyAsync(h->pl_shift.p, h->pl_shift_host.data(), ((size_t)L + 1) * 4, cudaMemcpyHostToDevice, st));
+      e = ust_launch_pods_relayout((long long)n, (long long)L, h->pl_idx.p, h->pl_off.p, h->pl_shift.p, h->s_podoff.p, h->s_podflags.p,
+                                   h->pl_flags.p, (int)new_total, h->pl_runs.p, h->s_podoff2.p, h->s_podflags2.p, 8 * h->num_sms, st);
+      h->launches += 2;
+      std::swap(h->s_podoff, h->s_podoff2);
+      std::swap(h->s_podflags, h->s_podflags2);
+    }
+    if (e) return h->fail(UST_ERR_CUDA, "pod-list kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+  }
   if (gather) {
     UST_CUDA(h, h->inserted.cols.upload(ins_state, ins_flags, ins_rev, ins_ds, 0, I, st));
     const Columns &in = h->inserted.cols, &s = h->staged, &x = h->splice_cols;
@@ -1045,9 +1146,10 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
     h->launches += 1;
   }
   if (sparse) std::swap(h->outs, h->outs_prev);  // the previous call's outputs step aside; this call writes the other pair
+  if (sparse && pods) std::swap(h->s_outcome, h->s_outcome_prev);
   int rc = apply_device(h, policy, n, h->staged.hot.p, h->staged.flags.p, h->staged.rev.p, h->staged.ds.p, n_ds, h->s_dsrev.p,
-                        nullptr, nullptr, 0, h->outs.next.p, h->outs.actions.p, actuator_outcome ? h->s_outcome.p : nullptr,
-                        nullptr, st);
+                        pods ? h->s_podoff.p : nullptr, pods ? h->s_podflags.p : nullptr, pods ? new_total : 0, h->outs.next.p,
+                        h->outs.actions.p, actuator_outcome || pods ? h->s_outcome.p : nullptr, nullptr, st);
   if (rc) return rc;
   if (!sparse) {
     if (N) {
@@ -1056,9 +1158,10 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
       if (actuator_outcome) UST_CUDA(h, cudaMemcpyAsync(actuator_outcome, h->s_outcome.p, N, cudaMemcpyDeviceToHost, st));
     }
   } else {
-    int e = ust_launch_diff((long long)n, h->outs.next.p, h->outs.actions.p, h->outs_prev.next.p, h->outs_prev.actions.p,
-                            h->sp_blocks.p, h->sp_count_dev, (long long)max_out, h->sp_idx.p, h->outs_sparse.next.p,
-                            h->outs_sparse.actions.p, st);
+    int e = ust_launch_diff((long long)n, h->outs.next.p, h->outs.actions.p, pods ? h->s_outcome.p : nullptr, h->outs_prev.next.p,
+                            h->outs_prev.actions.p, pods ? h->s_outcome_prev.p : nullptr, h->sp_blocks.p, h->sp_count_dev,
+                            (long long)max_out, h->sp_idx.p, h->outs_sparse.next.p, h->outs_sparse.actions.p,
+                            pods ? h->sp_outcome.p : nullptr, st);
     if (e) return h->fail(UST_ERR_CUDA, "diff kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 3;
     UST_CUDA(h, cudaMemcpyAsync(h->sp_count_host, h->sp_count_dev, sizeof(long long), cudaMemcpyDeviceToHost, st));
@@ -1069,11 +1172,13 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
       UST_CUDA(h, cudaMemcpyAsync(out_idx, h->sp_idx.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, st));
       UST_CUDA(h, cudaMemcpyAsync(next_state, h->outs_sparse.next.p, (size_t)cnt, cudaMemcpyDeviceToHost, st));
       UST_CUDA(h, cudaMemcpyAsync(actions, h->outs_sparse.actions.p, (size_t)cnt * 2, cudaMemcpyDeviceToHost, st));
+      if (pods) UST_CUDA(h, cudaMemcpyAsync(actuator_outcome, h->sp_outcome.p, (size_t)cnt, cudaMemcpyDeviceToHost, st));
     }
   }
-  rc = adopt_resident(h, finish_with_counters(h, st, out), n, n_ds);
+  rc = adopt_resident(h, finish_with_counters(h, st, out), n, n_ds, true, pods ? new_total : -1);
   if (sparse && (rc == UST_OK) && *n_out > max_out)
-    return h->fail(UST_ERR_TRUNCATED, "%lld outputs changed, the caller's arrays hold %lld: fetch them with ust_fetch_outputs", (long long)*n_out, (long long)max_out);
+    return h->fail(UST_ERR_TRUNCATED, "%lld outputs changed, the caller's arrays hold %lld: fetch them with %s", (long long)*n_out,
+                   (long long)max_out, pods ? "ust_fetch_outputs_pods" : "ust_fetch_outputs");
   return rc;
 }
 
@@ -1084,7 +1189,7 @@ int ust_apply_state_delta(ust_handle* h, const ust_policy* policy, int64_t n_cha
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  return delta_common(h, policy, nullptr, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, false, next_state, actions,
+  return delta_common(h, policy, nullptr, nullptr, false, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, false, next_state, actions,
                       actuator_outcome, 0, nullptr, nullptr, out);
 }
 
@@ -1095,7 +1200,7 @@ int ust_apply_state_delta_sparse(ust_handle* h, const ust_policy* policy, int64_
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  return delta_common(h, policy, nullptr, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
+  return delta_common(h, policy, nullptr, nullptr, false, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
                       nullptr, max_out, out_idx, n_out, out);
 }
 
@@ -1108,7 +1213,7 @@ int ust_apply_state_delta_splice(ust_handle* h, const ust_policy* policy, const 
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   // node indices of a shard are global ranges (ust_comm_init): a splice would have to move them on every rank
   if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_splice runs on one GPU");
-  return delta_common(h, policy, splice, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
+  return delta_common(h, policy, splice, nullptr, false, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
                       nullptr, max_out, out_idx, n_out, out);
 }
 
@@ -1121,8 +1226,38 @@ int ust_apply_state_delta_reorder(ust_handle* h, const ust_policy* policy, const
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   // node indices of a shard are global ranges (ust_comm_init): a reorder would have to move them on every rank
   if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_reorder runs on one GPU");
-  return delta_common(h, policy, nullptr, reorder, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state,
+  return delta_common(h, policy, nullptr, reorder, false, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state,
                       out_actions, nullptr, max_out, out_idx, n_out, out);
+}
+
+int ust_apply_state_delta_pods(ust_handle* h, const ust_policy* policy, const ust_pod_lists* lists, int64_t n_changed,
+                               const int64_t* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
+                               const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, int64_t max_out, int64_t* out_idx,
+                               uint8_t* out_next_state, uint16_t* out_actions, uint8_t* out_outcome, int64_t* n_out, ust_counters* out) {
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
+  // the pod lists of a shard hold that shard's nodes only; the call keeps to one GPU like the splice and the reorder
+  if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_pods runs on one GPU");
+  return delta_common(h, policy, nullptr, nullptr, true, lists, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true,
+                      out_next_state, out_actions, out_outcome, max_out, out_idx, n_out, out);
+}
+
+int ust_fetch_outputs_pods(ust_handle* h, uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome) {
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
+  if (h->pods_n < 0) return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident pod-list outputs");
+  if (h->pods_n > 0 && (!next_state || !actions || !actuator_outcome)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
+  UST_CUDA(h, cudaSetDevice(h->device));
+  const size_t N = (size_t)h->pods_n;
+  if (N) {
+    UST_CUDA(h, cudaMemcpyAsync(next_state, h->outs.next.p, N, cudaMemcpyDeviceToHost, h->stream));
+    UST_CUDA(h, cudaMemcpyAsync(actions, h->outs.actions.p, N * 2, cudaMemcpyDeviceToHost, h->stream));
+    UST_CUDA(h, cudaMemcpyAsync(actuator_outcome, h->s_outcome.p, N, cudaMemcpyDeviceToHost, h->stream));
+  }
+  UST_CUDA(h, cudaStreamSynchronize(h->stream));
+  return UST_OK;
 }
 
 int ust_fetch_outputs(ust_handle* h, uint8_t* next_state, uint16_t* actions) {

@@ -202,8 +202,19 @@ int ust_launch_sim_init(long long n, const uint32_t* flags, int32_t* entered, in
                         void* stream);
 int ust_launch_widen(long long n, const uint16_t* rev16, const int8_t* ds8, int32_t* rev_out, int32_t* ds_out, int grid,
                      void* stream);
-// sparse outputs of a delta call: nodes whose (next_state, actions) differ from the previous call's, in node order
-int ust_launch_diff(long long n, const uint8_t* next, const uint16_t* actions, const uint8_t* prev_next, const uint16_t* prev_actions,
-                    unsigned int* block_count, long long* n_out, long long cap, long long* out_idx, uint8_t* out_next,
-                    uint16_t* out_actions, void* stream);
+// sparse outputs of a delta call: nodes whose (next_state, actions) differ from the previous call's, in node order; with
+// `outcome` non-null (pod-list deltas) also those whose actuator_outcome differs, which is then written to out_outcome
+int ust_launch_diff(long long n, const uint8_t* next, const uint16_t* actions, const uint8_t* outcome, const uint8_t* prev_next,
+                    const uint16_t* prev_actions, const uint8_t* prev_outcome, unsigned int* block_count, long long* n_out, long long cap,
+                    long long* out_idx, uint8_t* out_next, uint16_t* out_actions, uint8_t* out_outcome, void* stream);
 int ust_diff_blocks(long long n);
+// replacement pod lists of the resident pod-list snapshot (ust_apply_state_delta_pods), checked by the caller: list k
+// (new_flags[new_off[k] .. new_off[k + 1])) replaces the list of node node_idx[k]. Same lengths: copied in place into
+// flags at the offsets in off (one launch). Otherwise: new offsets into o_off (n + 1) and the new CSR into o_flags
+// (new_total pods + 16 of padding), with shift[k] = sum over j < k of the length change of list j and `runs` holding
+// 4 n_lists + 3 entries (two launches)
+int ust_launch_pods_scatter(long long n_lists, const long long* node_idx, const int32_t* new_off, const uint16_t* new_flags,
+                            const int32_t* off, uint16_t* flags, int grid, void* stream);
+int ust_launch_pods_relayout(long long n, long long n_lists, const long long* node_idx, const int32_t* new_off, const int32_t* shift,
+                             const int32_t* off, const uint16_t* flags, const uint16_t* new_flags, int new_total, int32_t* runs,
+                             int32_t* o_off, uint16_t* o_flags, int grid, void* stream);

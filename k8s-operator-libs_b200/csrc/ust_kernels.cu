@@ -13,7 +13,8 @@
 // common_manager.go:462-523).
 // Around it: ust_pod_summary_kernel (pod lists -> one byte per node), ust_build_state*_kernel (BuildState),
 // ust_patch_kernel / ust_splice_kernel / ust_reorder_kernel / ust_feedback_kernel (delta updates, membership changes,
-// new node orders, rollout simulation),
+// new node orders, rollout simulation), ust_pods_scatter_kernel / ust_pods_runs_kernel / ust_pods_relayout_kernel
+// (replaced pod lists), ust_diff_*_kernel (sparse outputs),
 // ust_widen_kernel (packed host format).
 #include <climits>
 
@@ -941,6 +942,158 @@ __global__ void __launch_bounds__(kThreads) ust_reorder_kernel(long long n, long
   }
 }
 
+// Replacement pod lists of the resident pod-list snapshot (ust_apply_state_delta_pods). The host has checked the lists
+// (node_idx strictly increasing, offsets well formed) and knows every replaced list's old length, so it picks the path:
+//   every list keeps its length: ust_pods_scatter_kernel copies each new list over the old one, in place;
+//   some length changes: ust_pods_runs_kernel builds the run table of the new CSR, ust_pods_relayout_kernel writes the
+//   new offsets and pod_flags into the second CSR pair in one pass.
+// shift[k] (host-computed, n_lists + 1 entries) = sum over j < k of (new length - old length) of list j: node i's new
+// offset is off[i] + shift[#{k : node_idx[k] < i}].
+constexpr int kRelayTile = 8192;                   // new pod positions per CTA: 32 per thread, four 16-byte stores
+constexpr int kRelayRuns = 2048;                   // runs a CTA stages in shared memory (more: it searches them in global memory)
+constexpr int kOffTile = 2048;                     // offsets per CTA
+
+// One warp per list: 2 B read and written per pod of the replaced lists, 12 B per list.
+__global__ void __launch_bounds__(kThreads) ust_pods_scatter_kernel(long long n_lists, const long long* __restrict__ node_idx,
+                                                                    const int32_t* __restrict__ new_off,
+                                                                    const uint16_t* __restrict__ new_flags,
+                                                                    const int32_t* __restrict__ off, uint16_t* __restrict__ flags) {
+  const int lane = threadIdx.x & 31;
+  const long long warps = (long long)gridDim.x * kWarps;
+  for (long long k = (long long)blockIdx.x * kWarps + (threadIdx.x >> 5); k < n_lists; k += warps) {
+    const int s0 = __ldg(new_off + k), s1 = __ldg(new_off + k + 1);
+    const int d = __ldg(off + __ldg(node_idx + k)) - s0;
+    for (int p = s0 + lane; p < s1; p += 32) flags[d + p] = __ldg(new_flags + p);
+  }
+}
+
+// The new CSR as 2 n_lists + 1 runs of new pod positions [run_start[r], run_start[r + 1]) (run_start[2 n_lists + 1] =
+// new_total): even r = 2k, the unchanged nodes between list k - 1 and list k, old pods from run_src[r] on; odd r = 2k + 1,
+// new list k, from new_flags[run_src[r]] on. Runs may be empty.
+__global__ void __launch_bounds__(kThreads) ust_pods_runs_kernel(long long n_lists, const long long* __restrict__ node_idx,
+                                                                 const int32_t* __restrict__ new_off, const int32_t* __restrict__ shift,
+                                                                 const int32_t* __restrict__ off, int new_total,
+                                                                 int32_t* __restrict__ run_start, int32_t* __restrict__ run_src) {
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long k = (long long)blockIdx.x * kThreads + threadIdx.x; k <= n_lists; k += stride) {
+    const int prev_end = k ? __ldg(off + __ldg(node_idx + k - 1) + 1) : 0;  // old end of list k - 1
+    const int d = __ldg(shift + k);
+    run_start[2 * k] = prev_end + d;
+    run_src[2 * k] = prev_end;
+    if (k < n_lists) {
+      run_start[2 * k + 1] = __ldg(off + __ldg(node_idx + k)) + d;
+      run_src[2 * k + 1] = __ldg(new_off + k);
+    } else {
+      run_start[2 * k + 1] = new_total;
+    }
+  }
+}
+
+// Eight pods from src[s], s any position: two aligned 16-byte loads, shifted by s & 7 pods (the buffers hold 8 pods
+// of padding past their last pod, so the second load stays inside them).
+__device__ __forceinline__ uint4 pods8_at(const uint16_t* __restrict__ src, int s) {
+  const uint4* a = reinterpret_cast<const uint4*>(src + (s & ~7));
+  const uint4 lo = __ldg(a), hi = __ldg(a + 1);
+  uint32_t v0 = lo.x, v1 = lo.y, v2 = lo.z, v3 = lo.w, v4 = hi.x, v5 = hi.y, v6 = hi.z, v7 = hi.w;
+  const int w = (s & 7) >> 1;  // whole words
+  if (w & 2) { v0 = v2; v1 = v3; v2 = v4; v3 = v5; v4 = v6; v5 = v7; }
+  if (w & 1) { v0 = v1; v1 = v2; v2 = v3; v3 = v4; v4 = v5; }
+  const unsigned sh = (s & 1) * 16u;
+  return make_uint4(__funnelshift_r(v0, v1, sh), __funnelshift_r(v1, v2, sh), __funnelshift_r(v2, v3, sh), __funnelshift_r(v3, v4, sh));
+}
+
+union RelayoutSmem {
+  struct { int32_t start[kRelayRuns + 1]; int32_t src[kRelayRuns]; } pods;
+  struct { long long idx[kOffTile]; int32_t shift[kOffTile + 1]; } offs;
+};
+
+// CTAs [0, pod_ctas) gather the new pod_flags by tiles of kRelayTile new positions; the CTAs after them write the n + 1
+// new offsets by tiles of kOffTile nodes. Both search their tile's runs once and stage them in shared memory.
+// 2 B read + 2 B written per pod, 8 B per node, each new list once.
+__global__ void __launch_bounds__(kThreads) ust_pods_relayout_kernel(long long n, long long n_lists, const long long* __restrict__ node_idx,
+                                                                     const int32_t* __restrict__ shift, const int32_t* __restrict__ off,
+                                                                     int32_t* __restrict__ o_off, const int32_t* __restrict__ run_start,
+                                                                     const int32_t* __restrict__ run_src, const uint16_t* __restrict__ flags,
+                                                                     const uint16_t* __restrict__ new_flags, uint16_t* __restrict__ o_flags,
+                                                                     int new_total, int pod_ctas) {
+  __shared__ __align__(16) RelayoutSmem sm;
+  __shared__ long long s_bounds[2];
+  const int t = threadIdx.x;
+  if ((int)blockIdx.x >= pod_ctas) {
+    // ---- offsets: node i takes shift[c], c = #{k : node_idx[k] < i}
+    const long long b0 = (long long)(blockIdx.x - pod_ctas) * kOffTile;
+    const long long b1 = b0 + kOffTile < n + 1 ? b0 + kOffTile : n + 1;
+    if (t < 2) s_bounds[t] = splice_lower_bound(node_idx, n_lists, t ? b1 : b0);
+    __syncthreads();
+    const long long c0 = s_bounds[0];
+    const int nc = (int)(s_bounds[1] - c0);  // node_idx is strictly increasing: at most kOffTile of them fall in [b0, b1)
+    for (int j = t; j < nc; j += kThreads) sm.offs.idx[j] = __ldg(node_idx + c0 + j);
+    for (int j = t; j <= nc; j += kThreads) sm.offs.shift[j] = __ldg(shift + c0 + j);
+    __syncthreads();
+    for (int j = t; j < (int)(b1 - b0); j += kThreads) {
+      const long long i = b0 + j;
+      int lo = 0, hi = nc;  // first staged k with node_idx[k] >= i
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (sm.offs.idx[mid] < i) lo = mid + 1; else hi = mid;
+      }
+      o_off[i] = __ldcs(off + i) + sm.offs.shift[lo];
+    }
+    return;
+  }
+  // ---- pods: the runs that cover new positions [q0, q1)
+  const long long n_runs = 2 * n_lists + 1;
+  const int q0 = blockIdx.x * kRelayTile;
+  const int q1 = q0 + kRelayTile < new_total ? q0 + kRelayTile : new_total;
+  if (t < 2) {  // the last run that starts at or before q0 (t = 0) / q1 - 1 (t = 1)
+    const int v = t ? q1 - 1 : q0;
+    long long lo = 0, hi = n_runs;
+    while (hi - lo > 1) {
+      const long long mid = (lo + hi) >> 1;
+      if (__ldg(run_start + mid) <= v) lo = mid; else hi = mid;
+    }
+    s_bounds[t] = lo;
+  }
+  __syncthreads();
+  const long long r0 = s_bounds[0];
+  const int nr = (int)(s_bounds[1] - r0 + 1);
+  // empty runs are not bounded by the tile: a tile that meets more runs than fit reads them from global memory
+  const bool staged = nr <= kRelayRuns;
+  if (staged) {
+    for (int j = t; j <= nr; j += kThreads) sm.pods.start[j] = __ldg(run_start + r0 + j);
+    for (int j = t; j < nr; j += kThreads) sm.pods.src[j] = __ldg(run_src + r0 + j);
+  }
+  __syncthreads();
+  const int32_t* S = staged ? sm.pods.start : run_start + r0;
+  const int32_t* R = staged ? sm.pods.src : run_src + r0;
+  const int chunks = (q1 - q0 + 7) >> 3;
+#pragma unroll 2
+  for (int c = t; c < chunks; c += kThreads) {
+    const int q = q0 + 8 * c;
+    int r = 0, hi = nr;  // the run that holds q
+    while (hi - r > 1) {
+      const int mid = (r + hi) >> 1;
+      if (S[mid] <= q) r = mid; else hi = mid;
+    }
+    uint4 v;
+    if (q + 8 <= S[r + 1] && q + 8 <= new_total) {  // the chunk lies in one run: one shifted 16-byte copy
+      v = pods8_at(((r0 + r) & 1) ? new_flags : flags, R[r] + (q - S[r]));
+    } else {  // it straddles runs (or the end of the array): pod by pod
+      uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+      for (int e = 0; e < 8; e++) {
+        const int p = q + e;
+        if (p >= new_total) break;
+        while (S[r + 1] <= p) r++;
+        const uint16_t* src = ((r0 + r) & 1) ? new_flags : flags;
+        w[e >> 1] |= (uint32_t)__ldg(src + R[r] + (p - S[r])) << (16 * (e & 1));
+      }
+      v = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+    *reinterpret_cast<uint4*>(o_flags + q) = v;
+  }
+}
+
 // Rollout simulation (SURVEY 8f.3): the state feedback between two reconciles. Untimed (sp.timed == 0): "ideal actuators" - every call
 // the reference makes through its providers takes effect, every asynchronous actuator succeeds, and whatever a node
 // is waiting for (jobs, pod readiness, validation) has happened by the next reconcile. One streaming pass, in place:
@@ -1072,16 +1225,22 @@ __global__ void __launch_bounds__(kThreads) ust_widen_kernel(long long n, const 
 }
 // Sparse outputs of a delta call (SURVEY 8f.2): the nodes whose (next_state, actions) differ from the previous call's,
 // compacted in node order. Three launches: per-block counts, a one-CTA scan of the block counts, the ordered write.
-// 6 B/node read twice; the alternative is 3 B/node over PCIe.
+// 6 B/node read twice; the alternative is 3 B/node over PCIe. OUTCOME (ust_apply_state_delta_pods): actuator_outcome
+// is compared and returned too, 8 B/node read twice.
 constexpr int kDiffBlock = 4096;  // nodes per CTA: 16 per thread
-__device__ __forceinline__ unsigned diff_mask16(const uint8_t* next, const uint16_t* act, const uint8_t* pnext, const uint16_t* pact,
-                                                long long i0, long long n) {
+template <bool OUTCOME>
+__device__ __forceinline__ unsigned diff_mask16(const uint8_t* next, const uint16_t* act, const uint8_t* oc, const uint8_t* pnext,
+                                                const uint16_t* pact, const uint8_t* poc, long long i0, long long n) {
   unsigned m = 0;
   if (i0 + 16 <= n) {
     const uint4 a = __ldcs(reinterpret_cast<const uint4*>(next + i0)), b = __ldcs(reinterpret_cast<const uint4*>(pnext + i0));
     const uint4 c0 = __ldcs(reinterpret_cast<const uint4*>(act + i0)), c1 = __ldcs(reinterpret_cast<const uint4*>(act + i0 + 8));
     const uint4 d0 = __ldcs(reinterpret_cast<const uint4*>(pact + i0)), d1 = __ldcs(reinterpret_cast<const uint4*>(pact + i0 + 8));
-    const uint32_t x[4] = {a.x ^ b.x, a.y ^ b.y, a.z ^ b.z, a.w ^ b.w};
+    uint32_t x[4] = {a.x ^ b.x, a.y ^ b.y, a.z ^ b.z, a.w ^ b.w};
+    if constexpr (OUTCOME) {  // an outcome byte that differs counts like a next_state byte that differs
+      const uint4 e = __ldcs(reinterpret_cast<const uint4*>(oc + i0)), f = __ldcs(reinterpret_cast<const uint4*>(poc + i0));
+      x[0] |= e.x ^ f.x; x[1] |= e.y ^ f.y; x[2] |= e.z ^ f.z; x[3] |= e.w ^ f.w;
+    }
     const uint32_t y[8] = {c0.x ^ d0.x, c0.y ^ d0.y, c0.z ^ d0.z, c0.w ^ d0.w, c1.x ^ d1.x, c1.y ^ d1.y, c1.z ^ d1.z, c1.w ^ d1.w};
 #pragma unroll
     for (int k = 0; k < 16; k++) {
@@ -1091,18 +1250,21 @@ __device__ __forceinline__ unsigned diff_mask16(const uint8_t* next, const uint1
     }
   } else {
     for (int k = 0; k < 16; k++)
-      if (i0 + k < n && (next[i0 + k] != pnext[i0 + k] || act[i0 + k] != pact[i0 + k])) m |= 1u << k;
+      if (i0 + k < n && (next[i0 + k] != pnext[i0 + k] || act[i0 + k] != pact[i0 + k] || (OUTCOME && oc[i0 + k] != poc[i0 + k])))
+        m |= 1u << k;
   }
   return m;
 }
+template <bool OUTCOME>
 __global__ void __launch_bounds__(kThreads) ust_diff_count_kernel(long long n, const uint8_t* __restrict__ next, const uint16_t* __restrict__ act,
-                                                                  const uint8_t* __restrict__ pnext, const uint16_t* __restrict__ pact,
+                                                                  const uint8_t* __restrict__ oc, const uint8_t* __restrict__ pnext,
+                                                                  const uint16_t* __restrict__ pact, const uint8_t* __restrict__ poc,
                                                                   unsigned int* __restrict__ block_count) {
   __shared__ unsigned int tot;
   if (threadIdx.x == 0) tot = 0;
   __syncthreads();
   const long long i0 = (long long)blockIdx.x * kDiffBlock + 16 * threadIdx.x;
-  unsigned c = i0 < n ? __popc(diff_mask16(next, act, pnext, pact, i0, n)) : 0u;
+  unsigned c = i0 < n ? __popc(diff_mask16<OUTCOME>(next, act, oc, pnext, pact, poc, i0, n)) : 0u;
   c = __reduce_add_sync(kFull, c);
   if ((threadIdx.x & 31) == 0 && c) atomicAdd(&tot, c);
   __syncthreads();
@@ -1136,15 +1298,17 @@ __global__ void __launch_bounds__(1024) ust_diff_scan_kernel(int blocks, unsigne
   }
   if (t == 0) *n_out = (long long)carry;
 }
+template <bool OUTCOME>
 __global__ void __launch_bounds__(kThreads) ust_diff_write_kernel(long long n, const uint8_t* __restrict__ next, const uint16_t* __restrict__ act,
-                                                                  const uint8_t* __restrict__ pnext, const uint16_t* __restrict__ pact,
+                                                                  const uint8_t* __restrict__ oc, const uint8_t* __restrict__ pnext,
+                                                                  const uint16_t* __restrict__ pact, const uint8_t* __restrict__ poc,
                                                                   const unsigned int* __restrict__ block_off, long long cap,
                                                                   long long* __restrict__ out_idx, uint8_t* __restrict__ out_next,
-                                                                  uint16_t* __restrict__ out_act) {
+                                                                  uint16_t* __restrict__ out_act, uint8_t* __restrict__ out_oc) {
   __shared__ unsigned int wtot[kWarps];
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const long long i0 = (long long)blockIdx.x * kDiffBlock + 16 * t;
-  const unsigned m = i0 < n ? diff_mask16(next, act, pnext, pact, i0, n) : 0u;
+  const unsigned m = i0 < n ? diff_mask16<OUTCOME>(next, act, oc, pnext, pact, poc, i0, n) : 0u;
   const unsigned c = __popc(m);
   unsigned incl = c;
 #pragma unroll
@@ -1165,6 +1329,7 @@ __global__ void __launch_bounds__(kThreads) ust_diff_write_kernel(long long n, c
       out_idx[pos] = i0 + k;
       out_next[pos] = next[i0 + k];
       out_act[pos] = act[i0 + k];
+      if constexpr (OUTCOME) out_oc[pos] = oc[i0 + k];
     }
     pos++;
   }
@@ -1234,6 +1399,28 @@ int ust_launch_reorder(long long n, long long n_runs, const long long* run_off, 
                                                                             o_rev, o_ds, o_next, o_act);
   return (int)cudaGetLastError();
 }
+int ust_launch_pods_scatter(long long n_lists, const long long* node_idx, const int32_t* new_off, const uint16_t* new_flags,
+                            const int32_t* off, uint16_t* flags, int grid, void* stream) {
+  const long long want = (n_lists + kWarps - 1) / kWarps;
+  const int g = want < 1 ? 1 : (want < grid ? (int)want : grid);
+  ust_pods_scatter_kernel<<<g, kThreads, 0, (cudaStream_t)stream>>>(n_lists, node_idx, new_off, new_flags, off, flags);
+  return (int)cudaGetLastError();
+}
+int ust_launch_pods_relayout(long long n, long long n_lists, const long long* node_idx, const int32_t* new_off, const int32_t* shift,
+                             const int32_t* off, const uint16_t* flags, const uint16_t* new_flags, int new_total, int32_t* runs,
+                             int32_t* o_off, uint16_t* o_flags, int grid, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  int32_t* run_start = runs;                      // 2 n_lists + 2 entries
+  int32_t* run_src = runs + 2 * n_lists + 2;      // 2 n_lists + 1 entries
+  const long long want = (n_lists + 1 + kThreads - 1) / kThreads;
+  ust_pods_runs_kernel<<<(unsigned)(want < grid ? want : grid), kThreads, 0, st>>>(n_lists, node_idx, new_off, shift, off, new_total,
+                                                                                 run_start, run_src);
+  const int pod_ctas = (new_total + kRelayTile - 1) / kRelayTile;
+  const long long off_ctas = n / kOffTile + 1;    // offsets 0..n
+  ust_pods_relayout_kernel<<<(unsigned)(pod_ctas + off_ctas), kThreads, 0, st>>>(n, n_lists, node_idx, shift, off, o_off, run_start, run_src,
+                                                                                 flags, new_flags, o_flags, new_total, pod_ctas);
+  return (int)cudaGetLastError();
+}
 int ust_launch_feedback(long long n, uint8_t* hot, uint32_t* flags, int32_t* pod_rev, const int32_t* ds_idx, int n_ds,
                         const int32_t* ds_rev, const uint8_t* next, const uint16_t* actions, const uint8_t* outcome,
                         const ust_counters* step, const UstSimParams& sp, int32_t* entered, int32_t* wait_start,
@@ -1258,15 +1445,28 @@ int ust_launch_build_state_uids(long long n, const uint8_t* hot, const void* own
   ust_build_state_finish_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(n_ds, ds_desired, ds_count, ws, out);
   return (int)cudaGetLastError();
 }
-int ust_launch_diff(long long n, const uint8_t* next, const uint16_t* actions, const uint8_t* prev_next, const uint16_t* prev_actions,
-                    unsigned int* block_count, long long* n_out, long long cap, long long* out_idx, uint8_t* out_next,
-                    uint16_t* out_actions, void* stream) {
+int ust_launch_diff(long long n, const uint8_t* next, const uint16_t* actions, const uint8_t* outcome, const uint8_t* prev_next,
+                    const uint16_t* prev_actions, const uint8_t* prev_outcome, unsigned int* block_count, long long* n_out, long long cap,
+                    long long* out_idx, uint8_t* out_next, uint16_t* out_actions, uint8_t* out_outcome, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
   const long long blocks = (n + kDiffBlock - 1) / kDiffBlock;
-  if (blocks > 0) ust_diff_count_kernel<<<(unsigned)blocks, kThreads, 0, st>>>(n, next, actions, prev_next, prev_actions, block_count);
+  if (blocks > 0) {
+    if (outcome)
+      ust_diff_count_kernel<true><<<(unsigned)blocks, kThreads, 0, st>>>(n, next, actions, outcome, prev_next, prev_actions, prev_outcome,
+                                                                           block_count);
+    else
+      ust_diff_count_kernel<false><<<(unsigned)blocks, kThreads, 0, st>>>(n, next, actions, nullptr, prev_next, prev_actions, nullptr,
+                                                                            block_count);
+  }
   ust_diff_scan_kernel<<<1, 1024, 0, st>>>((int)blocks, block_count, n_out);
-  if (blocks > 0)
-    ust_diff_write_kernel<<<(unsigned)blocks, kThreads, 0, st>>>(n, next, actions, prev_next, prev_actions, block_count, cap, out_idx, out_next, out_actions);
+  if (blocks > 0) {
+    if (outcome)
+      ust_diff_write_kernel<true><<<(unsigned)blocks, kThreads, 0, st>>>(n, next, actions, outcome, prev_next, prev_actions, prev_outcome,
+                                                                           block_count, cap, out_idx, out_next, out_actions, out_outcome);
+    else
+      ust_diff_write_kernel<false><<<(unsigned)blocks, kThreads, 0, st>>>(n, next, actions, nullptr, prev_next, prev_actions, nullptr,
+                                                                            block_count, cap, out_idx, out_next, out_actions, nullptr);
+  }
   return (int)cudaGetLastError();
 }
 int ust_diff_blocks(long long n) { return (int)((n + kDiffBlock - 1) / kDiffBlock); }

@@ -99,6 +99,12 @@ class Reorder(C.Structure):
                 ("state", C.c_void_p), ("flags", C.c_void_p), ("pod_rev", C.c_void_p), ("ds_idx", C.c_void_p)]
 
 
+class PodLists(C.Structure):
+    """ust_pod_lists: replacement pod lists for some nodes of the resident pod-list snapshot (raw host addresses)."""
+    _fields_ = [("n_lists", C.c_int64), ("node_idx", C.c_void_p), ("pod_off", C.c_void_p), ("pod_flags", C.c_void_p),
+                ("n_pods", C.c_int64)]
+
+
 def make_policy(auto_upgrade=True, max_parallel_upgrades=0, max_unavailable=None, pod_deletion_enabled=False,
                 validation_enabled=False, pod_deletion=None, drain=None, wait_for_completion=None,
                 use_maintenance_operator=False, evaluate_actuators=False):

@@ -57,7 +57,11 @@ def load():
         lib.ust_apply_state_delta_reorder.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                                       C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                                       C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.ust_apply_state_delta_pods.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.ust_fetch_outputs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.ust_fetch_outputs_pods.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.ust_simulate_rollout.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.ust_simulate_rollout_timed.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                    C.c_void_p, C.c_void_p]
@@ -75,7 +79,7 @@ def load():
 
 
 EXPORTS = ["ust_abi_version", "ust_create", "ust_destroy", "ust_last_error", "ust_create_error", "ust_launch_count",
-           "ust_host_alloc", "ust_host_free", "ust_apply_state", "ust_apply_state_device", "ust_stream", "ust_apply_state_packed", "ust_apply_state_delta", "ust_apply_state_delta_sparse", "ust_apply_state_delta_splice", "ust_apply_state_delta_reorder", "ust_fetch_outputs", "ust_simulate_rollout", "ust_simulate_rollout_timed", "ust_sync",
+           "ust_host_alloc", "ust_host_free", "ust_apply_state", "ust_apply_state_device", "ust_stream", "ust_apply_state_packed", "ust_apply_state_delta", "ust_apply_state_delta_sparse", "ust_apply_state_delta_splice", "ust_apply_state_delta_reorder", "ust_apply_state_delta_pods", "ust_fetch_outputs", "ust_fetch_outputs_pods", "ust_simulate_rollout", "ust_simulate_rollout_timed", "ust_sync",
            "ust_build_state", "ust_build_state_uids", "ust_get_unique_id", "ust_comm_init", "ust_comm_set_mode", "ust_table_entry",
            "ust_table_window_shift"]
 
@@ -330,6 +334,47 @@ class Handle:
             int(ds_rev.shape[0]), _p(ds_rev), C.c_int64(int(max_out)), _p(out[0]), _p(out[1]), _p(out[2]), C.addressof(n_out),
             C.addressof(cnt))
         return rc, int(n_out.value), out[0], out[1], out[2], cnt.as_dict()
+
+    def apply_state_delta_pods(self, policy, lists, idx, changed, ds_rev, max_out, out=None):
+        """ust_apply_state_delta_pods: apply_state_delta_sparse on the resident pod-list snapshot after replacing the pod lists
+        of some nodes. `lists` is None or a dict with node_idx, pod_off and pod_flags. Returns (rc, n_out, out_idx, out_next,
+        out_actions, out_outcome, counters-dict); the arrays hold n_out entries when n_out <= max_out."""
+        keep = []
+
+        def arr(a, dt):
+            a = np.ascontiguousarray(a, dtype=dt)
+            keep.append(a)
+            return a
+
+        pl = None
+        if lists is not None:
+            ni = arr(lists["node_idx"], np.int64)
+            off = arr(lists["pod_off"], np.int32)
+            pf = arr(lists["pod_flags"], np.uint16)
+            pl = abi.PodLists(int(ni.shape[0]), _p(ni), _p(off), _p(pf), int(pf.shape[0]))
+        idx = arr(idx, np.int64)
+        ch = {"state": arr(changed["state"], np.uint8), "flags": arr(changed["flags"], np.uint32),
+              "pod_rev": arr(changed["pod_rev"], np.int32), "ds_idx": arr(changed["ds_idx"], np.int32)}
+        ds_rev = arr(ds_rev, np.int32)
+        if out is None:
+            out = (np.zeros(max_out + 1, np.int64), np.zeros(max_out + 1, np.uint8), np.zeros(max_out + 1, np.uint16),
+                   np.zeros(max_out + 1, np.uint8))
+        n_out = C.c_int64(0)
+        cnt = abi.Counters()
+        rc = self._lib.ust_apply_state_delta_pods(
+            self._h, C.addressof(policy) if policy is not None else None, C.addressof(pl) if pl is not None else None,
+            int(idx.shape[0]), _p(idx), _p(ch["state"]), _p(ch["flags"]), _p(ch["pod_rev"]), _p(ch["ds_idx"]),
+            int(ds_rev.shape[0]), _p(ds_rev), C.c_int64(int(max_out)), _p(out[0]), _p(out[1]), _p(out[2]), _p(out[3]),
+            C.addressof(n_out), C.addressof(cnt))
+        return rc, int(n_out.value), out[0], out[1], out[2], out[3], cnt.as_dict()
+
+    def fetch_outputs_pods(self, n):
+        """ust_fetch_outputs_pods: (rc, next_state, actions, actuator_outcome) of the last call on the pod-list snapshot."""
+        nxt = np.zeros(n, np.uint8)
+        act = np.zeros(n, np.uint16)
+        oc = np.zeros(n, np.uint8)
+        rc = self._lib.ust_fetch_outputs_pods(self._h, _p(nxt), _p(act), _p(oc))
+        return rc, nxt, act, oc
 
     def fetch_outputs(self, n):
         nxt = np.zeros(n, np.uint8)
