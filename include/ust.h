@@ -379,8 +379,10 @@ typedef struct ust_pod_lists {
  * The resident pod-list snapshot is left by
  *   - a ust_apply_state call with pods != NULL and actuator_outcome != NULL that produced counters (a reference-level
  *     abort counts),
- *   - a ust_apply_state_delta_pods call that produced counters (UST_ERR_TRUNCATED counts).
- * Only ust_apply_state_delta_pods and ust_fetch_outputs_pods use it: after a call with pod lists, ust_apply_state_delta,
+ *   - a ust_apply_state_delta_pods or ust_apply_state_delta_pods_reorder call that produced counters (UST_ERR_TRUNCATED
+ *     counts).
+ * Only ust_apply_state_delta_pods, ust_apply_state_delta_pods_reorder and ust_fetch_outputs_pods use it: after a call
+ * with pod lists, ust_apply_state_delta,
  * _sparse, _splice, _reorder, ust_fetch_outputs and the simulations find nothing resident, as before. Every call that
  * drops the resident snapshot drops the pod-list snapshot too: ust_apply_state without pods, _packed, both BuildStates,
  * the simulations, the node delta calls and any call that fails once its arguments were accepted.
@@ -402,6 +404,29 @@ int ust_apply_state_delta_pods(ust_handle* h, const ust_policy* policy, const us
                                const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev,
                                int64_t max_out, int64_t* out_idx, uint8_t* out_next_state, uint16_t* out_actions,
                                uint8_t* out_outcome, int64_t* n_out, ust_counters* out);
+/* ust_apply_state_delta_pods for any new node order of the resident pod-list snapshot: nodes join, leave and move (a
+ * restarted driver pod comes back under a new name, so its node moves in BuildState's list), and their pod lists move
+ * with them. `reorder` means what it means for ust_apply_state_delta_reorder. One call (1) puts the nodes, their pod
+ * lists and the previous call's outputs into the new order, (2) replaces the lists of lists->node_idx, (3) applies the
+ * n_changed node overwrites exactly as ust_apply_state_delta, then evaluates the whole new snapshot with its pod lists.
+ * lists->node_idx and idx are indices into the NEW snapshot. Every inserted node must be named in `lists` (an empty list
+ * is pod_off[k] == pod_off[k + 1]), so that a forgotten list is an error rather than a silent empty one. Sparse outputs
+ * in new-index order with out_outcome: every inserted node is reported, a node that stayed when its next_state, actions
+ * or actuator_outcome differs from what the previous call returned for it (wherever it moved), a node that left never.
+ * Counters, aborts, UST_ERR_TRUNCATED and ust_fetch_outputs_pods (then with the new node count) work as in
+ * ust_apply_state_delta_pods. reorder == NULL: exactly ust_apply_state_delta_pods (the same outputs and launches).
+ * A violated contract (everything ust_apply_state_delta_reorder rejects in `reorder`, node_idx unsorted, duplicated or
+ * outside the new snapshot, an inserted node missing from `lists`, malformed replacement offsets, a new pod total of 2^31
+ * or more, NULL arrays, idx outside the new snapshot, no resident pod-list snapshot, more than one rank set up by
+ * ust_comm_init) returns UST_ERR_INVALID_ARGUMENT before any device work: the resident snapshot stays as it was. The
+ * checks cost O(n + n_runs + n_lists + n_pods + n_changed) host time; the O(n) part moves one int32 list length per node.
+ * With a reorder the resident CSR is always gathered anew on the device, in one pass behind a run table. */
+int ust_apply_state_delta_pods_reorder(ust_handle* h, const ust_policy* policy, const ust_reorder* reorder /* nullable */,
+                                       const ust_pod_lists* lists /* nullable */, int64_t n_changed, const int64_t* idx,
+                                       const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
+                                       const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, int64_t max_out,
+                                       int64_t* out_idx, uint8_t* out_next_state, uint16_t* out_actions,
+                                       uint8_t* out_outcome, int64_t* n_out, ust_counters* out);
 /* The full outputs of the last call on the resident pod-list snapshot (n_nodes entries each). */
 int ust_fetch_outputs_pods(ust_handle* h, uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome);
 

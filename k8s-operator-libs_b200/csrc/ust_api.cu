@@ -9,6 +9,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <algorithm>
+#include <chrono>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -214,6 +215,14 @@ struct ust_handle {
   IndexedColumns inserted;
   std::vector<long long> run_off, run_src;
   std::vector<uint64_t> run_seen;
+  // a reorder of the pod-list snapshot: the previous outcome in the new order (swapped with s_outcome), the segments of
+  // the new pod CSR (seg_node, seg_src / pod_start, pod_src: see ust_launch_pods_reorder) and their host copies
+  DevBuf<uint8_t> splice_outcome;
+  DevBuf<long long> pr_segs;
+  DevBuf<int32_t> pr_pods;
+  std::vector<long long> seg_node, seg_src;
+  std::vector<int32_t> seg_pod;
+  long long pod_pass_ns = 0;  // diagnostics: host time of the last pods_reorder_segments
   DevBuf<int32_t> sim_entered, sim_wait, sim_valid;  // timed rollout simulation: per-node clocks
 
   // multi-GPU
@@ -969,10 +978,62 @@ static int reorder_runs(ust_handle* h, const ust_reorder* ro, int64_t n_old, int
   return rc;
 }
 
-// ust_apply_state_delta, _delta_sparse, _delta_splice, _delta_reorder and _delta_pods: bring the resident snapshot into a
-// new node order (optional: nodes leave, join and move), scatter the re-encoded nodes into it, evaluate everything, return
-// all outputs (dense) or the outputs that differ from the previous call's (sparse). `pods`: the pod-list snapshot, whose
-// lists `pl` (nullable) replaces first; its sparse outputs include actuator_outcome (written to `actuator_outcome`).
+// The pod lists of a reorder of the pod-list snapshot of n_new nodes, after reorder_runs: the runs and the replaced lists
+// (node_idx: new indices, checked) walked together. Fills h->pod_len_next with every new node's list length (moved run by
+// run from h->pod_len, the lengths of replaced and inserted lists written over it) and cuts the new snapshot into the
+// segments of ust_launch_pods_reorder, with their pod starts. Fails when an inserted node has no list or the new pod total
+// reaches 2^31. Linear in n_new (4 B read and written per node), otherwise O(n_runs + n_lists); h->pod_len is untouched.
+static int pods_reorder_segments(ust_handle* h, const ust_pod_lists* pl, int64_t L, int64_t n_new, int64_t* new_total) {
+  h->pod_len_next.resize((size_t)n_new);
+  int32_t* len = h->pod_len_next.data();
+  const int32_t* old = h->pod_len.data();
+  const size_t NR = h->run_src.size();
+  h->seg_node.clear();
+  h->seg_src.clear();
+  h->seg_pod.clear();
+  h->seg_node.reserve(NR + 2 * (size_t)L + 1);
+  h->seg_src.reserve(NR + 2 * (size_t)L);
+  h->seg_pod.reserve(NR + 2 * (size_t)L + 1);
+  int64_t k = 0, total = 0;  // next list; pods ahead of the segment being cut (int32 once the total is checked)
+  for (size_t r = 0; r < NR; r++) {
+    const long long o = h->run_off[r], e = h->run_off[r + 1], src = h->run_src[r];
+    for (long long p = o; p < e;) {
+      h->seg_node.push_back(p);
+      h->seg_pod.push_back((int32_t)total);
+      if (k < L && pl->node_idx[k] == p) {  // a replaced or inserted list: a segment of its own
+        len[p] = pl->pod_off[k + 1] - pl->pod_off[k];
+        h->seg_src.push_back(-1 - k);
+        total += len[p];
+        k++;
+        p++;
+      } else if (src < 0) {
+        return h->fail(UST_ERR_INVALID_ARGUMENT, "pod lists: inserted node %lld has no list: every inserted node needs one", p);
+      } else {  // old nodes up to the next replaced list
+        const long long q = k < L && pl->node_idx[k] < e ? pl->node_idx[k] : e;
+        const int32_t* from = old + src + (p - o);
+        int64_t pods = 0;
+        for (long long j = 0; j < q - p; j++) {
+          len[p + j] = from[j];
+          pods += from[j];
+        }
+        h->seg_src.push_back(src + (p - o));
+        total += pods;
+        p = q;
+      }
+    }
+  }
+  if (total >= (1LL << 31)) return h->fail(UST_ERR_INVALID_ARGUMENT, "pod lists: %lld pods in all, pod_off is int32", (long long)total);
+  h->seg_node.push_back(n_new);
+  h->seg_pod.push_back((int32_t)total);
+  *new_total = total;
+  return UST_OK;
+}
+
+// ust_apply_state_delta, _delta_sparse, _delta_splice, _delta_reorder, _delta_pods and _delta_pods_reorder: bring the
+// resident snapshot into a new node order (optional: nodes leave, join and move), scatter the re-encoded nodes into it,
+// evaluate everything, return all outputs (dense) or the outputs that differ from the previous call's (sparse). `pods`:
+// the pod-list snapshot, whose lists `pl` (nullable) replaces first (after its reorder, `ro`, which moves the lists and
+// the previous outcome with the nodes); its sparse outputs include actuator_outcome (written to `actuator_outcome`).
 static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splice* sp, const ust_reorder* ro, bool pods,
                         const ust_pod_lists* pl, int64_t n_changed, const int64_t* idx, const uint8_t* state, const uint32_t* flags,
                         const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, bool sparse,
@@ -1025,7 +1086,8 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
   for (int64_t k = 0; k < n_changed; k++)
     if (idx[k] < 0 || idx[k] >= n) return h->fail(UST_ERR_INVALID_ARGUMENT, "changed node %lld has index %lld outside the snapshot of %lld nodes", (long long)k, (long long)idx[k], (long long)n);
   // replacement pod lists, checked in O(n_lists + n_pods) against the host copy of the resident list lengths; with every
-  // length kept they are copied in place, otherwise the CSR is laid out anew (pl_shift_host: prefix of the length changes)
+  // length kept they are copied in place, otherwise the CSR is laid out anew (pl_shift_host: prefix of the length changes).
+  // Under a reorder the CSR is always gathered anew, from the segments that pods_reorder_segments cuts.
   const int64_t L = pods && pl ? pl->n_lists : 0;
   int64_t new_total = pods ? h->pods_total : 0;
   bool same_len = true;
@@ -1037,6 +1099,13 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
         return h->fail(UST_ERR_INVALID_ARGUMENT, "pod lists: node_idx[%lld] = %lld is not strictly increasing in [0, %lld)", (long long)k,
                        (long long)pl->node_idx[k], (long long)n);
     if (int rc = check_pod_offsets_host(h, L, pl->pod_off, pl->n_pods)) return rc;
+  }
+  const bool pods_gather = pods && ro;
+  if (pods_gather) {
+    const auto t0 = std::chrono::steady_clock::now();
+    if (int rc = pods_reorder_segments(h, pl, L, n, &new_total)) return rc;
+    h->pod_pass_ns = std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
+  } else if (L != 0) {
     h->pl_shift_host.resize((size_t)L + 1);
     int64_t d = 0;
     for (int64_t k = 0; k < L; k++) {
@@ -1063,10 +1132,19 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
     UST_CUDA(h, h->inserted.cols.reserve(I));
   }
   UST_CUDA(h, h->s_dsrev.reserve((size_t)n_ds + 1));
-  if (actuator_outcome || pods) UST_CUDA(h, h->s_outcome.reserve(N + 16));
+  // (under a reorder s_outcome holds the previous outcome at the old size, which the gather reads: it is not resized)
+  if (pods ? !ro : actuator_outcome != nullptr) UST_CUDA(h, h->s_outcome.reserve(N + 16));
   if (pods && sparse) {
     UST_CUDA(h, h->s_outcome_prev.reserve(N + 16));
     UST_CUDA(h, h->sp_outcome.reserve((size_t)max_out + 1));
+  }
+  const size_t S = pods_gather ? h->seg_src.size() : 0;
+  if (pods_gather) {
+    UST_CUDA(h, h->splice_outcome.reserve(N + 16));
+    UST_CUDA(h, h->pr_segs.reserve(2 * S + 1));
+    UST_CUDA(h, h->pr_pods.reserve(2 * S + 1));
+    UST_CUDA(h, h->s_podoff2.reserve(N + 1));
+    UST_CUDA(h, h->s_podflags2.reserve((size_t)new_total + 16));
   }
   if (L) {  // the new lists carry 8 pods of padding for the relayout's 16-byte loads, the new CSR too
     UST_CUDA(h, h->pl_idx.reserve((size_t)L));
@@ -1088,12 +1166,26 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
     UST_CUDA(h, h->outs_sparse.reserve((size_t)max_out));
   }
   drop_resident(h);  // until the patched snapshot has been evaluated
-  for (int64_t k = 0; k < L; k++) h->pod_len[(size_t)pl->node_idx[k]] = pl->pod_off[k + 1] - pl->pod_off[k];
+  if (pods_gather) std::swap(h->pod_len, h->pod_len_next);
+  else for (int64_t k = 0; k < L; k++) h->pod_len[(size_t)pl->node_idx[k]] = pl->pod_off[k + 1] - pl->pod_off[k];
   if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsrev.p, ds_rev, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
   if (L) {
-    UST_CUDA(h, cudaMemcpyAsync(h->pl_idx.p, pl->node_idx, (size_t)L * 8, cudaMemcpyHostToDevice, st));
+    if (!pods_gather) UST_CUDA(h, cudaMemcpyAsync(h->pl_idx.p, pl->node_idx, (size_t)L * 8, cudaMemcpyHostToDevice, st));
     UST_CUDA(h, cudaMemcpyAsync(h->pl_off.p, pl->pod_off, ((size_t)L + 1) * 4, cudaMemcpyHostToDevice, st));
     if (pl->n_pods) UST_CUDA(h, cudaMemcpyAsync(h->pl_flags.p, pl->pod_flags, (size_t)pl->n_pods * 2, cudaMemcpyHostToDevice, st));
+  }
+  if (pods_gather) {  // the run table and the gather of the new CSR, into the second pair
+    long long* segs = h->pr_segs.p;
+    UST_CUDA(h, cudaMemcpyAsync(segs, h->seg_node.data(), (S + 1) * 8, cudaMemcpyHostToDevice, st));
+    if (S) UST_CUDA(h, cudaMemcpyAsync(segs + S + 1, h->seg_src.data(), S * 8, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, cudaMemcpyAsync(h->pr_pods.p, h->seg_pod.data(), (S + 1) * 4, cudaMemcpyHostToDevice, st));
+    int e = ust_launch_pods_reorder((long long)n, (long long)S, segs, h->pr_pods.p, h->s_podoff.p, h->s_podflags.p, h->pl_off.p,
+                                    h->pl_flags.p, (int)new_total, h->s_podoff2.p, h->s_podflags2.p, 8 * h->num_sms, st);
+    if (e) return h->fail(UST_ERR_CUDA, "pod-list reorder kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    h->launches += 2;
+    std::swap(h->s_podoff, h->s_podoff2);
+    std::swap(h->s_podflags, h->s_podflags2);
+  } else if (L) {
     int e;
     if (same_len) {
       e = ust_launch_pods_scatter((long long)L, h->pl_idx.p, h->pl_off.p, h->pl_flags.p, h->s_podoff.p, h->s_podflags.p, 8 * h->num_sms, st);
@@ -1118,9 +1210,10 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
       UST_CUDA(h, cudaMemcpyAsync(off, h->run_off.data(), (NR + 1) * 8, cudaMemcpyHostToDevice, st));
       if (NR) UST_CUDA(h, cudaMemcpyAsync(src, h->run_src.data(), NR * 8, cudaMemcpyHostToDevice, st));
       e = ust_launch_reorder((long long)n, (long long)NR, off, src, in.hot.p, in.flags.p, in.rev.p, in.ds.p, s.hot.p, s.flags.p, s.rev.p,
-                             s.ds.p, h->outs.next.p, h->outs.actions.p, x.hot.p, x.flags.p, x.rev.p, x.ds.p, h->splice_outs.next.p,
-                             h->splice_outs.actions.p, st);
+                             s.ds.p, h->outs.next.p, h->outs.actions.p, pods ? h->s_outcome.p : nullptr, x.hot.p, x.flags.p, x.rev.p,
+                             x.ds.p, h->splice_outs.next.p, h->splice_outs.actions.p, pods ? h->splice_outcome.p : nullptr, st);
       if (e) return h->fail(UST_ERR_CUDA, "reorder kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+      if (pods) std::swap(h->s_outcome, h->splice_outcome);  // the previous outcome in the new order
     } else {
       // a splice keeps its own kernel: the gather kernel measured slower on splices (DESIGN.md §3.4)
       if (R) UST_CUDA(h, cudaMemcpyAsync(h->removed.p, sp->remove_idx, R * 8, cudaMemcpyHostToDevice, st));
@@ -1240,6 +1333,20 @@ int ust_apply_state_delta_pods(ust_handle* h, const ust_policy* policy, const us
   // the pod lists of a shard hold that shard's nodes only; the call keeps to one GPU like the splice and the reorder
   if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_pods runs on one GPU");
   return delta_common(h, policy, nullptr, nullptr, true, lists, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true,
+                      out_next_state, out_actions, out_outcome, max_out, out_idx, n_out, out);
+}
+
+int ust_apply_state_delta_pods_reorder(ust_handle* h, const ust_policy* policy, const ust_reorder* reorder, const ust_pod_lists* lists,
+                                       int64_t n_changed, const int64_t* idx, const uint8_t* state, const uint32_t* flags,
+                                       const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, int64_t max_out,
+                                       int64_t* out_idx, uint8_t* out_next_state, uint16_t* out_actions, uint8_t* out_outcome,
+                                       int64_t* n_out, ust_counters* out) {
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
+  // node indices and pod lists of a shard are its own: a reorder would have to move them on every rank
+  if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_pods_reorder runs on one GPU");
+  return delta_common(h, policy, nullptr, reorder, true, lists, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true,
                       out_next_state, out_actions, out_outcome, max_out, out_idx, n_out, out);
 }
 
@@ -1476,6 +1583,9 @@ int ust_debug_podlut_mismatches(const ust_policy* p) {
 }
 
 long long ust_debug_relaxed_calls(ust_handle* h) { return h ? (long long)h->relaxed_calls : -1; }
+
+// diagnostics: host nanoseconds of the last list-length pass (pods_reorder_segments) of ust_apply_state_delta_pods_reorder
+long long ust_debug_pod_pass_ns(ust_handle* h) { return h ? h->pod_pass_ns : -1; }
 
 // diagnostics (not in include/ust.h): %globaltimer stamps taken by CTA 0 of the last fused launch
 int ust_debug_stamps(ust_handle* h, unsigned long long* out, int n_ctas) {

@@ -183,11 +183,12 @@ int ust_launch_splice(long long n, long long n_rm, const long long* rm, long lon
                       int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, void* stream);
 // new node order of the resident snapshot (ust_apply_state_delta_reorder): the resident columns and the previous
 // outputs, gathered into the o_* arrays (n entries). Run r covers new positions [run_off[r], run_off[r + 1]) and reads old
-// nodes from run_src[r] on, or inserted nodes from -1 - run_src[r] on (run_src[r] < 0); checked by the caller
+// nodes from run_src[r] on, or inserted nodes from -1 - run_src[r] on (run_src[r] < 0); checked by the caller. With `oc`
+// non-null (ust_apply_state_delta_pods_reorder) the previous actuator_outcome is gathered into o_oc as well
 int ust_launch_reorder(long long n, long long n_runs, const long long* run_off, const long long* run_src, const uint8_t* ins_hot,
                        const uint32_t* ins_flags, const int32_t* ins_rev, const int32_t* ins_ds, const uint8_t* hot, const uint32_t* flags,
-                       const int32_t* rev, const int32_t* ds, const uint8_t* next, const uint16_t* act, uint8_t* o_hot, uint32_t* o_flags,
-                       int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, void* stream);
+                       const int32_t* rev, const int32_t* ds, const uint8_t* next, const uint16_t* act, const uint8_t* oc, uint8_t* o_hot,
+                       uint32_t* o_flags, int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, uint8_t* o_oc, void* stream);
 // rollout simulation: the clock of the feedback between two reconciles (include/ust.h, ust_sim_options)
 struct UstSimParams {
   int timed;            // 0: whatever a node waits for has happened by the next reconcile
@@ -218,3 +219,12 @@ int ust_launch_pods_scatter(long long n_lists, const long long* node_idx, const 
 int ust_launch_pods_relayout(long long n, long long n_lists, const long long* node_idx, const int32_t* new_off, const int32_t* shift,
                              const int32_t* off, const uint16_t* flags, const uint16_t* new_flags, int new_total, int32_t* runs,
                              int32_t* o_off, uint16_t* o_flags, int grid, void* stream);
+// the pod-list CSR of the resident pod-list snapshot in a new node order (ust_apply_state_delta_pods_reorder), checked by
+// the caller: n_segs segments of the new snapshot, each a stretch of consecutive old nodes or one new list. segs holds
+// seg_node (n_segs + 1 entries: first new node of each segment, then n) and seg_src (n_segs: first old node, or -1 - k for
+// list k of new_off / new_flags); seg_pods holds pod_start (n_segs + 1: first new pod of each segment, then new_total) and
+// room for n_segs more entries that the first launch fills. New offsets into o_off (n + 1), the new CSR into o_flags
+// (new_total pods + 16 of padding); two launches
+int ust_launch_pods_reorder(long long n, long long n_segs, const long long* segs, int32_t* seg_pods, const int32_t* off,
+                            const uint16_t* flags, const int32_t* new_off, const uint16_t* new_flags, int new_total, int32_t* o_off,
+                            uint16_t* o_flags, int grid, void* stream);

@@ -14,7 +14,8 @@
 // Around it: ust_pod_summary_kernel (pod lists -> one byte per node), ust_build_state*_kernel (BuildState),
 // ust_patch_kernel / ust_splice_kernel / ust_reorder_kernel / ust_feedback_kernel (delta updates, membership changes,
 // new node orders, rollout simulation), ust_pods_scatter_kernel / ust_pods_runs_kernel / ust_pods_relayout_kernel
-// (replaced pod lists), ust_diff_*_kernel (sparse outputs),
+// (replaced pod lists), ust_pods_reorder_runs_kernel / ust_pods_reorder_kernel (pod lists in a new node order),
+// ust_diff_*_kernel (sparse outputs),
 // ust_widen_kernel (packed host format).
 #include <climits>
 
@@ -885,9 +886,11 @@ __global__ void __launch_bounds__(kThreads) ust_splice_kernel(long long n, long 
 // it finds the runs that cover them once, by binary search, and stages their offsets and sources in shared memory
 // (every run is at least one position long, so at most kGatherTile of them meet a tile). Each thread then finds its
 // positions' runs in that range, walking forward from the run of its previous position.
-// 16 B read + 16 B written per node, 16 B per run; a run is read contiguously.
+// 16 B read + 16 B written per node, 16 B per run; a run is read contiguously. OUTCOME (ust_apply_state_delta_pods_reorder):
+// the previous actuator_outcome travels too (1 B more each way; 0xFF for inserted nodes).
 constexpr int kGatherTile = 2048;
 
+template <bool OUTCOME>
 __global__ void __launch_bounds__(kThreads) ust_reorder_kernel(long long n, long long n_runs, const long long* __restrict__ run_off,
                                                                const long long* __restrict__ run_src,
                                                                const uint8_t* __restrict__ ins_hot, const uint32_t* __restrict__ ins_flags,
@@ -895,9 +898,11 @@ __global__ void __launch_bounds__(kThreads) ust_reorder_kernel(long long n, long
                                                                const uint8_t* __restrict__ hot, const uint32_t* __restrict__ flags,
                                                                const int32_t* __restrict__ rev, const int32_t* __restrict__ ds,
                                                                const uint8_t* __restrict__ next, const uint16_t* __restrict__ act,
+                                                               const uint8_t* __restrict__ oc,
                                                                uint8_t* __restrict__ o_hot, uint32_t* __restrict__ o_flags,
                                                                int32_t* __restrict__ o_rev, int32_t* __restrict__ o_ds,
-                                                               uint8_t* __restrict__ o_next, uint16_t* __restrict__ o_act) {
+                                                               uint8_t* __restrict__ o_next, uint16_t* __restrict__ o_act,
+                                                               uint8_t* __restrict__ o_oc) {
   __shared__ long long s_off[kGatherTile];
   __shared__ long long s_src[kGatherTile];
   __shared__ long long s_runs[2];
@@ -934,10 +939,12 @@ __global__ void __launch_bounds__(kThreads) ust_reorder_kernel(long long n, long
       const long long i = src + k;
       o_hot[p] = __ldcs(hot + i); o_flags[p] = __ldcs(flags + i); o_rev[p] = __ldcs(rev + i); o_ds[p] = __ldcs(ds + i);
       o_next[p] = __ldcs(next + i); o_act[p] = __ldcs(act + i);
+      if (OUTCOME) o_oc[p] = __ldcs(oc + i);
     } else {
       const long long i = -1 - src + k;
       o_hot[p] = __ldg(ins_hot + i); o_flags[p] = __ldg(ins_flags + i); o_rev[p] = __ldg(ins_rev + i); o_ds[p] = __ldg(ins_ds + i);
       o_next[p] = 0xFF; o_act[p] = 0;
+      if (OUTCOME) o_oc[p] = 0xFF;
     }
   }
 }
@@ -1087,6 +1094,138 @@ __global__ void __launch_bounds__(kThreads) ust_pods_relayout_kernel(long long n
         while (S[r + 1] <= p) r++;
         const uint16_t* src = ((r0 + r) & 1) ? new_flags : flags;
         w[e >> 1] |= (uint32_t)__ldg(src + R[r] + (p - S[r])) << (16 * (e & 1));
+      }
+      v = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+    *reinterpret_cast<uint4*>(o_flags + q) = v;
+  }
+}
+
+// The pod-list CSR of the resident pod-list snapshot in a new node order, with replaced and inserted lists
+// (ust_apply_state_delta_pods_reorder). The host cuts the new snapshot into S segments, each a stretch of consecutive
+// old nodes or one new list: segment s covers new nodes [seg_node[s], seg_node[s + 1]) and new pods [pod_start[s],
+// pod_start[s + 1]) (seg_node[S] = n, pod_start[S] = new_total), read from old nodes seg_src[s], seg_src[s] + 1, ...
+// (seg_src >= 0) or from new list -1 - seg_src[s]. ust_pods_reorder_runs_kernel finds each segment's first source pod
+// (pod_src: old pod off[seg_src], or -1 - new_off[k] for list k); ust_pods_reorder_kernel then writes the n + 1 new offsets
+// and the new pod_flags into the second CSR pair in one pass, as ust_pods_relayout_kernel does.
+constexpr int kReorderOffTile = 1024;  // offsets per CTA: a full shuffle puts one segment on every node
+
+__global__ void __launch_bounds__(kThreads) ust_pods_reorder_runs_kernel(long long n_segs, const long long* __restrict__ seg_src,
+                                                                         const int32_t* __restrict__ off,
+                                                                         const int32_t* __restrict__ new_off,
+                                                                         int32_t* __restrict__ pod_src) {
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long s = (long long)blockIdx.x * kThreads + threadIdx.x; s < n_segs; s += stride) {
+    const long long src = __ldg(seg_src + s);
+    pod_src[s] = src >= 0 ? __ldg(off + src) : -1 - __ldg(new_off + (-1 - src));
+  }
+}
+
+union PodsReorderSmem {
+  struct { int32_t start[kRelayRuns + 1]; int32_t src[kRelayRuns]; } pods;
+  struct { long long node[kReorderOffTile]; long long src[kReorderOffTile]; int32_t start[kReorderOffTile]; int32_t psrc[kReorderOffTile]; } offs;
+};
+
+// CTAs [0, pod_ctas) gather the new pod_flags by tiles of kRelayTile new positions; the CTAs after them write the n + 1
+// new offsets by tiles of kReorderOffTile nodes. Both search their tile's segments once and stage them in shared memory.
+// 2 B read + 2 B written per pod, 8 B per node, a few dozen bytes per segment.
+__global__ void __launch_bounds__(kThreads) ust_pods_reorder_kernel(long long n, long long n_segs, const long long* __restrict__ seg_node,
+                                                                    const long long* __restrict__ seg_src,
+                                                                    const int32_t* __restrict__ pod_start,
+                                                                    const int32_t* __restrict__ pod_src, const int32_t* __restrict__ off,
+                                                                    const uint16_t* __restrict__ flags, const uint16_t* __restrict__ new_flags,
+                                                                    int32_t* __restrict__ o_off, uint16_t* __restrict__ o_flags,
+                                                                    int new_total, int pod_ctas) {
+  __shared__ __align__(16) PodsReorderSmem sm;
+  __shared__ long long s_bounds[2];
+  const int t = threadIdx.x;
+  if ((int)blockIdx.x >= pod_ctas) {
+    // ---- offsets: node i of segment s takes pod_start[s] + off[seg_src[s] + i - seg_node[s]] - pod_src[s] (old nodes) or
+    // pod_start[s] (a new list); node n takes new_total
+    const long long b0 = (long long)(blockIdx.x - pod_ctas) * kReorderOffTile;
+    const long long b1 = b0 + kReorderOffTile < n ? b0 + kReorderOffTile : n;  // nodes [b0, b1) of [0, n)
+    if (b1 > b0) {
+      if (t < 2) {  // the last segment that starts at or before b0 (t = 0) / b1 - 1 (t = 1)
+        const long long v = t ? b1 - 1 : b0;
+        long long lo = 0, hi = n_segs;
+        while (hi - lo > 1) {
+          const long long mid = (lo + hi) >> 1;
+          if (__ldg(seg_node + mid) <= v) lo = mid; else hi = mid;
+        }
+        s_bounds[t] = lo;
+      }
+      __syncthreads();
+      const long long s0 = s_bounds[0];
+      const int ns = (int)(s_bounds[1] - s0 + 1);  // every segment holds a node: at most kReorderOffTile of them
+      for (int j = t; j < ns; j += kThreads) {
+        sm.offs.node[j] = __ldg(seg_node + s0 + j);
+        sm.offs.src[j] = __ldg(seg_src + s0 + j);
+        sm.offs.start[j] = __ldg(pod_start + s0 + j);
+        sm.offs.psrc[j] = __ldg(pod_src + s0 + j);
+      }
+      __syncthreads();
+      int r = 0;
+      for (int j = t; j < (int)(b1 - b0); j += kThreads) {
+        const long long i = b0 + j;
+        int hi = ns;
+        while (hi - r > 1) {
+          const int mid = (r + hi) >> 1;
+          if (sm.offs.node[mid] <= i) r = mid; else hi = mid;
+        }
+        const long long src = sm.offs.src[r];
+        o_off[i] = src >= 0 ? sm.offs.start[r] + (__ldcs(off + src + (i - sm.offs.node[r])) - sm.offs.psrc[r]) : sm.offs.start[r];
+      }
+    }
+    if (b0 <= n && n < b0 + kReorderOffTile && t == 0) o_off[n] = new_total;
+    return;
+  }
+  // ---- pods: the segments that cover new positions [q0, q1) (empty ones included)
+  const int q0 = blockIdx.x * kRelayTile;
+  const int q1 = q0 + kRelayTile < new_total ? q0 + kRelayTile : new_total;
+  if (t < 2) {  // the last segment that starts at or before q0 (t = 0) / q1 - 1 (t = 1)
+    const int v = t ? q1 - 1 : q0;
+    long long lo = 0, hi = n_segs;
+    while (hi - lo > 1) {
+      const long long mid = (lo + hi) >> 1;
+      if (__ldg(pod_start + mid) <= v) lo = mid; else hi = mid;
+    }
+    s_bounds[t] = lo;
+  }
+  __syncthreads();
+  const long long r0 = s_bounds[0];
+  const int nr = (int)(s_bounds[1] - r0 + 1);
+  // empty segments are not bounded by the tile: a tile that meets more of them than fit reads them from global memory
+  const bool staged = nr <= kRelayRuns;
+  if (staged) {
+    for (int j = t; j <= nr; j += kThreads) sm.pods.start[j] = __ldg(pod_start + r0 + j);
+    for (int j = t; j < nr; j += kThreads) sm.pods.src[j] = __ldg(pod_src + r0 + j);
+  }
+  __syncthreads();
+  const int32_t* S = staged ? sm.pods.start : pod_start + r0;
+  const int32_t* R = staged ? sm.pods.src : pod_src + r0;
+  const int chunks = (q1 - q0 + 7) >> 3;
+#pragma unroll 2
+  for (int c = t; c < chunks; c += kThreads) {
+    const int q = q0 + 8 * c;
+    int r = 0, hi = nr;  // the segment that holds q
+    while (hi - r > 1) {
+      const int mid = (r + hi) >> 1;
+      if (S[mid] <= q) r = mid; else hi = mid;
+    }
+    uint4 v;
+    if (q + 8 <= S[r + 1] && q + 8 <= new_total) {  // the chunk lies in one segment: one shifted 16-byte copy
+      const int src = R[r];
+      v = src >= 0 ? pods8_at(flags, src + (q - S[r])) : pods8_at(new_flags, -1 - src + (q - S[r]));
+    } else {  // it straddles segments (or the end of the array): pod by pod
+      uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+      for (int e = 0; e < 8; e++) {
+        const int p = q + e;
+        if (p >= new_total) break;
+        while (S[r + 1] <= p) r++;
+        const int src = R[r];
+        const uint16_t x = src >= 0 ? __ldg(flags + src + (p - S[r])) : __ldg(new_flags + (-1 - src) + (p - S[r]));
+        w[e >> 1] |= (uint32_t)x << (16 * (e & 1));
       }
       v = make_uint4(w[0], w[1], w[2], w[3]);
     }
@@ -1391,12 +1530,17 @@ int ust_launch_splice(long long n, long long n_rm, const long long* rm, long lon
 }
 int ust_launch_reorder(long long n, long long n_runs, const long long* run_off, const long long* run_src, const uint8_t* ins_hot,
                        const uint32_t* ins_flags, const int32_t* ins_rev, const int32_t* ins_ds, const uint8_t* hot, const uint32_t* flags,
-                       const int32_t* rev, const int32_t* ds, const uint8_t* next, const uint16_t* act, uint8_t* o_hot, uint32_t* o_flags,
-                       int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, void* stream) {
+                       const int32_t* rev, const int32_t* ds, const uint8_t* next, const uint16_t* act, const uint8_t* oc, uint8_t* o_hot,
+                       uint32_t* o_flags, int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, uint8_t* o_oc, void* stream) {
   const long long grid = n > 0 ? (n + kGatherTile - 1) / kGatherTile : 1;  // one launch also for the empty snapshot
-  ust_reorder_kernel<<<(unsigned)grid, kThreads, 0, (cudaStream_t)stream>>>(n, n_runs, run_off, run_src, ins_hot, ins_flags, ins_rev,
-                                                                            ins_ds, hot, flags, rev, ds, next, act, o_hot, o_flags,
-                                                                            o_rev, o_ds, o_next, o_act);
+  if (oc)
+    ust_reorder_kernel<true><<<(unsigned)grid, kThreads, 0, (cudaStream_t)stream>>>(n, n_runs, run_off, run_src, ins_hot, ins_flags, ins_rev,
+                                                                                  ins_ds, hot, flags, rev, ds, next, act, oc, o_hot, o_flags,
+                                                                                  o_rev, o_ds, o_next, o_act, o_oc);
+  else
+    ust_reorder_kernel<false><<<(unsigned)grid, kThreads, 0, (cudaStream_t)stream>>>(n, n_runs, run_off, run_src, ins_hot, ins_flags, ins_rev,
+                                                                                   ins_ds, hot, flags, rev, ds, next, act, nullptr, o_hot,
+                                                                                   o_flags, o_rev, o_ds, o_next, o_act, nullptr);
   return (int)cudaGetLastError();
 }
 int ust_launch_pods_scatter(long long n_lists, const long long* node_idx, const int32_t* new_off, const uint16_t* new_flags,
@@ -1419,6 +1563,23 @@ int ust_launch_pods_relayout(long long n, long long n_lists, const long long* no
   const long long off_ctas = n / kOffTile + 1;    // offsets 0..n
   ust_pods_relayout_kernel<<<(unsigned)(pod_ctas + off_ctas), kThreads, 0, st>>>(n, n_lists, node_idx, shift, off, o_off, run_start, run_src,
                                                                                  flags, new_flags, o_flags, new_total, pod_ctas);
+  return (int)cudaGetLastError();
+}
+int ust_launch_pods_reorder(long long n, long long n_segs, const long long* segs, int32_t* seg_pods, const int32_t* off,
+                            const uint16_t* flags, const int32_t* new_off, const uint16_t* new_flags, int new_total, int32_t* o_off,
+                            uint16_t* o_flags, int grid, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long* seg_node = segs;                // n_segs + 1 entries
+  const long long* seg_src = segs + n_segs + 1;    // n_segs entries
+  const int32_t* pod_start = seg_pods;             // n_segs + 1 entries
+  int32_t* pod_src = seg_pods + n_segs + 1;        // n_segs entries
+  const long long want = (n_segs + kThreads - 1) / kThreads;
+  ust_pods_reorder_runs_kernel<<<(unsigned)(want < 1 ? 1 : (want < grid ? want : grid)), kThreads, 0, st>>>(n_segs, seg_src, off, new_off,
+                                                                                                          pod_src);
+  const int pod_ctas = (new_total + kRelayTile - 1) / kRelayTile;
+  const long long off_ctas = n / kReorderOffTile + 1;  // offsets 0..n
+  ust_pods_reorder_kernel<<<(unsigned)(pod_ctas + off_ctas), kThreads, 0, st>>>(n, n_segs, seg_node, seg_src, pod_start, pod_src, off, flags,
+                                                                                new_flags, o_off, o_flags, new_total, pod_ctas);
   return (int)cudaGetLastError();
 }
 int ust_launch_feedback(long long n, uint8_t* hot, uint32_t* flags, int32_t* pod_rev, const int32_t* ds_idx, int n_ds,

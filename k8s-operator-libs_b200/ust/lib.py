@@ -60,6 +60,10 @@ def load():
         lib.ust_apply_state_delta_pods.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.ust_apply_state_delta_pods_reorder.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
+                                                           C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                           C.c_void_p]
         lib.ust_fetch_outputs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         lib.ust_fetch_outputs_pods.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.ust_simulate_rollout.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -79,7 +83,7 @@ def load():
 
 
 EXPORTS = ["ust_abi_version", "ust_create", "ust_destroy", "ust_last_error", "ust_create_error", "ust_launch_count",
-           "ust_host_alloc", "ust_host_free", "ust_apply_state", "ust_apply_state_device", "ust_stream", "ust_apply_state_packed", "ust_apply_state_delta", "ust_apply_state_delta_sparse", "ust_apply_state_delta_splice", "ust_apply_state_delta_reorder", "ust_apply_state_delta_pods", "ust_fetch_outputs", "ust_fetch_outputs_pods", "ust_simulate_rollout", "ust_simulate_rollout_timed", "ust_sync",
+           "ust_host_alloc", "ust_host_free", "ust_apply_state", "ust_apply_state_device", "ust_stream", "ust_apply_state_packed", "ust_apply_state_delta", "ust_apply_state_delta_sparse", "ust_apply_state_delta_splice", "ust_apply_state_delta_reorder", "ust_apply_state_delta_pods", "ust_apply_state_delta_pods_reorder", "ust_fetch_outputs", "ust_fetch_outputs_pods", "ust_simulate_rollout", "ust_simulate_rollout_timed", "ust_sync",
            "ust_build_state", "ust_build_state_uids", "ust_get_unique_id", "ust_comm_init", "ust_comm_set_mode", "ust_table_entry",
            "ust_table_window_shift"]
 
@@ -366,6 +370,49 @@ class Handle:
             int(idx.shape[0]), _p(idx), _p(ch["state"]), _p(ch["flags"]), _p(ch["pod_rev"]), _p(ch["ds_idx"]),
             int(ds_rev.shape[0]), _p(ds_rev), C.c_int64(int(max_out)), _p(out[0]), _p(out[1]), _p(out[2]), _p(out[3]),
             C.addressof(n_out), C.addressof(cnt))
+        return rc, int(n_out.value), out[0], out[1], out[2], out[3], cnt.as_dict()
+
+    def apply_state_delta_pods_reorder(self, policy, reorder, lists, idx, changed, ds_rev, max_out, out=None):
+        """ust_apply_state_delta_pods_reorder: apply_state_delta_pods after the resident pod-list snapshot took a new node
+        order. `reorder` is None or a dict as for apply_state_delta_reorder, `lists` None or a dict as for
+        apply_state_delta_pods; lists["node_idx"] and `idx` index the reordered snapshot, and every inserted node needs a
+        list. Returns what apply_state_delta_pods returns, in new-index order."""
+        keep = []
+
+        def arr(a, dt):
+            a = np.ascontiguousarray(a, dtype=dt)
+            keep.append(a)
+            return a
+
+        ro = None
+        if reorder is not None:
+            src = arr(reorder.get("run_src", np.zeros(0)), np.int64)
+            ln = arr(reorder.get("run_len", np.zeros(0)), np.int64)
+            ins = {k: arr(reorder[k], dt) if k in reorder else None
+                   for k, dt in (("state", np.uint8), ("flags", np.uint32), ("pod_rev", np.int32), ("ds_idx", np.int32))}
+            n_ins = reorder.get("n_insert", 0 if ins["state"] is None else int(ins["state"].shape[0]))
+            ro = abi.Reorder(int(src.shape[0]), _p(src), _p(ln), int(n_ins), _p(ins["state"]), _p(ins["flags"]),
+                             _p(ins["pod_rev"]), _p(ins["ds_idx"]))
+        pl = None
+        if lists is not None:
+            ni = arr(lists["node_idx"], np.int64)
+            off = arr(lists["pod_off"], np.int32)
+            pf = arr(lists["pod_flags"], np.uint16)
+            pl = abi.PodLists(int(ni.shape[0]), _p(ni), _p(off), _p(pf), int(pf.shape[0]))
+        idx = arr(idx, np.int64)
+        ch = {"state": arr(changed["state"], np.uint8), "flags": arr(changed["flags"], np.uint32),
+              "pod_rev": arr(changed["pod_rev"], np.int32), "ds_idx": arr(changed["ds_idx"], np.int32)}
+        ds_rev = arr(ds_rev, np.int32)
+        if out is None:
+            out = (np.zeros(max_out + 1, np.int64), np.zeros(max_out + 1, np.uint8), np.zeros(max_out + 1, np.uint16),
+                   np.zeros(max_out + 1, np.uint8))
+        n_out = C.c_int64(0)
+        cnt = abi.Counters()
+        rc = self._lib.ust_apply_state_delta_pods_reorder(
+            self._h, C.addressof(policy) if policy is not None else None, C.addressof(ro) if ro is not None else None,
+            C.addressof(pl) if pl is not None else None, int(idx.shape[0]), _p(idx), _p(ch["state"]), _p(ch["flags"]),
+            _p(ch["pod_rev"]), _p(ch["ds_idx"]), int(ds_rev.shape[0]), _p(ds_rev), C.c_int64(int(max_out)), _p(out[0]),
+            _p(out[1]), _p(out[2]), _p(out[3]), C.addressof(n_out), C.addressof(cnt))
         return rc, int(n_out.value), out[0], out[1], out[2], out[3], cnt.as_dict()
 
     def fetch_outputs_pods(self, n):
