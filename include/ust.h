@@ -496,6 +496,42 @@ int ust_build_state_uids(ust_handle* h, int64_t n_pods, const uint8_t* state, co
                          int32_t n_ds, const uint64_t* ds_uid, const int32_t* ds_desired, int32_t* ds_idx_out,
                          ust_counters* out);
 
+/* New order of the resident driver-pod list of n pods, as runs - exactly the run rules of ust_reorder:
+ *   run_src[r] >= 0: old pods run_src[r] .. run_src[r] + run_len[r] - 1;  run_src[r] == -1: the next run_len[r] joined pods */
+typedef struct ust_driver_pod_reorder {
+  int64_t n_runs;
+  const int64_t* run_src;
+  const int64_t* run_len;
+  int64_t n_insert;
+  const uint8_t* state;        /* per joined pod, as in ust_build_state_uids */
+  const uint64_t* owner_uid;   /* per joined pod, 2 x uint64 ((0,0) = no owner reference) */
+} ust_driver_pod_reorder;
+
+/* Delta form of ust_build_state_uids: the driver-pod list stays resident on the device, and a reconcile sends only the pods
+ * that joined, left, moved or changed. The list exists from ust_create and starts empty (n = 0): the first call sends every
+ * pod as one inserted run. One call
+ *   1. applies `reorder` (NULL: the order does not change),
+ *   2. overwrites state / owner_uid of the n_changed pods at idx - distinct indices into the NEW list,
+ *   3. joins and counts the whole list against the DaemonSet table, which is passed in full every call.
+ * Counters, return codes and owner indices are exactly those of ust_build_state_uids on the updated arrays, including
+ * UST_ERR_DS_UNSCHEDULED with error_index. Sparse outputs in new-index order: out_idx[k], out_ds_idx[k] for k < *n_out, for
+ * every joined pod and every pod whose owner index differs from the one the previous call returned for it (wherever it
+ * moved). When *n_out > max_out nothing is written to the out_* arrays and UST_ERR_TRUNCATED is returned (unless
+ * UST_ERR_DS_UNSCHEDULED applies, which keeps its own code): ust_fetch_build_state then returns every owner index.
+ * Residency: a call that produced counters keeps the list resident (UST_ERR_DS_UNSCHEDULED and UST_ERR_TRUNCATED included);
+ * a call that fails after its arguments were accepted empties it. The list lives in device buffers of its own: no other
+ * entry point reads or drops it, and neither of these two touches the ApplyState snapshots or their outputs.
+ * A violated contract (everything ust_apply_state_delta_reorder rejects in its runs, NULL insert arrays with n_insert > 0,
+ * idx duplicated or outside the new list, n_ds < 0, an empty or duplicated DaemonSet UID, max_out < 0, NULL arrays where
+ * counts are non-zero, a new list of 2^31 pods or more) returns UST_ERR_INVALID_ARGUMENT before any device work, with the list left as it was. The checks
+ * cost O(n + n_runs + n_changed + n_ds) host time. */
+int ust_build_state_delta(ust_handle* h, const ust_driver_pod_reorder* reorder /* nullable */,
+                          int64_t n_changed, const int64_t* idx, const uint8_t* state, const uint64_t* owner_uid,
+                          int32_t n_ds, const uint64_t* ds_uid, const int32_t* ds_desired,
+                          int64_t max_out, int64_t* out_idx, int32_t* out_ds_idx, int64_t* n_out, ust_counters* out);
+/* Every owner index of the resident driver-pod list (the last ust_build_state_delta's); n_pods must equal its size. */
+int ust_fetch_build_state(ust_handle* h, int64_t n_pods, int32_t* ds_idx);
+
 /* ---- introspection ----------------------------------------------------------------------------- */
 
 /* The kernel evaluates a node by one lookup in a per-policy table indexed by (state code, 9-bit window

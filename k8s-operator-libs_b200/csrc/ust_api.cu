@@ -224,6 +224,20 @@ struct ust_handle {
   std::vector<int32_t> seg_pod;
   long long pod_pass_ns = 0;  // diagnostics: host time of the last pods_reorder_segments
   DevBuf<int32_t> sim_entered, sim_wait, sim_valid;  // timed rollout simulation: per-node clocks
+  // the resident driver-pod list of ust_build_state_delta (bs_n pods, 0 until the first call; nothing else reads or drops
+  // it): state bytes, owner UIDs and the owner indices of the last call in `bs`. `bs2` is the gather target of a reorder
+  // (hot / uid allocated on the first reorder; swapped with `bs` afterwards); bs2.owner receives a call's owner indices
+  // (swapped with bs.owner afterwards). The joined and the overwritten pods as uploaded; the sparse owner indices.
+  struct PodList {
+    DevBuf<uint8_t> hot;
+    DevBuf<uint64_t> uid;
+    DevBuf<int32_t> owner;
+  };
+  PodList bs, bs2;
+  int64_t bs_n = 0;
+  DevBuf<uint8_t> bs_ins_hot, bs_chg_hot;
+  DevBuf<uint64_t> bs_ins_uid, bs_chg_uid;
+  DevBuf<int32_t> bs_out_ds;
 
   // multi-GPU
   int rank = 0, world = 1, comm_mode = 0;
@@ -744,6 +758,44 @@ static int build_state_launch(ust_handle* h, int64_t n_pods, int32_t n_ds, cudaS
   return UST_OK;
 }
 
+// The DaemonSet map of BuildState's owner join, keyed by UID (common_manager.go:181-185): an open-addressing table at load
+// factor <= 1/4 (ust_uid_hash, linear probing, (0, 0) = empty slot) and the DaemonSet index of every slot. The UIDs must be
+// non-empty and distinct.
+struct DsTable {
+  size_t slots = 8;
+  std::vector<uint64_t> tab;
+  std::vector<int32_t> idx;
+};
+static int ds_table(ust_handle* h, int32_t n_ds, const uint64_t* ds_uid, DsTable* t) {
+  size_t& slots = t->slots;
+  while (slots < 4 * (size_t)n_ds) slots <<= 1;
+  t->tab.assign(2 * slots, 0);
+  t->idx.assign(slots, -2);
+  uint64_t* tab = t->tab.data();
+  for (int32_t d = 0; d < n_ds; d++) {
+    const uint64_t x = ds_uid[2 * (size_t)d], y = ds_uid[2 * (size_t)d + 1];
+    if ((x | y) == 0) return h->fail(UST_ERR_INVALID_ARGUMENT, "DaemonSet %d has an empty UID", (int)d);
+    size_t s = ust_uid_hash(x, y) & (slots - 1);
+    while ((tab[2 * s] | tab[2 * s + 1]) != 0) {
+      if (tab[2 * s] == x && tab[2 * s + 1] == y)
+        return h->fail(UST_ERR_INVALID_ARGUMENT, "DaemonSets %d and %d share a UID", (int)t->idx[s], (int)d);
+      s = (s + 1) & (slots - 1);
+    }
+    tab[2 * s] = x; tab[2 * s + 1] = y; t->idx[s] = d;
+  }
+  return UST_OK;
+}
+// the table and DesiredNumberScheduled per DaemonSet, enqueued on `st` (the caller synchronises before `t` goes)
+static int upload_ds_table(ust_handle* h, const DsTable& t, int32_t n_ds, const int32_t* ds_desired, cudaStream_t st) {
+  UST_CUDA(h, h->s_dsuid.reserve(2 * t.slots));
+  UST_CUDA(h, h->s_dsorder.reserve(t.slots));
+  UST_CUDA(h, h->s_dsdesired.reserve((size_t)n_ds + 1));
+  UST_CUDA(h, cudaMemcpyAsync(h->s_dsuid.p, t.tab.data(), t.slots * 16, cudaMemcpyHostToDevice, st));
+  UST_CUDA(h, cudaMemcpyAsync(h->s_dsorder.p, t.idx.data(), t.slots * 4, cudaMemcpyHostToDevice, st));
+  if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsdesired.p, ds_desired, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
+  return UST_OK;
+}
+
 extern "C" {
 
 int ust_abi_version(void) { return UST_ABI_VERSION; }
@@ -939,25 +991,24 @@ static bool mark_bits(uint64_t* w, long long a, long long len, bool set) {
   return true;
 }
 
-// A reorder checked in full and turned into runs, O(n + n_runs): a bitmap over the old snapshot finds old nodes that two
-// runs name. Sets *n_new to the new snapshot's size.
-static int reorder_runs(ust_handle* h, const ust_reorder* ro, int64_t n_old, int64_t* n_new) {
-  if (ro->n_runs < 0 || ro->n_insert < 0 || (ro->n_runs > 0 && (!ro->run_src || !ro->run_len)) ||
-      (ro->n_insert > 0 && (!ro->state || !ro->flags || !ro->pod_rev || !ro->ds_idx)))
-    return h->fail(UST_ERR_INVALID_ARGUMENT, "bad reorder");
+// A reorder (n_runs runs run_src / run_len over n_old old entries, n_insert inserted ones) checked in full and turned into
+// runs, O(n + n_runs): a bitmap over the old snapshot finds old nodes that two runs name. Sets *n_new to the new size.
+static int reorder_runs(ust_handle* h, int64_t n_runs, const int64_t* run_src, const int64_t* run_len, int64_t n_insert, int64_t n_old,
+                        int64_t* n_new) {
+  if (n_runs < 0 || n_insert < 0 || (n_runs > 0 && (!run_src || !run_len))) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad reorder");
   const size_t words = ((size_t)n_old + 63) / 64;
   if (h->run_seen.size() < words) h->run_seen.resize(words, 0);
   clear_runs(h);
   int rc = UST_OK;
   int64_t marked = 0, ins = 0;  // runs whose old nodes are marked; inserted nodes taken
-  for (int64_t r = 0; r < ro->n_runs && rc == UST_OK; r++) {
-    const long long src = ro->run_src[r], len = ro->run_len[r];
+  for (int64_t r = 0; r < n_runs && rc == UST_OK; r++) {
+    const long long src = run_src[r], len = run_len[r];
     if (len < 1 || src < -1)
       rc = h->fail(UST_ERR_INVALID_ARGUMENT, "reorder: run %lld has source %lld and length %lld", (long long)r, src, len);
     else if (len >= (1LL << 40) - h->run_off.back())
       rc = h->fail(UST_ERR_INVALID_ARGUMENT, "too many nodes");
-    else if (src < 0 && len > ro->n_insert - ins)
-      rc = h->fail(UST_ERR_INVALID_ARGUMENT, "reorder: the inserted runs take more than the %lld inserted nodes", (long long)ro->n_insert);
+    else if (src < 0 && len > n_insert - ins)
+      rc = h->fail(UST_ERR_INVALID_ARGUMENT, "reorder: the inserted runs take more than the %lld inserted nodes", (long long)n_insert);
     else if (src >= 0 && (src >= n_old || len > n_old - src))
       rc = h->fail(UST_ERR_INVALID_ARGUMENT, "reorder: run %lld (old nodes %lld + %lld) leaves the snapshot of %lld nodes", (long long)r, src,
                    len, (long long)n_old);
@@ -971,9 +1022,9 @@ static int reorder_runs(ust_handle* h, const ust_reorder* ro, int64_t n_old, int
     }
   }
   for (int64_t r = 0; r < marked; r++)  // the bitmap is all zero again
-    if (ro->run_src[r] >= 0) mark_bits(h->run_seen.data(), ro->run_src[r], ro->run_len[r], false);
-  if (rc == UST_OK && ins != ro->n_insert)
-    rc = h->fail(UST_ERR_INVALID_ARGUMENT, "reorder: the inserted runs take %lld of the %lld inserted nodes", (long long)ins, (long long)ro->n_insert);
+    if (run_src[r] >= 0) mark_bits(h->run_seen.data(), run_src[r], run_len[r], false);
+  if (rc == UST_OK && ins != n_insert)
+    rc = h->fail(UST_ERR_INVALID_ARGUMENT, "reorder: the inserted runs take %lld of the %lld inserted nodes", (long long)ins, (long long)n_insert);
   *n_new = h->run_off.back();
   return rc;
 }
@@ -1052,7 +1103,8 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
   const int32_t *ins_rev = nullptr, *ins_ds = nullptr;
   bool gather = false;
   if (ro) {
-    if (int rc = reorder_runs(h, ro, n_old, &n)) return rc;
+    if (ro->n_insert > 0 && (!ro->state || !ro->flags || !ro->pod_rev || !ro->ds_idx)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad reorder");
+    if (int rc = reorder_runs(h, ro->n_runs, ro->run_src, ro->run_len, ro->n_insert, n_old, &n)) return rc;
     gather = true;
     n_ins = ro->n_insert;
     ins_state = ro->state; ins_flags = ro->flags; ins_rev = ro->pod_rev; ins_ds = ro->ds_idx;
@@ -1511,22 +1563,8 @@ int ust_build_state_uids(ust_handle* h, int64_t n_pods, const uint8_t* state, co
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   if (n_pods < 0 || (n_pods > 0 && (!state || !owner_uid || !ds_idx_out)) || n_ds < 0 || (n_ds > 0 && (!ds_uid || !ds_desired)))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
-  // the DaemonSet map is keyed by UID (common_manager.go:181-185): an open-addressing table at load factor <= 1/4
-  size_t slots = 8;
-  while (slots < 4 * (size_t)n_ds) slots <<= 1;
-  std::vector<uint64_t> tab(2 * slots, 0);
-  std::vector<int32_t> tab_idx(slots, -2);
-  for (int32_t d = 0; d < n_ds; d++) {
-    const uint64_t x = ds_uid[2 * (size_t)d], y = ds_uid[2 * (size_t)d + 1];
-    if ((x | y) == 0) return h->fail(UST_ERR_INVALID_ARGUMENT, "DaemonSet %d has an empty UID", (int)d);
-    size_t s = ust_uid_hash(x, y) & (slots - 1);
-    while ((tab[2 * s] | tab[2 * s + 1]) != 0) {
-      if (tab[2 * s] == x && tab[2 * s + 1] == y)
-        return h->fail(UST_ERR_INVALID_ARGUMENT, "DaemonSets %d and %d share a UID", (int)tab_idx[s], (int)d);
-      s = (s + 1) & (slots - 1);
-    }
-    tab[2 * s] = x; tab[2 * s + 1] = y; tab_idx[s] = d;
-  }
+  DsTable tab;
+  if (int rc = ds_table(h, n_ds, ds_uid, &tab)) return rc;
   drop_resident(h);  // shares the staging arrays
   UST_CUDA(h, cudaSetDevice(h->device));
   StreamDrain drain(h);
@@ -1535,23 +1573,147 @@ int ust_build_state_uids(ust_handle* h, int64_t n_pods, const uint8_t* state, co
   UST_CUDA(h, h->staged.hot.reserve(N + 16));
   UST_CUDA(h, h->staged.ds.reserve(N + 4));
   UST_CUDA(h, h->s_uid.reserve(2 * N + 2));
-  UST_CUDA(h, h->s_dsuid.reserve(2 * slots));
-  UST_CUDA(h, h->s_dsorder.reserve(slots));
-  UST_CUDA(h, h->s_dsdesired.reserve((size_t)n_ds + 1));
   if (N) {
     UST_CUDA(h, cudaMemcpyAsync(h->staged.hot.p, state, N, cudaMemcpyHostToDevice, st));
     UST_CUDA(h, cudaMemcpyAsync(h->s_uid.p, owner_uid, N * 16, cudaMemcpyHostToDevice, st));
   }
-  UST_CUDA(h, cudaMemcpyAsync(h->s_dsuid.p, tab.data(), slots * 16, cudaMemcpyHostToDevice, st));
-  UST_CUDA(h, cudaMemcpyAsync(h->s_dsorder.p, tab_idx.data(), slots * 4, cudaMemcpyHostToDevice, st));
-  if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsdesired.p, ds_desired, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
+  if (int rc = upload_ds_table(h, tab, n_ds, ds_desired, st)) return rc;
   int rc = build_state_launch(h, n_pods, n_ds, st, [&](int grid) {
-    return ust_launch_build_state_uids(n_pods, h->staged.hot.p, h->s_uid.p, n_ds, h->s_dsuid.p, h->s_dsorder.p, (int)slots,
+    return ust_launch_build_state_uids(n_pods, h->staged.hot.p, h->s_uid.p, n_ds, h->s_dsuid.p, h->s_dsorder.p, (int)tab.slots,
                                        h->s_dsdesired.p, h->staged.ds.p, h->ds_count.p, h->ws, h->counters_dev, grid, st);
   });
   if (rc) return rc;
   if (N) UST_CUDA(h, cudaMemcpyAsync(ds_idx_out, h->staged.ds.p, N * 4, cudaMemcpyDeviceToHost, st));
-  return finish_with_counters(h, st, out);  // synchronises the stream: `tab` / `tab_idx` outlive their copies
+  return finish_with_counters(h, st, out);  // synchronises the stream: the table outlives its copies
+}
+
+int ust_build_state_delta(ust_handle* h, const ust_driver_pod_reorder* reorder, int64_t n_changed, const int64_t* idx,
+                          const uint8_t* state, const uint64_t* owner_uid, int32_t n_ds, const uint64_t* ds_uid,
+                          const int32_t* ds_desired, int64_t max_out, int64_t* out_idx, int32_t* out_ds_idx, int64_t* n_out,
+                          ust_counters* out) {
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
+  // the new order and every argument, checked in full before anything is touched
+  const int64_t n_old = h->bs_n;
+  int64_t n = n_old;
+  if (reorder) {
+    if (reorder->n_insert > 0 && (!reorder->state || !reorder->owner_uid)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad reorder");
+    if (int rc = reorder_runs(h, reorder->n_runs, reorder->run_src, reorder->run_len, reorder->n_insert, n_old, &n)) return rc;
+  }
+  // the tile offsets of the sparse outputs are 32-bit
+  if (n >= (1LL << 31)) return h->fail(UST_ERR_INVALID_ARGUMENT, "too many pods: the driver-pod list holds fewer than 2^31");
+  if (n_changed < 0 || (n_changed > 0 && (!idx || !state || !owner_uid)) || max_out < 0 || !n_out ||
+      (max_out > 0 && (!out_idx || !out_ds_idx)))
+    return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
+  if (n_ds < 0 || (n_ds > 0 && (!ds_uid || !ds_desired))) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad DaemonSet table");
+  {  // idx: distinct indices into the new list (the reorder's bitmap, all zero again afterwards)
+    const size_t words = ((size_t)n + 63) / 64;
+    if (h->run_seen.size() < words) h->run_seen.resize(words, 0);
+    int64_t k = 0;
+    int rc = UST_OK;
+    for (; k < n_changed; k++) {
+      if (idx[k] < 0 || idx[k] >= n) {
+        rc = h->fail(UST_ERR_INVALID_ARGUMENT, "changed pod %lld has index %lld outside the list of %lld pods", (long long)k, (long long)idx[k], (long long)n);
+        break;
+      }
+      if (!mark_bits(h->run_seen.data(), idx[k], 1, true)) {
+        rc = h->fail(UST_ERR_INVALID_ARGUMENT, "changed pod %lld: index %lld is named twice", (long long)k, (long long)idx[k]);
+        break;
+      }
+    }
+    for (int64_t j = 0; j < k; j++) mark_bits(h->run_seen.data(), idx[j], 1, false);
+    if (rc) return rc;
+  }
+  DsTable tab;
+  if (int rc = ds_table(h, n_ds, ds_uid, &tab)) return rc;
+  h->bs_n = 0;  // empty until the call has produced counters
+  UST_CUDA(h, cudaSetDevice(h->device));
+  StreamDrain drain(h);
+  cudaStream_t st = h->stream;
+  const size_t N = (size_t)n, M = (size_t)n_changed, NR = h->run_src.size();
+  const size_t I = reorder ? (size_t)reorder->n_insert : 0;
+  if (reorder) {  // the new order, gathered into the second set, which becomes the resident one
+    UST_CUDA(h, h->bs2.hot.reserve(N + 16));
+    UST_CUDA(h, h->bs2.uid.reserve(2 * N + 2));
+    UST_CUDA(h, h->bs2.owner.reserve(N + 4));
+    UST_CUDA(h, h->runs.reserve(2 * NR + 2));
+    UST_CUDA(h, h->bs_ins_hot.reserve(I + 1));
+    UST_CUDA(h, h->bs_ins_uid.reserve(2 * I + 2));
+    long long* off = h->runs.p;
+    long long* src = h->runs.p + NR + 1;
+    UST_CUDA(h, cudaMemcpyAsync(off, h->run_off.data(), (NR + 1) * 8, cudaMemcpyHostToDevice, st));
+    if (NR) UST_CUDA(h, cudaMemcpyAsync(src, h->run_src.data(), NR * 8, cudaMemcpyHostToDevice, st));
+    if (I) {
+      UST_CUDA(h, cudaMemcpyAsync(h->bs_ins_hot.p, reorder->state, I, cudaMemcpyHostToDevice, st));
+      UST_CUDA(h, cudaMemcpyAsync(h->bs_ins_uid.p, reorder->owner_uid, I * 16, cudaMemcpyHostToDevice, st));
+    }
+    int e = ust_launch_build_state_reorder((long long)n, (long long)NR, off, src, h->bs_ins_hot.p, h->bs_ins_uid.p, h->bs.hot.p,
+                                           h->bs.uid.p, h->bs.owner.p, h->bs2.hot.p, h->bs2.uid.p, h->bs2.owner.p, st);
+    if (e) return h->fail(UST_ERR_CUDA, "driver-pod reorder kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    h->launches += 1;
+    std::swap(h->bs, h->bs2);
+  } else {  // same size as before: no-ops once the list holds pods
+    UST_CUDA(h, h->bs.hot.reserve(N + 16));
+    UST_CUDA(h, h->bs.uid.reserve(2 * N + 2));
+    UST_CUDA(h, h->bs.owner.reserve(N + 4));
+  }
+  UST_CUDA(h, h->bs2.owner.reserve(N + 4));  // this call's owner indices
+  if (M) {
+    UST_CUDA(h, h->changed.idx.reserve(M + 1));
+    UST_CUDA(h, h->bs_chg_hot.reserve(M + 1));
+    UST_CUDA(h, h->bs_chg_uid.reserve(2 * M + 2));
+    static_assert(sizeof(long long) == sizeof(int64_t), "index width");
+    UST_CUDA(h, cudaMemcpyAsync(h->changed.idx.p, idx, M * 8, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, cudaMemcpyAsync(h->bs_chg_hot.p, state, M, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, cudaMemcpyAsync(h->bs_chg_uid.p, owner_uid, M * 16, cudaMemcpyHostToDevice, st));
+    int e = ust_launch_build_state_patch((long long)M, h->changed.idx.p, h->bs_chg_hot.p, h->bs_chg_uid.p, h->bs.hot.p, h->bs.uid.p, st);
+    if (e) return h->fail(UST_ERR_CUDA, "driver-pod patch kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+    h->launches += 1;
+  }
+  const int tiles = ust_build_state_tiles((long long)n);
+  UST_CUDA(h, h->sp_blocks.reserve((size_t)tiles + 1));
+  UST_CUDA(h, h->sp_idx.reserve((size_t)max_out + 1));
+  UST_CUDA(h, h->bs_out_ds.reserve((size_t)max_out + 1));
+  if (int rc = upload_ds_table(h, tab, n_ds, ds_desired, st)) return rc;
+  int rc = build_state_launch(h, n, n_ds, st, [&](int grid) {
+    return ust_launch_build_state_delta((long long)n, h->bs.hot.p, h->bs.uid.p, n_ds, h->s_dsuid.p, h->s_dsorder.p, (int)tab.slots,
+                                        h->s_dsdesired.p, h->bs.owner.p, h->bs2.owner.p, h->sp_blocks.p, h->ds_count.p, h->ws,
+                                        h->counters_dev, grid, st);
+  });
+  if (rc) return rc;
+  int e = ust_launch_build_state_write((long long)n, h->bs2.owner.p, h->bs.owner.p, h->sp_blocks.p, h->sp_count_dev, (long long)max_out,
+                                       h->sp_idx.p, h->bs_out_ds.p, st);
+  if (e) return h->fail(UST_ERR_CUDA, "driver-pod diff kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+  h->launches += tiles > 0 ? 2 : 1;
+  UST_CUDA(h, cudaMemcpyAsync(h->sp_count_host, h->sp_count_dev, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  UST_CUDA(h, cudaStreamSynchronize(st));
+  const int64_t cnt = *h->sp_count_host;
+  *n_out = cnt;
+  if (cnt <= max_out && cnt > 0) {
+    UST_CUDA(h, cudaMemcpyAsync(out_idx, h->sp_idx.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, st));
+    UST_CUDA(h, cudaMemcpyAsync(out_ds_idx, h->bs_out_ds.p, (size_t)cnt * 4, cudaMemcpyDeviceToHost, st));
+  }
+  rc = finish_with_counters(h, st, out);
+  if (rc == UST_ERR_CUDA) return rc;
+  std::swap(h->bs.owner, h->bs2.owner);  // this call's owner indices are the previous ones of the next call
+  h->bs_n = n;
+  if (rc == UST_OK && cnt > max_out)
+    return h->fail(UST_ERR_TRUNCATED, "%lld owner indices changed, the caller's arrays hold %lld: fetch them with ust_fetch_build_state",
+                   (long long)cnt, (long long)max_out);
+  return rc;
+}
+
+int ust_fetch_build_state(ust_handle* h, int64_t n_pods, int32_t* ds_idx) {
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
+  if (n_pods != h->bs_n) return h->fail(UST_ERR_INVALID_ARGUMENT, "the resident driver-pod list holds %lld pods, not %lld", (long long)h->bs_n, (long long)n_pods);
+  if (n_pods > 0 && !ds_idx) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
+  UST_CUDA(h, cudaSetDevice(h->device));
+  if (n_pods) UST_CUDA(h, cudaMemcpyAsync(ds_idx, h->bs.owner.p, (size_t)n_pods * 4, cudaMemcpyDeviceToHost, h->stream));
+  UST_CUDA(h, cudaStreamSynchronize(h->stream));
+  return UST_OK;
 }
 
 uint32_t ust_table_entry(const ust_policy* policy, unsigned state_code, uint32_t w) {

@@ -173,6 +173,22 @@ static inline unsigned ust_uid_hash(unsigned long long x, unsigned long long y) 
 int ust_launch_build_state_uids(long long n, const uint8_t* hot, const void* owner_uid, int n_ds, const void* ds_tab,
                                 const int32_t* ds_tab_idx, int tab_slots, const int32_t* ds_desired, int32_t* ds_idx_out,
                                 unsigned long long* ds_count, UstWorkspace* ws, ust_counters* out, int grid, void* stream);
+// resident driver-pod list (ust_build_state_delta): the join + count + diff pass and the finish kernel (`prev` holds each
+// pod's previous owner index, `cur` receives the new one, tile_count one changed count per kBuildTile pods), then the scan
+// of the tile counts and the ordered write of the changed (index, owner index) pairs, at most `cap` of them (four launches)
+int ust_launch_build_state_delta(long long n, const uint8_t* hot, const void* owner_uid, int n_ds, const void* ds_tab,
+                                 const int32_t* ds_tab_idx, int tab_slots, const int32_t* ds_desired, const int32_t* prev,
+                                 int32_t* cur, unsigned int* tile_count, unsigned long long* ds_count, UstWorkspace* ws,
+                                 ust_counters* out, int grid, void* stream);
+int ust_launch_build_state_write(long long n, const int32_t* cur, const int32_t* prev, unsigned int* tile_count, long long* n_out,
+                                 long long cap, long long* out_idx, int32_t* out_ds, void* stream);
+int ust_build_state_tiles(long long n);
+// the driver-pod list in a new order (runs as for ust_launch_reorder), inserted pods with previous owner index INT32_MIN
+int ust_launch_build_state_reorder(long long n, long long n_runs, const long long* run_off, const long long* run_src,
+                                   const uint8_t* ins_hot, const void* ins_uid, const uint8_t* hot, const void* uid,
+                                   const int32_t* prev, uint8_t* o_hot, void* o_uid, int32_t* o_prev, void* stream);
+int ust_launch_build_state_patch(long long m, const long long* idx, const uint8_t* state, const void* uid, uint8_t* hot_out,
+                                 void* uid_out, void* stream);
 int ust_launch_patch(long long m, const long long* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
                      const int32_t* ds_idx, uint8_t* hot_out, uint32_t* flags_out, int32_t* rev_out, int32_t* ds_out, void* stream);
 // membership splice (ust_apply_state_delta_splice): the resident columns and the previous outputs, rewritten in the new node

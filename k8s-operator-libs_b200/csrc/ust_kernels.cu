@@ -755,6 +755,207 @@ __global__ void ust_build_state_finish_kernel(int n_ds, const int32_t* ds_desire
   for (int d = 0; d < n_ds; d++) ds_count[d] = 0;
 }
 
+// The resident driver-pod list of ust_build_state_delta. The join and the counts are those of ust_build_state_uid_kernel<true>
+// (same table, same counters, same finish kernel); the pass also compares each pod's owner index with the previous call's
+// and works in fixed tiles of kBuildTile pods, so that the changed count of every tile comes out of it: the scan of
+// ust_diff_scan_kernel and ust_build_state_write_kernel then compact the changed pods in index order. 21 B read + 4 B
+// written per pod here, 8 B read per pod by the write pass.
+constexpr int kBuildTile = 4096;  // pods per tile: 16 per thread
+
+__global__ void __launch_bounds__(kThreads) ust_build_state_delta_kernel(long long n, const uint8_t* __restrict__ hot,
+                                                                         const ulonglong2* __restrict__ owner, int n_ds,
+                                                                         const ulonglong2* __restrict__ ds_tab,
+                                                                         const int32_t* __restrict__ ds_tab_idx, int tab_slots,
+                                                                         const int32_t* __restrict__ prev, int32_t* __restrict__ cur,
+                                                                         unsigned int* __restrict__ tile_count,
+                                                                         unsigned long long* ds_count, UstWorkspace* ws) {
+  __shared__ ulonglong2 tab[kUidTabSmem];
+  __shared__ int ord[kUidTabSmem];
+  __shared__ unsigned int cnt_ds[kUidTabSmem / 4];
+  __shared__ unsigned long long inc[256];
+  __shared__ unsigned int cnt[16];
+  __shared__ unsigned int tile_changed;
+  const int t = threadIdx.x;
+  const bool in_smem = tab_slots <= kUidTabSmem;  // then n_ds <= kUidTabSmem / 4 too
+  if (in_smem) {
+    for (int i = t; i < tab_slots; i += kThreads) { tab[i] = ds_tab[i]; ord[i] = ds_tab_idx[i]; }
+    for (int i = t; i < n_ds; i += kThreads) cnt_ds[i] = 0;
+  }
+  {
+    const unsigned b = t, code = b & 15u;
+    unsigned long long v = 0;
+    if (code < 14) {
+      v = 1ull << (4 * code);
+      if (b & (UST_HOT_UNSCHEDULABLE | UST_HOT_NOT_READY)) v |= 1ull << 56;
+      if (code == UST_STATE_UPGRADE_REQUIRED && !(b & UST_HOT_SKIP)) v |= 1ull << 60;
+    }
+    inc[b] = v;
+  }
+  if (t < 16) cnt[t] = 0;
+  if (t == 0) tile_changed = 0;
+  __syncthreads();
+  const ulonglong2* table = in_smem ? tab : ds_tab;
+  const int* order = in_smem ? ord : ds_tab_idx;
+  const unsigned slot_mask = (unsigned)tab_slots - 1u;
+  uint32_t B[4] = {0, 0, 0, 0}, lo = 0, hi = 0;
+  int pending = 0;
+  long long excluded = 0;
+  unsigned long long dsl = 0;
+  auto spill = [&]() {
+    widen(lo, hi, B);
+#pragma unroll
+    for (int f = 0; f < 16; f++) {
+      const unsigned v = p1_field(B, f);
+      if (v) atomicAdd(&cnt[f], v);
+    }
+    if (dsl) {
+#pragma unroll
+      for (int q = 0; q < 8; q++) {
+        const unsigned v = (unsigned)(dsl >> (8 * q)) & 0xFFu;
+        if (v) atomicAdd(&cnt_ds[q], v);
+      }
+      dsl = 0;
+    }
+    B[0] = B[1] = B[2] = B[3] = 0;
+    pending = 0;
+  };
+  constexpr int kU = 4;
+  const long long tiles = (n + kBuildTile - 1) / kBuildTile;
+  for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {  // CTA-uniform trip counts
+    unsigned changed = 0;
+    for (int j = 0; j < kBuildTile; j += kThreads * kU) {
+      const long long i0 = tile * kBuildTile + j;
+      ulonglong2 u[kU];
+      unsigned hb[kU];
+      int pv[kU];
+#pragma unroll
+      for (int k = 0; k < kU; k++) {
+        const long long i = i0 + (long long)k * kThreads + t;
+        u[k] = make_ulonglong2(0ull, 0ull);
+        hb[k] = UST_STATE_EXCLUDED;
+        pv[k] = 0;
+        if (i < n) { u[k] = __ldcs(owner + i); hb[k] = __ldg(hot + i); pv[k] = __ldcs(prev + i); }
+      }
+#pragma unroll
+      for (int k = 0; k < kU; k++) {
+        const long long i = i0 + (long long)k * kThreads + t;
+        const bool valid = i < n;
+        int d = -2;
+        if (valid) {
+          if ((u[k].x | u[k].y) == 0ull) {
+            d = -1;  // IsOrphanedPod
+          } else {
+            unsigned slot = ust_uid_hash(u[k].x, u[k].y) & slot_mask;
+            for (;;) {
+              const ulonglong2 e = table[slot];
+              if (e.x == u[k].x && e.y == u[k].y) { d = order[slot]; break; }
+              if ((e.x | e.y) == 0ull) break;
+              slot = (slot + 1u) & slot_mask;
+            }
+          }
+          __stcs(cur + i, d);
+          changed += d != pv[k] ? 1u : 0u;
+          if (d != -2 && (hb[k] & 15u) < 14u) {
+            const unsigned long long v = inc[hb[k]];
+            lo += (uint32_t)v;
+            hi += (uint32_t)(v >> 32);
+          } else {
+            excluded++;
+          }
+          if ((++pending & 7) == 0) widen(lo, hi, B);
+        }
+        if (n_ds <= 8) {
+          if (d >= 0) dsl += 1ull << (8 * d);
+        } else {
+          const unsigned act = __ballot_sync(kFull, d >= 0);
+          if (d >= 0) {
+            const unsigned peers = __match_any_sync(act, d);
+            if ((t & 31) == __ffs(peers) - 1) {
+              if (in_smem) atomicAdd(&cnt_ds[d], (unsigned)__popc(peers));
+              else atomicAdd(&ds_count[d], (unsigned long long)__popc(peers));
+            }
+          }
+        }
+      }
+      if (pending >= 240) spill();
+    }
+    changed = __reduce_add_sync(kFull, changed);
+    if ((t & 31) == 0 && changed) atomicAdd(&tile_changed, changed);
+    __syncthreads();
+    if (t == 0) { tile_count[tile] = tile_changed; tile_changed = 0; }
+    __syncthreads();
+  }
+  spill();
+  __syncthreads();
+  for (int o = 16; o > 0; o >>= 1) excluded += __shfl_xor_sync(kFull, excluded, o);
+  if ((t & 31) == 0 && excluded) atomicAdd(&ws->bs_acc[UST_STATE_EXCLUDED], (unsigned long long)excluded);
+  if (t < 14) { if (cnt[t]) atomicAdd(&ws->bs_acc[t], (unsigned long long)cnt[t]); }
+  else if (t == 14) { if (cnt[14]) atomicAdd(&ws->bs_acc[16], (unsigned long long)cnt[14]); }
+  else if (t == 15) { if (cnt[15]) atomicAdd(&ws->bs_acc[17], (unsigned long long)cnt[15]); }
+  if (in_smem)
+    for (int i = t; i < n_ds; i += kThreads)
+      if (cnt_ds[i]) atomicAdd(&ds_count[i], (unsigned long long)cnt_ds[i]);
+}
+
+// The ordered write of ust_build_state_delta's sparse outputs: tile b's changed pods go to positions tile_off[b] .. (the
+// scanned tile counts), in index order; those at or beyond `cap` are not written.
+__global__ void __launch_bounds__(kThreads) ust_build_state_write_kernel(long long n, const int32_t* __restrict__ cur,
+                                                                         const int32_t* __restrict__ prev,
+                                                                         const unsigned int* __restrict__ tile_off, long long cap,
+                                                                         long long* __restrict__ out_idx, int32_t* __restrict__ out_ds) {
+  __shared__ unsigned int wtot[kWarps];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const long long i0 = (long long)blockIdx.x * kBuildTile + 16 * t;
+  int c16[16];
+  unsigned m = 0;
+  if (i0 + 16 <= n) {  // cur and prev are 16-byte aligned (device allocations), i0 a multiple of 16
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const int4 a = __ldcs(reinterpret_cast<const int4*>(cur + i0) + q), b = __ldcs(reinterpret_cast<const int4*>(prev + i0) + q);
+      c16[4 * q] = a.x; c16[4 * q + 1] = a.y; c16[4 * q + 2] = a.z; c16[4 * q + 3] = a.w;
+      m |= (unsigned)(a.x != b.x) << (4 * q) | (unsigned)(a.y != b.y) << (4 * q + 1) | (unsigned)(a.z != b.z) << (4 * q + 2) |
+           (unsigned)(a.w != b.w) << (4 * q + 3);
+    }
+  } else {
+#pragma unroll
+    for (int k = 0; k < 16; k++) {
+      c16[k] = 0;
+      if (i0 + k < n) { c16[k] = cur[i0 + k]; m |= (unsigned)(c16[k] != prev[i0 + k]) << k; }
+    }
+  }
+  const unsigned c = __popc(m);
+  unsigned incl = c;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned u = __shfl_up_sync(kFull, incl, o);
+    if (lane >= o) incl += u;
+  }
+  if (lane == 31) wtot[warp] = incl;
+  __syncthreads();
+  unsigned before = 0;
+  for (int w = 0; w < warp; w++) before += wtot[w];
+  long long pos = (long long)tile_off[blockIdx.x] + before + incl - c;
+#pragma unroll
+  for (int k = 0; k < 16; k++) {
+    if (!((m >> k) & 1u)) continue;
+    if (pos < cap) { out_idx[pos] = i0 + k; out_ds[pos] = c16[k]; }
+    pos++;
+  }
+}
+
+// The n_changed overwrites of ust_build_state_delta: state byte and owner UID of the pods at idx (new indices).
+__global__ void __launch_bounds__(kThreads) ust_build_state_patch_kernel(long long m, const long long* __restrict__ idx,
+                                                                         const uint8_t* __restrict__ state,
+                                                                         const ulonglong2* __restrict__ uid, uint8_t* hot_out,
+                                                                         ulonglong2* uid_out) {
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long k = (long long)blockIdx.x * kThreads + threadIdx.x; k < m; k += stride) {
+    const long long i = __ldg(idx + k);
+    hot_out[i] = __ldg(state + k);
+    uid_out[i] = __ldg(uid + k);
+  }
+}
+
 // Delta update of the resident snapshot (SURVEY 8f.2): scatter the re-encoded nodes into the SoA arrays.
 __global__ void __launch_bounds__(kThreads) ust_patch_kernel(long long m, const long long* __restrict__ idx,
                                                              const uint8_t* __restrict__ state, const uint32_t* __restrict__ flags,
@@ -890,19 +1091,12 @@ __global__ void __launch_bounds__(kThreads) ust_splice_kernel(long long n, long 
 // the previous actuator_outcome travels too (1 B more each way; 0xFF for inserted nodes).
 constexpr int kGatherTile = 2048;
 
-template <bool OUTCOME>
-__global__ void __launch_bounds__(kThreads) ust_reorder_kernel(long long n, long long n_runs, const long long* __restrict__ run_off,
-                                                               const long long* __restrict__ run_src,
-                                                               const uint8_t* __restrict__ ins_hot, const uint32_t* __restrict__ ins_flags,
-                                                               const int32_t* __restrict__ ins_rev, const int32_t* __restrict__ ins_ds,
-                                                               const uint8_t* __restrict__ hot, const uint32_t* __restrict__ flags,
-                                                               const int32_t* __restrict__ rev, const int32_t* __restrict__ ds,
-                                                               const uint8_t* __restrict__ next, const uint16_t* __restrict__ act,
-                                                               const uint8_t* __restrict__ oc,
-                                                               uint8_t* __restrict__ o_hot, uint32_t* __restrict__ o_flags,
-                                                               int32_t* __restrict__ o_rev, int32_t* __restrict__ o_ds,
-                                                               uint8_t* __restrict__ o_next, uint16_t* __restrict__ o_act,
-                                                               uint8_t* __restrict__ o_oc) {
+// The run lookup of the gather kernels (ust_reorder_kernel, ust_build_state_reorder_kernel): copy(p, src, k) for every new
+// position p of this CTA's tile, with the source of p's run (old start, or -1 - offset into the inserted entries) and p's
+// offset k in that run.
+template <class Copy>
+__device__ __forceinline__ void gather_runs(long long n, long long n_runs, const long long* __restrict__ run_off,
+                                            const long long* __restrict__ run_src, Copy copy) {
   __shared__ long long s_off[kGatherTile];
   __shared__ long long s_src[kGatherTile];
   __shared__ long long s_runs[2];
@@ -934,7 +1128,24 @@ __global__ void __launch_bounds__(kThreads) ust_reorder_kernel(long long n, long
       const int mid = (r + hi) >> 1;
       if (s_off[mid] <= p) r = mid; else hi = mid;
     }
-    const long long src = s_src[r], k = p - s_off[r];
+    copy(p, s_src[r], p - s_off[r]);
+  }
+}
+
+template <bool OUTCOME>
+__global__ void __launch_bounds__(kThreads) ust_reorder_kernel(long long n, long long n_runs, const long long* __restrict__ run_off,
+                                                               const long long* __restrict__ run_src,
+                                                               const uint8_t* __restrict__ ins_hot, const uint32_t* __restrict__ ins_flags,
+                                                               const int32_t* __restrict__ ins_rev, const int32_t* __restrict__ ins_ds,
+                                                               const uint8_t* __restrict__ hot, const uint32_t* __restrict__ flags,
+                                                               const int32_t* __restrict__ rev, const int32_t* __restrict__ ds,
+                                                               const uint8_t* __restrict__ next, const uint16_t* __restrict__ act,
+                                                               const uint8_t* __restrict__ oc,
+                                                               uint8_t* __restrict__ o_hot, uint32_t* __restrict__ o_flags,
+                                                               int32_t* __restrict__ o_rev, int32_t* __restrict__ o_ds,
+                                                               uint8_t* __restrict__ o_next, uint16_t* __restrict__ o_act,
+                                                               uint8_t* __restrict__ o_oc) {
+  gather_runs(n, n_runs, run_off, run_src, [=](long long p, long long src, long long k) {
     if (src >= 0) {
       const long long i = src + k;
       o_hot[p] = __ldcs(hot + i); o_flags[p] = __ldcs(flags + i); o_rev[p] = __ldcs(rev + i); o_ds[p] = __ldcs(ds + i);
@@ -946,7 +1157,27 @@ __global__ void __launch_bounds__(kThreads) ust_reorder_kernel(long long n, long
       o_next[p] = 0xFF; o_act[p] = 0;
       if (OUTCOME) o_oc[p] = 0xFF;
     }
-  }
+  });
+}
+
+// The resident driver-pod list of ust_build_state_delta in a new order: state byte, owner UID and previous owner index of
+// every pod that stays, from its old position; a joined pod takes its inserted values and previous owner index INT32_MIN,
+// which no owner index equals, so the diff reports it. 21 B read + 21 B written per pod.
+__global__ void __launch_bounds__(kThreads) ust_build_state_reorder_kernel(long long n, long long n_runs, const long long* __restrict__ run_off,
+                                                                           const long long* __restrict__ run_src,
+                                                                           const uint8_t* __restrict__ ins_hot, const ulonglong2* __restrict__ ins_uid,
+                                                                           const uint8_t* __restrict__ hot, const ulonglong2* __restrict__ uid,
+                                                                           const int32_t* __restrict__ prev, uint8_t* __restrict__ o_hot,
+                                                                           ulonglong2* __restrict__ o_uid, int32_t* __restrict__ o_prev) {
+  gather_runs(n, n_runs, run_off, run_src, [=](long long p, long long src, long long k) {
+    if (src >= 0) {
+      const long long i = src + k;
+      o_hot[p] = __ldcs(hot + i); o_uid[p] = __ldcs(uid + i); o_prev[p] = __ldcs(prev + i);
+    } else {
+      const long long i = -1 - src + k;
+      o_hot[p] = __ldg(ins_hot + i); o_uid[p] = __ldg(ins_uid + i); o_prev[p] = INT32_MIN;
+    }
+  });
 }
 
 // Replacement pod lists of the resident pod-list snapshot (ust_apply_state_delta_pods). The host has checked the lists
@@ -1631,3 +1862,42 @@ int ust_launch_diff(long long n, const uint8_t* next, const uint16_t* actions, c
   return (int)cudaGetLastError();
 }
 int ust_diff_blocks(long long n) { return (int)((n + kDiffBlock - 1) / kDiffBlock); }
+int ust_build_state_tiles(long long n) { return (int)((n + kBuildTile - 1) / kBuildTile); }
+int ust_launch_build_state_delta(long long n, const uint8_t* hot, const void* owner_uid, int n_ds, const void* ds_tab,
+                                 const int32_t* ds_tab_idx, int tab_slots, const int32_t* ds_desired, const int32_t* prev,
+                                 int32_t* cur, unsigned int* tile_count, unsigned long long* ds_count, UstWorkspace* ws,
+                                 ust_counters* out, int grid, void* stream) {
+  const long long tiles = ust_build_state_tiles(n);
+  if (grid > tiles) grid = tiles < 1 ? 1 : (int)tiles;
+  ust_build_state_delta_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(
+      n, hot, reinterpret_cast<const ulonglong2*>(owner_uid), n_ds, reinterpret_cast<const ulonglong2*>(ds_tab), ds_tab_idx, tab_slots,
+      prev, cur, tile_count, ds_count, ws);
+  ust_build_state_finish_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(n_ds, ds_desired, ds_count, ws, out);
+  return (int)cudaGetLastError();
+}
+int ust_launch_build_state_write(long long n, const int32_t* cur, const int32_t* prev, unsigned int* tile_count, long long* n_out,
+                                 long long cap, long long* out_idx, int32_t* out_ds, void* stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long tiles = ust_build_state_tiles(n);
+  ust_diff_scan_kernel<<<1, 1024, 0, st>>>((int)tiles, tile_count, n_out);
+  if (tiles > 0)
+    ust_build_state_write_kernel<<<(unsigned)tiles, kThreads, 0, st>>>(n, cur, prev, tile_count, cap, out_idx, out_ds);
+  return (int)cudaGetLastError();
+}
+int ust_launch_build_state_reorder(long long n, long long n_runs, const long long* run_off, const long long* run_src,
+                                   const uint8_t* ins_hot, const void* ins_uid, const uint8_t* hot, const void* uid,
+                                   const int32_t* prev, uint8_t* o_hot, void* o_uid, int32_t* o_prev, void* stream) {
+  const long long grid = n > 0 ? (n + kGatherTile - 1) / kGatherTile : 1;
+  ust_build_state_reorder_kernel<<<(unsigned)grid, kThreads, 0, (cudaStream_t)stream>>>(
+      n, n_runs, run_off, run_src, ins_hot, reinterpret_cast<const ulonglong2*>(ins_uid), hot, reinterpret_cast<const ulonglong2*>(uid),
+      prev, o_hot, reinterpret_cast<ulonglong2*>(o_uid), o_prev);
+  return (int)cudaGetLastError();
+}
+int ust_launch_build_state_patch(long long m, const long long* idx, const uint8_t* state, const void* uid, uint8_t* hot_out,
+                                 void* uid_out, void* stream) {
+  if (m <= 0) return 0;
+  const long long grid = (m + kThreads - 1) / kThreads;
+  ust_build_state_patch_kernel<<<(unsigned)(grid > 65535 * 16 ? 65535 * 16 : grid), kThreads, 0, (cudaStream_t)stream>>>(
+      m, idx, state, reinterpret_cast<const ulonglong2*>(uid), hot_out, reinterpret_cast<ulonglong2*>(uid_out));
+  return (int)cudaGetLastError();
+}

@@ -2,6 +2,7 @@
 #include "upgrade.hpp"
 
 #include <algorithm>
+#include <climits>
 #include <thread>
 #include <unordered_map>
 #include <cstring>
@@ -192,53 +193,81 @@ static Uid128 uid128(const std::string& uid) {
 }
 
 // ---- BuildState (upgrade_state.go:99-164) --------------------------------------------------------------------
+// What BuildState lists (upgrade_state.go:105-119): the DaemonSets keyed by UID (common_manager.go:180-186) and, in the map's
+// order, their 128-bit UIDs and DesiredNumberScheduled (padded by one entry: never pass empty vectors' data()); the pods.
+struct Listed {
+  std::map<std::string, DaemonSet*> daemonSets;
+  std::vector<DaemonSet*> dsByIndex;
+  std::vector<uint64_t> dsUid;
+  std::vector<int32_t> desired;
+  std::vector<Pod*> podList;
+};
+static Error list(K8sClient* client, const std::string& ns, const StringMap& driverLabels, Listed* l) {
+  std::vector<DaemonSet*> dsList;
+  if (Error e = client->ListDaemonSets(ns, driverLabels, &dsList)) return Errorf("error getting DaemonSet list: " + *e);
+  for (DaemonSet* ds : dsList) l->daemonSets[ds->UID] = ds;
+  if (Error e = client->ListPods(ns, driverLabels, &l->podList)) return e;
+  for (const auto& kv : l->daemonSets) {
+    const Uid128 u = uid128(kv.first);
+    l->dsByIndex.push_back(kv.second);
+    l->dsUid.push_back(u.hi); l->dsUid.push_back(u.lo);
+    l->desired.push_back(kv.second->DesiredNumberScheduled);
+  }
+  l->dsUid.resize(l->dsUid.size() + 2); l->desired.push_back(0);
+  return std::nullopt;
+}
+
+// A driver pod's state byte and the 128-bit UID of its OwnerReferences[0] ((0, 0) = none), as the owner join takes them.
+static void derivePod(const Pod& pod, uint8_t* state, uint64_t* owner) {
+  // upgrade_state.go:149-152: a pod not yet scheduled to a node is skipped - after the count check
+  *state = (pod.NodeName.empty() && pod.Phase == "Pending") ? UST_STATE_EXCLUDED : UST_STATE_OTHER;
+  owner[0] = owner[1] = 0;
+  if (!IsOrphanedPod(pod)) {
+    const Uid128 u = uid128(pod.OwnerReferences[0].UID);
+    owner[0] = u.hi; owner[1] = u.lo;
+  }
+}
+
+int ClusterUpgradeStateManagerImpl::BuildStateDevice(int64_t n, const uint8_t* state, const uint64_t* owner, int32_t n_ds,
+                                                     const uint64_t* ds_uid, const int32_t* desired, int32_t* owner_idx, ust_counters* c) {
+  if (handle_ == nullptr) return UST_ERR_CUDA;
+  return ust_build_state_uids(handle_, n, state, owner, n_ds, ds_uid, desired, owner_idx, c);
+}
+
+static const char* const kNoDeviceBuildState = "no H100 device bound to this manager: BuildState has no CPU path";
+
 Error ClusterUpgradeStateManagerImpl::BuildState(const std::string& ns, const StringMap& driverLabels,
                                                  std::unique_ptr<ClusterUpgradeState>* out) {
-  if (handle_ == nullptr) return Errorf("no H100 device bound to this manager: BuildState has no CPU path");
-  std::vector<DaemonSet*> dsList;
-  if (Error e = K8sClient->ListDaemonSets(ns, driverLabels, &dsList)) return Errorf("error getting DaemonSet list: " + *e);
-  std::map<std::string, DaemonSet*> daemonSets;  // UID -> DaemonSet  (common_manager.go:180-186)
-  for (DaemonSet* ds : dsList) daemonSets[ds->UID] = ds;
-  std::vector<Pod*> podList;
-  if (Error e = K8sClient->ListPods(ns, driverLabels, &podList)) return e;
+  Listed l;
+  if (Error e = list(K8sClient, ns, driverLabels, &l)) return e;
 
   // The owner join runs on the GPU (ust_build_state_uids): every listed pod goes in with the 128-bit form of its
   // OwnerReferences[0].UID, the DaemonSets with theirs; back comes, per pod, the owning DaemonSet's index, -1 for an
   // orphaned pod, -2 for a pod owned by something else (dropped: GetPodsOwnedbyDs skips it, GetOrphanedPods does
   // not take it - common_manager.go:190-222), after the per-DaemonSet count check of upgrade_state.go:128-131.
-  std::vector<DaemonSet*> dsByIndex;
-  std::vector<uint64_t> dsUid;
-  std::vector<int32_t> desired;
-  for (const auto& kv : daemonSets) {
-    const Uid128 u = uid128(kv.first);
-    dsByIndex.push_back(kv.second);
-    dsUid.push_back(u.hi); dsUid.push_back(u.lo);
-    desired.push_back(kv.second->DesiredNumberScheduled);
-  }
-  const size_t np = podList.size();
+  const size_t np = l.podList.size();
   std::vector<uint8_t> podState(np + 1);
   std::vector<uint64_t> owner(2 * np + 2, 0);
   std::vector<int32_t> owner_idx(np + 1, -2);
-  for (size_t i = 0; i < np; i++) {
-    Pod* pod = podList[i];
-    // upgrade_state.go:149-152: a pod not yet scheduled to a node is skipped - after the count check
-    podState[i] = (pod->NodeName.empty() && pod->Phase == "Pending") ? UST_STATE_EXCLUDED : UST_STATE_OTHER;
-    if (!IsOrphanedPod(*pod)) {
-      const Uid128 u = uid128(pod->OwnerReferences[0].UID);
-      owner[2 * i] = u.hi; owner[2 * i + 1] = u.lo;
-    }
-  }
-  dsUid.resize(dsUid.size() + 2); desired.push_back(0);  // never pass empty vectors' data()
+  for (size_t i = 0; i < np; i++) derivePod(*l.podList[i], &podState[i], &owner[2 * i]);
   ust_counters c;
-  int rc = ust_build_state_uids(handle_, (int64_t)np, podState.data(), owner.data(), (int32_t)dsByIndex.size(), dsUid.data(),
-                                desired.data(), owner_idx.data(), &c);
+  int rc = BuildStateDevice((int64_t)np, podState.data(), owner.data(), (int32_t)l.dsByIndex.size(), l.dsUid.data(), l.desired.data(),
+                            owner_idx.data(), &c);
   if (rc == UST_ERR_DS_UNSCHEDULED) return Errorf("driver DaemonSet should not have Unscheduled pods");  // upgrade_state.go:128-131
-  if (rc != UST_OK) return Errorf(ust_last_error(handle_));
+  if (rc != UST_OK) return Errorf(handle_ ? ust_last_error(handle_) : kNoDeviceBuildState);
+  return assembleState(l.podList, podState.data(), owner_idx.data(), l.daemonSets, out);
+}
 
+// BuildState after the owner join: the snapshot from the pods' state bytes and owner indices.
+Error ClusterUpgradeStateManagerImpl::assembleState(const std::vector<Pod*>& podList, const uint8_t* podState, const int32_t* owner_idx,
+                                                    std::map<std::string, DaemonSet*>& daemonSets,
+                                                    std::unique_ptr<ClusterUpgradeState>* out) {
+  const size_t np = podList.size();
+  const size_t nds = daemonSets.size();
   // filteredPodList in the reference's order: DaemonSet by DaemonSet (map order), then the orphans (:126-136)
   std::vector<Pod*> filtered;
   std::vector<uint8_t> state;
-  std::vector<std::vector<size_t>> byOwner(dsByIndex.size() + 1);  // last bucket: orphans
+  std::vector<std::vector<size_t>> byOwner(nds + 1);  // last bucket: orphans
   for (size_t i = 0; i < np; i++) {
     if (owner_idx[i] >= 0) byOwner[(size_t)owner_idx[i]].push_back(i);
     else if (owner_idx[i] == -1) byOwner.back().push_back(i);
@@ -266,6 +295,131 @@ Error ClusterUpgradeStateManagerImpl::BuildState(const std::string& ns, const St
   }
   *out = std::move(st);
   return std::nullopt;
+}
+
+// A new order given per position as the old index it takes (-1: an entry that joins), as the maximal runs of ust_reorder /
+// ust_driver_pod_reorder: consecutive old entries, joined entries.
+static void orderRuns(const std::vector<int64_t>& from, std::vector<int64_t>* run_src, std::vector<int64_t>* run_len) {
+  for (size_t p = 0; p < from.size(); p++) {
+    const bool cont = p > 0 && ((from[p] < 0 && from[p - 1] < 0) || (from[p] >= 0 && from[p - 1] >= 0 && from[p] == from[p - 1] + 1));
+    if (cont) { run_len->back()++; continue; }
+    run_src->push_back(from[p] < 0 ? -1 : from[p]);
+    run_len->push_back(1);
+  }
+}
+
+// ---- incremental BuildState (upgrade.hpp) ------------------------------------------------------------------------------
+void ClusterUpgradeStateManagerImpl::ResetBuildIncremental() { podCache_ = PodCache(); }
+
+int ClusterUpgradeStateManagerImpl::BuildStateCached(int32_t n_ds, const uint64_t* ds_uid, const int32_t* desired, PodCache* cache,
+                                                     ust_counters* c) {
+  PodCache& k = *cache;
+  if (handle_ == nullptr) return UST_ERR_CUDA;
+  const size_t n = k.state.size(), m = k.changed.size(), ni = k.insert_at.size();
+  // the joined and the overwritten pods' values (never pass NULL for empty arrays)
+  std::vector<uint8_t> ist(ni + 1), cst(m + 1);
+  std::vector<uint64_t> iuid(2 * ni + 2), cuid(2 * m + 2);
+  for (size_t j = 0; j < ni; j++) {
+    const size_t i = (size_t)k.insert_at[j];
+    ist[j] = k.state[i]; iuid[2 * j] = k.owner[2 * i]; iuid[2 * j + 1] = k.owner[2 * i + 1];
+  }
+  std::vector<int64_t> ix(k.changed);
+  ix.push_back(0);
+  for (size_t j = 0; j < m; j++) {
+    const size_t i = (size_t)k.changed[j];
+    cst[j] = k.state[i]; cuid[2 * j] = k.owner[2 * i]; cuid[2 * j + 1] = k.owner[2 * i + 1];
+  }
+  const ust_driver_pod_reorder ro = {(int64_t)k.run_src.size(), k.run_src.data(), k.run_len.data(), (int64_t)ni, ist.data(), iuid.data()};
+  const int64_t cap = (int64_t)(n / 4 + 1024);
+  std::vector<int64_t> oi((size_t)cap + 1);
+  std::vector<int32_t> od((size_t)cap + 1);
+  int64_t n_out = 0;
+  const int rc = ust_build_state_delta(handle_, k.reorder ? &ro : nullptr, (int64_t)m, ix.data(), cst.data(), cuid.data(), n_ds, ds_uid,
+                                       desired, cap, oi.data(), od.data(), &n_out, c);
+  if (rc == UST_ERR_CUDA || rc == UST_ERR_INVALID_ARGUMENT) return rc;
+  if (n_out > cap) {  // nothing was written to the arrays (UST_ERR_TRUNCATED, or UST_ERR_DS_UNSCHEDULED with its own code)
+    buildStats_.outputs_received += (int64_t)n;
+    const int frc = ust_fetch_build_state(handle_, (int64_t)n, k.ownerIdx.data());
+    if (frc != UST_OK) return frc;
+    return rc == UST_ERR_TRUNCATED ? UST_OK : rc;
+  }
+  for (int64_t j = 0; j < n_out; j++) k.ownerIdx[(size_t)oi[(size_t)j]] = od[(size_t)j];
+  buildStats_.outputs_received += n_out;
+  return rc;
+}
+
+Error ClusterUpgradeStateManagerImpl::BuildStateIncremental(const std::string& ns, const StringMap& driverLabels,
+                                                            std::unique_ptr<ClusterUpgradeState>* out) {
+  Listed l;
+  if (Error e = list(K8sClient, ns, driverLabels, &l)) return e;
+  PodCache& k = podCache_;
+  buildStats_.reconciles++;
+  const bool full = !k.valid;
+  const size_t nOld = full ? 0 : k.state.size(), np = l.podList.size();
+  // the list in this reconcile's order: per position the cached pod it continues (-1: a pod that joins)
+  PodCache nk;
+  nk.posOf.reserve(np);
+  nk.rv.resize(np);
+  nk.state.resize(np);
+  nk.owner.resize(2 * np);
+  nk.ownerIdx.resize(np);
+  std::vector<int64_t> from(np, -1);
+  std::vector<char> present(nOld, 0);
+  bool moved = false;
+  int64_t last = -1, removed = (int64_t)nOld;
+  for (size_t i = 0; i < np; i++) {
+    const Pod& pod = *l.podList[i];
+    const std::string key = pod.Namespace + "/" + pod.Name;
+    if (!nk.posOf.emplace(key, i).second) {
+      ResetBuildIncremental();
+      return Errorf("pod " + key + " is listed twice");
+    }
+    nk.rv[i] = pod.ResourceVersion;
+    auto it = full ? k.posOf.end() : k.posOf.find(key);
+    if (it == k.posOf.end()) {  // joins
+      derivePod(pod, &nk.state[i], &nk.owner[2 * i]);
+      buildStats_.rederived++;
+      nk.insert_at.push_back((int64_t)i);
+      nk.ownerIdx[i] = INT32_MIN;  // comes back from the device: every joined pod is reported
+      continue;
+    }
+    const size_t q = it->second;
+    present[q] = 1;
+    removed--;
+    moved = moved || (int64_t)q < last;
+    last = (int64_t)q;
+    from[i] = (int64_t)q;
+    nk.ownerIdx[i] = k.ownerIdx[q];
+    if (!pod.ResourceVersion.empty() && pod.ResourceVersion == k.rv[q]) {
+      nk.state[i] = k.state[q]; nk.owner[2 * i] = k.owner[2 * q]; nk.owner[2 * i + 1] = k.owner[2 * q + 1];
+      buildStats_.reused++;
+      continue;
+    }
+    derivePod(pod, &nk.state[i], &nk.owner[2 * i]);
+    buildStats_.rederived++;
+    if (nk.state[i] != k.state[q] || nk.owner[2 * i] != k.owner[2 * q] || nk.owner[2 * i + 1] != k.owner[2 * q + 1])
+      nk.changed.push_back((int64_t)i);
+  }
+  // joins, leaves and moves travel as one reorder (after a reset: the whole list as one inserted run)
+  nk.reorder = full || moved || removed > 0 || !nk.insert_at.empty();
+  if (nk.reorder) orderRuns(from, &nk.run_src, &nk.run_len);
+  if (full) {
+    buildStats_.full_uploads++;
+  } else {
+    buildStats_.inserted += (int64_t)nk.insert_at.size();
+    buildStats_.removed += removed;
+    buildStats_.reorders += nk.reorder ? 1 : 0;
+  }
+  k = std::move(nk);
+  ust_counters c;
+  const int rc = BuildStateCached((int32_t)l.dsByIndex.size(), l.dsUid.data(), l.desired.data(), &k, &c);
+  if (rc != UST_OK && rc != UST_ERR_DS_UNSCHEDULED) {  // the device list is not what the cache holds: start over
+    ResetBuildIncremental();
+    return Errorf(handle_ ? ust_last_error(handle_) : kNoDeviceBuildState);
+  }
+  k.valid = true;
+  if (rc == UST_ERR_DS_UNSCHEDULED) return Errorf("driver DaemonSet should not have Unscheduled pods");  // upgrade_state.go:128-131
+  return assembleState(l.podList, k.state.data(), k.ownerIdx.data(), l.daemonSets, out);
 }
 
 // ---- ApplyState = Encode -> kernel -> Replay -------------------------------------------------------------------
@@ -750,12 +904,7 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
     if (!present[i]) sp.remove_idx.push_back((int64_t)i);
   if (moved) {  // maximal runs of consecutive old slots, joins as inserted runs
     sp.insert_before.clear();
-    for (size_t p = 0; p < from.size(); p++) {
-      const bool cont = p > 0 && ((from[p] < 0 && from[p - 1] < 0) || (from[p] >= 0 && from[p - 1] >= 0 && from[p] == from[p - 1] + 1));
-      if (cont) { sp.run_len.back()++; continue; }
-      sp.run_src.push_back(from[p] < 0 ? -1 : from[p]);
-      sp.run_len.push_back(1);
-    }
+    orderRuns(from, &sp.run_src, &sp.run_len);
   }
   // The host arrays move to the new order (linear). Joined slots start empty and are encoded by the walk below.
   std::vector<char> joined;

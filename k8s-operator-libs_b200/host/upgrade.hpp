@@ -300,7 +300,45 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
   const IncrementalStats& Stats() const { return stats_; }
   void ResetIncremental();
 
+  // ---- incremental BuildState: the driver-pod list stays on the device (ust_build_state_delta) -----------------------------
+  // The same contract, result and errors as BuildState, for a reconcile loop that calls it again and again. The manager keeps
+  // the raw ListPods order (keyed by Namespace/Name) with each pod's state byte, owner UID and owner index; a pod's state
+  // byte and owner UID are re-derived only when its resourceVersion changed (or is ""), pods that join, leave or move in the
+  // list go to the device as runs of one reorder, and only the owner indices that changed come back. With
+  // ApplyStateIncremental on the same manager the whole reconcile stays incremental: BuildState's list never leaves the
+  // device, and neither does ApplyState's snapshot. The first call (and the first after a reset) sends every pod.
+  Error BuildStateIncremental(const std::string& ns, const StringMap& driverLabels, std::unique_ptr<ClusterUpgradeState>* out);
+  struct BuildStats {
+    int64_t reconciles = 0, full_uploads = 0;
+    int64_t rederived = 0, reused = 0;  // pods whose state byte and owner UID were derived anew / taken from the cache
+    int64_t inserted = 0, removed = 0;  // pods that joined / left the cached list
+    int64_t reorders = 0;               // reconciles whose list moved on the device (a join, a leave or a move)
+    int64_t outputs_received = 0;       // owner indices that came back (sparse, or all of them after a truncation)
+  };
+  const BuildStats& BuildStateStats() const { return buildStats_; }
+  void ResetBuildIncremental();
+
  protected:
+  // The cached driver-pod list of BuildStateIncremental, in this reconcile's ListPods order, and what changed since the
+  // device last saw it: with `reorder`, the new order as ust_driver_pod_reorder runs (after a reset: the whole list as one
+  // inserted run) and the joined pods' positions; the positions whose values were overwritten.
+  struct PodCache {
+    std::unordered_map<std::string, size_t> posOf;  // Namespace/Name -> position
+    std::vector<std::string> rv;                     // resourceVersion the pod's values were derived at
+    std::vector<uint8_t> state;
+    std::vector<uint64_t> owner;                     // two per pod
+    std::vector<int32_t> ownerIdx;                   // owning DaemonSet index / -1 / -2 (INT32_MIN until a joined pod's comes back)
+    std::vector<int64_t> run_src, run_len, insert_at, changed;
+    bool reorder = false;
+    bool valid = false;
+  };
+  // The device call of BuildState: ust_build_state_uids. Returns the ABI's return code.
+  virtual int BuildStateDevice(int64_t n, const uint8_t* state, const uint64_t* owner, int32_t n_ds, const uint64_t* ds_uid,
+                               const int32_t* desired, int32_t* owner_idx, ust_counters* c);
+  // The device half of BuildStateIncremental: hand cache->run_src / changed to ust_build_state_delta and patch the owner
+  // indices that changed into cache->ownerIdx (already in the new order), or fetch them all. Returns the ABI's return code.
+  // (Both virtual so that the host-logic test can put the oracle behind them.)
+  virtual int BuildStateCached(int32_t n_ds, const uint64_t* ds_uid, const int32_t* desired, PodCache* cache, ust_counters* c);
   // The device half of ApplyStateIncremental: evaluate the cached snapshot. full: upload all of it and fetch all
   // outputs; else apply cache->pending to the resident snapshot, upload the entries `changed` and patch the outputs that
   // differ into cache_.next / cache_.actions (whose entries already follow the splice).
@@ -340,8 +378,12 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
  private:
   Error encodeOne(const NodeUpgradeState* ns, int code, int32_t ds, bool dsErr, std::map<std::string, int32_t>* intern,
                   const std::vector<int32_t>& ds_rev, uint8_t* hot, uint32_t* flags, int32_t* rev, std::string* deferred);
+  Error assembleState(const std::vector<Pod*>& podList, const uint8_t* podState, const int32_t* owner_idx,
+                      std::map<std::string, DaemonSet*>& daemonSets, std::unique_ptr<ClusterUpgradeState>* out);
   Cache cache_;
   IncrementalStats stats_;
+  PodCache podCache_;
+  BuildStats buildStats_;
   ust_handle* handle_ = nullptr;
   StateOptions opts_;
   bool podDeletionStateEnabled_ = false, validationStateEnabled_ = false;

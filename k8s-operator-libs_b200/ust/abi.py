@@ -99,6 +99,12 @@ class Reorder(C.Structure):
                 ("state", C.c_void_p), ("flags", C.c_void_p), ("pod_rev", C.c_void_p), ("ds_idx", C.c_void_p)]
 
 
+class DriverPodReorder(C.Structure):
+    """ust_driver_pod_reorder: a new order of the resident driver-pod list as runs of old and joined pods (raw host addresses)."""
+    _fields_ = [("n_runs", C.c_int64), ("run_src", C.c_void_p), ("run_len", C.c_void_p), ("n_insert", C.c_int64),
+                ("state", C.c_void_p), ("owner_uid", C.c_void_p)]
+
+
 class PodLists(C.Structure):
     """ust_pod_lists: replacement pod lists for some nodes of the resident pod-list snapshot (raw host addresses)."""
     _fields_ = [("n_lists", C.c_int64), ("node_idx", C.c_void_p), ("pod_off", C.c_void_p), ("pod_flags", C.c_void_p),

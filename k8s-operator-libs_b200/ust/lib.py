@@ -72,6 +72,9 @@ def load():
         lib.ust_build_state.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
         lib.ust_build_state_uids.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                              C.c_void_p, C.c_void_p]
+        lib.ust_build_state_delta.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                              C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.ust_fetch_build_state.argtypes = [C.c_void_p, C.c_int64, C.c_void_p]
         lib.ust_get_unique_id.argtypes = [C.c_void_p]
         lib.ust_comm_init.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         lib.ust_comm_set_mode.argtypes = [C.c_void_p, C.c_int]
@@ -84,7 +87,7 @@ def load():
 
 EXPORTS = ["ust_abi_version", "ust_create", "ust_destroy", "ust_last_error", "ust_create_error", "ust_launch_count",
            "ust_host_alloc", "ust_host_free", "ust_apply_state", "ust_apply_state_device", "ust_stream", "ust_apply_state_packed", "ust_apply_state_delta", "ust_apply_state_delta_sparse", "ust_apply_state_delta_splice", "ust_apply_state_delta_reorder", "ust_apply_state_delta_pods", "ust_apply_state_delta_pods_reorder", "ust_fetch_outputs", "ust_fetch_outputs_pods", "ust_simulate_rollout", "ust_simulate_rollout_timed", "ust_sync",
-           "ust_build_state", "ust_build_state_uids", "ust_get_unique_id", "ust_comm_init", "ust_comm_set_mode", "ust_table_entry",
+           "ust_build_state", "ust_build_state_uids", "ust_build_state_delta", "ust_fetch_build_state", "ust_get_unique_id", "ust_comm_init", "ust_comm_set_mode", "ust_table_entry",
            "ust_table_window_shift"]
 
 
@@ -482,6 +485,47 @@ class Handle:
         rc = self._lib.ust_build_state_uids(self._h, n, _p(state), _p(owner_uid), int(ds_uid.shape[0]), _p(ds_uid),
                                             _p(ds_desired), _p(ds_idx), C.addressof(cnt))
         return rc, ds_idx, cnt.as_dict()
+
+    def build_state_delta(self, reorder, idx, state, owner_uid, ds_uid, ds_desired, max_out, out=None):
+        """ust_build_state_delta on the resident driver-pod list. `reorder` is None or a dict with run_src, run_len and the
+        joined pods' state / owner_uid ((n_insert, 2) uint64; n_insert defaults to their count); `idx` (new indices), `state`
+        and `owner_uid` are the overwritten pods. Returns (rc, n_out, out_idx, out_ds_idx, counters-dict); the arrays hold
+        n_out entries when n_out <= max_out."""
+        keep = []
+
+        def arr(a, dt):
+            a = np.ascontiguousarray(a, dtype=dt)
+            keep.append(a)
+            return a
+
+        ro = None
+        if reorder is not None:
+            src = arr(reorder.get("run_src", np.zeros(0)), np.int64)
+            ln = arr(reorder.get("run_len", np.zeros(0)), np.int64)
+            ist = arr(reorder["state"], np.uint8) if "state" in reorder else None
+            iuid = arr(reorder["owner_uid"], np.uint64) if "owner_uid" in reorder else None
+            n_ins = reorder.get("n_insert", 0 if ist is None else int(ist.shape[0]))
+            ro = abi.DriverPodReorder(int(src.shape[0]), _p(src), _p(ln), int(n_ins), _p(ist), _p(iuid))
+        idx = arr(idx, np.int64)
+        state = arr(state, np.uint8)
+        owner_uid = arr(owner_uid, np.uint64)
+        ds_uid = arr(ds_uid, np.uint64).reshape(-1, 2)
+        ds_desired = arr(ds_desired, np.int32)
+        if out is None:
+            out = (np.zeros(max_out + 1, np.int64), np.zeros(max_out + 1, np.int32))
+        n_out = C.c_int64(0)
+        cnt = abi.Counters()
+        rc = self._lib.ust_build_state_delta(
+            self._h, C.addressof(ro) if ro is not None else None, int(idx.shape[0]), _p(idx), _p(state), _p(owner_uid),
+            int(ds_uid.shape[0]), _p(ds_uid), _p(ds_desired), C.c_int64(int(max_out)), _p(out[0]), _p(out[1]),
+            C.addressof(n_out), C.addressof(cnt))
+        return rc, int(n_out.value), out[0], out[1], cnt.as_dict()
+
+    def fetch_build_state(self, n):
+        """ust_fetch_build_state: (rc, owner index per pod) of the resident driver-pod list of n pods."""
+        ds_idx = np.full(n, -3, np.int32)
+        rc = self._lib.ust_fetch_build_state(self._h, int(n), _p(ds_idx))
+        return rc, ds_idx
 
     def comm_init(self, rank, world, unique_id_bytes):
         buf = (C.c_char * abi.UST_UNIQUE_ID_BYTES).from_buffer_copy(unique_id_bytes) if unique_id_bytes else None
