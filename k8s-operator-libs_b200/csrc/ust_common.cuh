@@ -1,7 +1,7 @@
-// ust_common.cuh — device code shared by the streaming kernel (ust_stream.cu) and the verification kernel
-// (ust_kernels.cu): PTX wrappers (mbarrier, TMA bulk copy, programmatic dependent launch, system-scope accesses),
-// the cluster-wide arithmetic between the two (GetUpgradesAvailable and friends), and the decision a call's last
-// CTA makes about the slot speculation.
+// ust_common.cuh — device code shared by the streaming kernel (ust_stream.cu) and the kernels of ust_kernels.cu: PTX
+// wrappers (mbarrier, TMA bulk copy, programmatic dependent launch, system-scope accesses), the byte-sliced counters of
+// the streaming and BuildState passes, the cluster-wide arithmetic between the streaming and the verification kernel
+// (GetUpgradesAvailable and friends), and the decision a call's last CTA makes about the slot speculation.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -100,6 +100,34 @@ __device__ __forceinline__ int pass_of_state(unsigned code) {
 __device__ __forceinline__ uint32_t cand_mask4(uint32_t x) {
   const uint32_t y = (x & 0x2F2F2F2Fu) ^ 0x01010101u;  // zero byte <=> code == 1 && !SKIP
   return ~(((y & 0x7F7F7F7Fu) + 0x7F7F7F7Fu) | y) & 0x80808080u;
+}
+
+// ---- byte-sliced SIMD-in-register counting (the streaming pass and the BuildState passes) -------------------------
+// A hot byte increments sixteen 4-bit one-hot fields packed in 64 bits: fields 0-13 count the state codes, field 14 the
+// unavailable nodes, field 15 the upgrade candidates; codes 14 and 15 count nothing. GetCurrentUnavailableNodes
+// (common_manager.go:146-165) counts every snapshot entry that is cordoned or not ready; an upgrade candidate is
+// upgrade-required and not marked skip (upgrade_inplace.go:82). A thread sums the increments of up to 8 nodes in two
+// registers (lo = fields 0-7, hi = fields 8-15), widens the nibbles into four byte-lane words and keeps going.
+__device__ __forceinline__ unsigned long long hot_increments(unsigned b) {
+  const unsigned code = b & 15u;
+  unsigned long long v = 0;
+  if (code < 14) {
+    v = 1ull << (4 * code);
+    if (b & (UST_HOT_UNSCHEDULABLE | UST_HOT_NOT_READY)) v |= 1ull << 56;
+    if (code == UST_STATE_UPGRADE_REQUIRED && !(b & UST_HOT_SKIP)) v |= 1ull << 60;
+  }
+  return v;
+}
+// byte lanes: B[0] = fields 0,2,4,6  B[1] = fields 1,3,5,7  B[2] = fields 8,10,12,14  B[3] = fields 9,11,13,15
+__device__ __forceinline__ unsigned field_of(const uint32_t (&B)[4], int f) {
+  return (B[(f >> 3) * 2 + (f & 1)] >> (8 * ((f & 7) >> 1))) & 0xFFu;
+}
+__device__ __forceinline__ void widen(uint32_t& lo, uint32_t& hi, uint32_t (&B)[4]) {
+  B[0] += lo & 0x0F0F0F0Fu;
+  B[1] += (lo >> 4) & 0x0F0F0F0Fu;
+  B[2] += hi & 0x0F0F0F0Fu;
+  B[3] += (hi >> 4) & 0x0F0F0F0Fu;
+  lo = hi = 0;
 }
 
 // four table entries (actions | next << 16 | outcome << 24) -> the three output words of a 4-node group

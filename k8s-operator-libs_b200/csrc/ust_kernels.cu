@@ -17,6 +17,11 @@
 // (replaced pod lists), ust_pods_reorder_runs_kernel / ust_pods_reorder_kernel (pod lists in a new node order),
 // ust_diff_*_kernel (sparse outputs),
 // ust_widen_kernel (packed host format).
+// The auxiliary kernels share their building blocks, each written once: the BuildState join and counts (build_prologue,
+// build_join, build_count, build_count_ds, build_spill, build_finish), the searches over sorted run / segment starts
+// (last_le in global memory, last_le_from over a staged slice), the gathers of a new order (gather_runs for node columns,
+// gather_pods for a pod-list CSR), and the compaction in index order behind a scan of CTA counts (cta_sum,
+// cta_first_pos).
 #include <climits>
 
 #include "ust_common.cuh"
@@ -50,18 +55,6 @@ struct __align__(128) Shared {
   int redo, cut, lo, hi;
   DecideShared D;
 };
-
-// byte lanes: B[0] = fields 0,2,4,6  B[1] = fields 1,3,5,7  B[2] = fields 8,10,12,14  B[3] = fields 9,11,13,15
-__device__ __forceinline__ unsigned p1_field(const uint32_t (&B)[4], int f) {
-  return (B[(f >> 3) * 2 + (f & 1)] >> (8 * ((f & 7) >> 1))) & 0xFFu;
-}
-__device__ __forceinline__ void widen(uint32_t& lo, uint32_t& hi, uint32_t (&B)[4]) {
-  B[0] += lo & 0x0F0F0F0Fu;
-  B[1] += (lo >> 4) & 0x0F0F0F0Fu;
-  B[2] += hi & 0x0F0F0F0Fu;
-  B[3] += (hi >> 4) & 0x0F0F0F0Fu;
-  lo = hi = 0;
-}
 
 // ------------------------------------------------------------------------------------------------
 // per-node transition
@@ -590,11 +583,154 @@ __global__ void __launch_bounds__(kThreads, 6) ust_pod_summary_kernel(long long 
 // by UID) is an open-addressing hash table built by the host at load factor <= 1/4 (ust_uid_hash, linear probing,
 // (0, 0) = empty slot) and copied to shared memory: one 16-byte lookup per pod in the common case. Counting is
 // byte-sliced as in the streaming pass; per-DaemonSet counts are packed byte counters (<= 8 DaemonSets) or
-// warp-aggregated atomics.
+// warp-aggregated atomics. ust_build_state_uid_kernel and ust_build_state_delta_kernel share these pieces and differ in
+// their loops only.
 constexpr int kUidTabSmem = 2048;  // hash slots held in shared memory (DaemonSets <= 512); larger tables stay in global memory
+constexpr int kBuildU = 4;         // pods per thread and iteration: four 16-byte loads in flight
+constexpr int kBuildSpill = 240;   // pods a thread counts between spills (a byte lane holds 255)
+
+// The pieces of a BuildState pass. The kernel declares the shared arrays - tab / ord (the hash table, UID only),
+// cnt_ds[kUidTabSmem / 4] (owned pods per DaemonSet), inc[256] (hot byte -> hot_increments) and cnt[16] (the counted
+// fields) - and keeps a thread's counts in registers: nibble sums lo / hi and byte lanes B (ust_common.cuh), `pending`
+// pods since the last spill, `excluded` pods in no bucket, and with n_ds <= 8 `dsl`, its owned-pod count per DaemonSet,
+// one byte each.
+//
+// Prologue, whole CTA, before a barrier: the hash table staged (UID, when it fits), the counters cleared, the increment
+// table filled. Returns in_smem: the table (UID) or the per-DaemonSet counters (index form) are in shared memory.
+template <bool UID>
+__device__ __forceinline__ bool build_prologue(ulonglong2* tab, int* ord, unsigned int* cnt_ds, unsigned long long* inc,
+                                               unsigned int* cnt, int n_ds, const ulonglong2* __restrict__ ds_tab,
+                                               const int32_t* __restrict__ ds_tab_idx, int tab_slots) {
+  const int t = threadIdx.x;
+  const bool in_smem = UID ? tab_slots <= kUidTabSmem : n_ds <= kUidTabSmem / 4;  // UID: then n_ds <= kUidTabSmem / 4 too
+  if (in_smem) {
+    if (UID)
+      for (int i = t; i < tab_slots; i += kThreads) { tab[i] = ds_tab[i]; ord[i] = ds_tab_idx[i]; }
+    for (int i = t; i < n_ds; i += kThreads) cnt_ds[i] = 0;
+  }
+  inc[t] = hot_increments(t);
+  if (t < 16) cnt[t] = 0;
+  return in_smem;
+}
+
+// The owner join of one pod with owner UID u: -1 = orphaned (IsOrphanedPod), -2 = owned by none of the driver DaemonSets
+// (dropped), else the DaemonSet's index. Linear probing; the table is at most a quarter full.
+__device__ __forceinline__ int build_join(const ulonglong2& u, const ulonglong2* table, const int* order, unsigned slot_mask) {
+  int d = -2;
+  if ((u.x | u.y) == 0ull) {
+    d = -1;  // IsOrphanedPod
+  } else {
+    unsigned slot = ust_uid_hash(u.x, u.y) & slot_mask;
+    for (;;) {
+      const ulonglong2 e = table[slot];
+      if (e.x == u.x && e.y == u.y) { d = order[slot]; break; }
+      if ((e.x | e.y) == 0ull) break;  // empty slot: not a driver DaemonSet's pod
+      slot = (slot + 1u) & slot_mask;
+    }
+  }
+  return d;
+}
+
+// The counts of one existing pod with hot byte hb; `owned` = not dropped by the join. In the snapshot unless dropped or
+// marked pending-unscheduled by the host (code 14).
+__device__ __forceinline__ void build_count(unsigned hb, bool owned, const unsigned long long* inc, uint32_t (&B)[4], uint32_t& lo,
+                                            uint32_t& hi, int& pending, long long& excluded) {
+  if (owned && (hb & 15u) < 14u) {
+    const unsigned long long v = inc[hb];
+    lo += (uint32_t)v;
+    hi += (uint32_t)(v >> 32);
+  } else {
+    excluded++;
+  }
+  if ((++pending & 7) == 0) widen(lo, hi, B);
+}
+
+// Per-DaemonSet owned-pod counts (before the pending-skip, upgrade_state.go:128), whole warp; d < 0 counts for none. A
+// handful of DaemonSets (the usual case): eight byte counters packed in a register, flushed with the other counters;
+// otherwise one atomic per distinct DaemonSet per warp.
+__device__ __forceinline__ void build_count_ds(int d, unsigned long long& dsl, unsigned int* cnt_ds, unsigned long long* ds_count,
+                                               int n_ds, bool in_smem) {
+  if (n_ds <= 8) {
+    if (d >= 0) dsl += 1ull << (8 * d);
+  } else {
+    const unsigned act = __ballot_sync(kFull, d >= 0);
+    if (d >= 0) {
+      const unsigned peers = __match_any_sync(act, d);
+      if ((threadIdx.x & 31) == __ffs(peers) - 1) {
+        if (in_smem) atomicAdd(&cnt_ds[d], (unsigned)__popc(peers));
+        else atomicAdd(&ds_count[d], (unsigned long long)__popc(peers));
+      }
+    }
+  }
+}
+
+// A thread's byte lanes and packed DaemonSet counts into shared memory; due every kBuildSpill pods and at the end.
+__device__ __forceinline__ void build_spill(uint32_t (&B)[4], uint32_t& lo, uint32_t& hi, int& pending, unsigned long long& dsl,
+                                            unsigned int* cnt, unsigned int* cnt_ds) {
+  widen(lo, hi, B);
+#pragma unroll
+  for (int f = 0; f < 16; f++) {
+    const unsigned v = field_of(B, f);
+    if (v) atomicAdd(&cnt[f], v);
+  }
+  if (dsl) {
+#pragma unroll
+    for (int q = 0; q < 8; q++) {
+      const unsigned v = (unsigned)(dsl >> (8 * q)) & 0xFFu;
+      if (v) atomicAdd(&cnt_ds[q], v);
+    }
+    dsl = 0;
+  }
+  B[0] = B[1] = B[2] = B[3] = 0;
+  pending = 0;
+}
+
+// Epilogue, whole CTA, after the last spill and a barrier: fields 0..13 per state code, 14 unavailable, 15 candidates ->
+// ws->bs_acc[0..13], [16], [17]; the pods in no bucket -> ws->bs_acc[UST_STATE_EXCLUDED]; the per-DaemonSet counts ->
+// ds_count.
+__device__ __forceinline__ void build_finish(int t, long long excluded, const unsigned int* cnt, const unsigned int* cnt_ds,
+                                             unsigned long long* ds_count, int n_ds, bool in_smem, UstWorkspace* ws) {
+  for (int o = 16; o > 0; o >>= 1) excluded += __shfl_xor_sync(kFull, excluded, o);
+  if ((t & 31) == 0 && excluded) atomicAdd(&ws->bs_acc[UST_STATE_EXCLUDED], (unsigned long long)excluded);
+  if (t < 14) { if (cnt[t]) atomicAdd(&ws->bs_acc[t], (unsigned long long)cnt[t]); }
+  else if (t == 14) { if (cnt[14]) atomicAdd(&ws->bs_acc[16], (unsigned long long)cnt[14]); }
+  else if (t == 15) { if (cnt[15]) atomicAdd(&ws->bs_acc[17], (unsigned long long)cnt[15]); }
+  if (in_smem)
+    for (int i = t; i < n_ds; i += kThreads)
+      if (cnt_ds[i]) atomicAdd(&ds_count[i], (unsigned long long)cnt_ds[i]);
+}
+
+// The sum over a CTA of every thread's count c: warp reduction, then one shared-memory atomic per warp into `tot`, which
+// the caller zeroed before a barrier. Whole CTA; `tot` holds the sum after the helper's barrier. The caller reads it on
+// one thread, which may also reset it for the next sum: the next barrier orders that reset before any new atomic.
+__device__ __forceinline__ void cta_sum(unsigned c, unsigned int& tot) {
+  c = __reduce_add_sync(kFull, c);
+  if ((threadIdx.x & 31) == 0 && c) atomicAdd(&tot, c);
+  __syncthreads();
+}
+
+// The first output position of this thread's c outputs when the CTA writes its outputs in thread order from
+// cta_off[blockIdx.x] on (the scanned CTA counts, ust_diff_scan_kernel): warp shuffle-up scan, per-warp totals in shared
+// memory, sum of the earlier warps. Whole CTA.
+__device__ __forceinline__ long long cta_first_pos(unsigned c, const unsigned int* __restrict__ cta_off) {
+  __shared__ unsigned int wtot[kWarps];
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  unsigned incl = c;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned u = __shfl_up_sync(kFull, incl, o);
+    if (lane >= o) incl += u;
+  }
+  if (lane == 31) wtot[warp] = incl;
+  __syncthreads();
+  unsigned before = 0;
+  for (int w = 0; w < warp; w++) before += wtot[w];
+  return (long long)cta_off[blockIdx.x] + before + incl - c;
+}
 
 // UID = false is the index form (ust_build_state: the host has already resolved the owner, ds_idx_in holds it; an index
-// outside [0, n_ds) counts for no DaemonSet): same counting machinery, no join, nothing dropped.
+// outside [0, n_ds) counts for no DaemonSet): same counting, no join, nothing dropped. A grid-stride loop over chunks of
+// kThreads * kBuildU pods.
 template <bool UID>
 __global__ void __launch_bounds__(kThreads) ust_build_state_uid_kernel(long long n, const uint8_t* __restrict__ hot,
                                                                        const ulonglong2* __restrict__ owner,
@@ -606,26 +742,10 @@ __global__ void __launch_bounds__(kThreads) ust_build_state_uid_kernel(long long
   __shared__ ulonglong2 tab[kUidTabSmem];
   __shared__ int ord[kUidTabSmem];
   __shared__ unsigned int cnt_ds[kUidTabSmem / 4];
-  __shared__ unsigned long long inc[256];  // hot byte -> sixteen 4-bit one-hot increments (fields as in the streaming pass)
+  __shared__ unsigned long long inc[256];
   __shared__ unsigned int cnt[16];
   const int t = threadIdx.x;
-  const bool in_smem = UID ? tab_slots <= kUidTabSmem : n_ds <= kUidTabSmem / 4;  // UID: then n_ds <= kUidTabSmem / 4 too
-  if (in_smem) {
-    if (UID)
-      for (int i = t; i < tab_slots; i += kThreads) { tab[i] = ds_tab[i]; ord[i] = ds_tab_idx[i]; }
-    for (int i = t; i < n_ds; i += kThreads) cnt_ds[i] = 0;
-  }
-  {
-    const unsigned b = t, code = b & 15u;
-    unsigned long long v = 0;
-    if (code < 14) {
-      v = 1ull << (4 * code);
-      if (b & (UST_HOT_UNSCHEDULABLE | UST_HOT_NOT_READY)) v |= 1ull << 56;
-      if (code == UST_STATE_UPGRADE_REQUIRED && !(b & UST_HOT_SKIP)) v |= 1ull << 60;
-    }
-    inc[b] = v;
-  }
-  if (t < 16) cnt[t] = 0;
+  const bool in_smem = build_prologue<UID>(tab, ord, cnt_ds, inc, cnt, n_ds, ds_tab, ds_tab_idx, tab_slots);
   __syncthreads();
   const ulonglong2* table = in_smem ? tab : ds_tab;
   const int* order = in_smem ? ord : ds_tab_idx;
@@ -633,33 +753,14 @@ __global__ void __launch_bounds__(kThreads) ust_build_state_uid_kernel(long long
   uint32_t B[4] = {0, 0, 0, 0}, lo = 0, hi = 0;
   int pending = 0;
   long long excluded = 0;
-  unsigned long long dsl = 0;  // n_ds <= 8: this thread's owned-pod count per DaemonSet, one byte each
-  auto spill = [&]() {
-    widen(lo, hi, B);
+  unsigned long long dsl = 0;
+  const long long stride = (long long)gridDim.x * kThreads * kBuildU;
+  for (long long i0 = (long long)blockIdx.x * kThreads * kBuildU; i0 < n; i0 += stride) {  // warp-uniform trip count
+    ulonglong2 u[kBuildU];
+    int dk[kBuildU];
+    unsigned hb[kBuildU];
 #pragma unroll
-    for (int f = 0; f < 16; f++) {
-      const unsigned v = p1_field(B, f);
-      if (v) atomicAdd(&cnt[f], v);
-    }
-    if (dsl) {
-#pragma unroll
-      for (int q = 0; q < 8; q++) {
-        const unsigned v = (unsigned)(dsl >> (8 * q)) & 0xFFu;
-        if (v) atomicAdd(&cnt_ds[q], v);
-      }
-      dsl = 0;
-    }
-    B[0] = B[1] = B[2] = B[3] = 0;
-    pending = 0;
-  };
-  constexpr int kU = 4;  // pods per thread and iteration: four 16-byte loads in flight
-  const long long stride = (long long)gridDim.x * kThreads * kU;
-  for (long long i0 = (long long)blockIdx.x * kThreads * kU; i0 < n; i0 += stride) {  // warp-uniform trip count
-    ulonglong2 u[kU];
-    int dk[kU];
-    unsigned hb[kU];
-#pragma unroll
-    for (int k = 0; k < kU; k++) {
+    for (int k = 0; k < kBuildU; k++) {
       const long long i = i0 + (long long)k * kThreads + t;
       u[k] = make_ulonglong2(0ull, 0ull);
       dk[k] = -1;
@@ -670,63 +771,21 @@ __global__ void __launch_bounds__(kThreads) ust_build_state_uid_kernel(long long
       }
     }
 #pragma unroll
-    for (int k = 0; k < kU; k++) {
+    for (int k = 0; k < kBuildU; k++) {
       const long long i = i0 + (long long)k * kThreads + t;
-      const bool valid = i < n;
       int d = -2;
-      if (valid) {
-        if (!UID) {
-          d = (dk[k] >= 0 && dk[k] < n_ds) ? dk[k] : -1;
-        } else if ((u[k].x | u[k].y) == 0ull) {
-          d = -1;  // IsOrphanedPod
-        } else {
-          unsigned slot = ust_uid_hash(u[k].x, u[k].y) & slot_mask;
-          for (;;) {  // linear probing; the table is at most a quarter full
-            const ulonglong2 e = table[slot];
-            if (e.x == u[k].x && e.y == u[k].y) { d = order[slot]; break; }
-            if ((e.x | e.y) == 0ull) break;  // empty slot: not a driver DaemonSet's pod
-            slot = (slot + 1u) & slot_mask;
-          }
-        }
+      if (i < n) {
+        d = UID ? build_join(u[k], table, order, slot_mask) : ((dk[k] >= 0 && dk[k] < n_ds) ? dk[k] : -1);
         if (UID) __stcs(ds_idx_out + i, d);
-        if (d != -2 && (hb[k] & 15u) < 14u) {  // in the snapshot (the host marks a pending-unscheduled pod with code 14)
-          const unsigned long long v = inc[hb[k]];
-          lo += (uint32_t)v;
-          hi += (uint32_t)(v >> 32);
-        } else {
-          excluded++;
-        }
-        if ((++pending & 7) == 0) widen(lo, hi, B);
+        build_count(hb[k], d != -2, inc, B, lo, hi, pending, excluded);
       }
-      // per-DaemonSet owned-pod counts (before the pending-skip, upgrade_state.go:128). A handful of DaemonSets
-      // (the usual case): eight byte counters packed in a register, flushed with the other counters; otherwise
-      // one atomic per distinct DaemonSet per warp
-      if (n_ds <= 8) {
-        if (d >= 0) dsl += 1ull << (8 * d);
-      } else {
-        const unsigned act = __ballot_sync(kFull, d >= 0);
-        if (d >= 0) {
-          const unsigned peers = __match_any_sync(act, d);
-          if ((t & 31) == __ffs(peers) - 1) {
-            if (in_smem) atomicAdd(&cnt_ds[d], (unsigned)__popc(peers));
-            else atomicAdd(&ds_count[d], (unsigned long long)__popc(peers));
-          }
-        }
-      }
+      build_count_ds(d, dsl, cnt_ds, ds_count, n_ds, in_smem);
     }
-    if (pending >= 240) spill();
+    if (pending >= kBuildSpill) build_spill(B, lo, hi, pending, dsl, cnt, cnt_ds);
   }
-  spill();
+  build_spill(B, lo, hi, pending, dsl, cnt, cnt_ds);
   __syncthreads();
-  // fields 0..13 per state code, 14 unavailable, 15 candidates -> ws->bs_acc[0..13], [16], [17]
-  for (int o = 16; o > 0; o >>= 1) excluded += __shfl_xor_sync(kFull, excluded, o);
-  if ((t & 31) == 0 && excluded) atomicAdd(&ws->bs_acc[UST_STATE_EXCLUDED], (unsigned long long)excluded);
-  if (t < 14) { if (cnt[t]) atomicAdd(&ws->bs_acc[t], (unsigned long long)cnt[t]); }
-  else if (t == 14) { if (cnt[14]) atomicAdd(&ws->bs_acc[16], (unsigned long long)cnt[14]); }
-  else if (t == 15) { if (cnt[15]) atomicAdd(&ws->bs_acc[17], (unsigned long long)cnt[15]); }
-  if (in_smem)
-    for (int i = t; i < n_ds; i += kThreads)
-      if (cnt_ds[i]) atomicAdd(&ds_count[i], (unsigned long long)cnt_ds[i]);
+  build_finish(t, excluded, cnt, cnt_ds, ds_count, n_ds, in_smem, ws);
 }
 
 __global__ void ust_build_state_finish_kernel(int n_ds, const int32_t* ds_desired, unsigned long long* ds_count,
@@ -755,11 +814,11 @@ __global__ void ust_build_state_finish_kernel(int n_ds, const int32_t* ds_desire
   for (int d = 0; d < n_ds; d++) ds_count[d] = 0;
 }
 
-// The resident driver-pod list of ust_build_state_delta. The join and the counts are those of ust_build_state_uid_kernel<true>
-// (same table, same counters, same finish kernel); the pass also compares each pod's owner index with the previous call's
-// and works in fixed tiles of kBuildTile pods, so that the changed count of every tile comes out of it: the scan of
-// ust_diff_scan_kernel and ust_build_state_write_kernel then compact the changed pods in index order. 21 B read + 4 B
-// written per pod here, 8 B read per pod by the write pass.
+// The resident driver-pod list of ust_build_state_delta: the join and the counts of the BuildState pieces above (same
+// finish kernel); the pass also compares each pod's owner index with the previous call's and works in fixed tiles of
+// kBuildTile pods, so that the changed count of every tile comes out of it (cta_sum): the scan of ust_diff_scan_kernel
+// and ust_build_state_write_kernel then compact the changed pods in index order. 21 B read + 4 B written per pod here,
+// 8 B read per pod by the write pass.
 constexpr int kBuildTile = 4096;  // pods per tile: 16 per thread
 
 __global__ void __launch_bounds__(kThreads) ust_build_state_delta_kernel(long long n, const uint8_t* __restrict__ hot,
@@ -776,22 +835,7 @@ __global__ void __launch_bounds__(kThreads) ust_build_state_delta_kernel(long lo
   __shared__ unsigned int cnt[16];
   __shared__ unsigned int tile_changed;
   const int t = threadIdx.x;
-  const bool in_smem = tab_slots <= kUidTabSmem;  // then n_ds <= kUidTabSmem / 4 too
-  if (in_smem) {
-    for (int i = t; i < tab_slots; i += kThreads) { tab[i] = ds_tab[i]; ord[i] = ds_tab_idx[i]; }
-    for (int i = t; i < n_ds; i += kThreads) cnt_ds[i] = 0;
-  }
-  {
-    const unsigned b = t, code = b & 15u;
-    unsigned long long v = 0;
-    if (code < 14) {
-      v = 1ull << (4 * code);
-      if (b & (UST_HOT_UNSCHEDULABLE | UST_HOT_NOT_READY)) v |= 1ull << 56;
-      if (code == UST_STATE_UPGRADE_REQUIRED && !(b & UST_HOT_SKIP)) v |= 1ull << 60;
-    }
-    inc[b] = v;
-  }
-  if (t < 16) cnt[t] = 0;
+  const bool in_smem = build_prologue<true>(tab, ord, cnt_ds, inc, cnt, n_ds, ds_tab, ds_tab_idx, tab_slots);
   if (t == 0) tile_changed = 0;
   __syncthreads();
   const ulonglong2* table = in_smem ? tab : ds_tab;
@@ -801,35 +845,16 @@ __global__ void __launch_bounds__(kThreads) ust_build_state_delta_kernel(long lo
   int pending = 0;
   long long excluded = 0;
   unsigned long long dsl = 0;
-  auto spill = [&]() {
-    widen(lo, hi, B);
-#pragma unroll
-    for (int f = 0; f < 16; f++) {
-      const unsigned v = p1_field(B, f);
-      if (v) atomicAdd(&cnt[f], v);
-    }
-    if (dsl) {
-#pragma unroll
-      for (int q = 0; q < 8; q++) {
-        const unsigned v = (unsigned)(dsl >> (8 * q)) & 0xFFu;
-        if (v) atomicAdd(&cnt_ds[q], v);
-      }
-      dsl = 0;
-    }
-    B[0] = B[1] = B[2] = B[3] = 0;
-    pending = 0;
-  };
-  constexpr int kU = 4;
   const long long tiles = (n + kBuildTile - 1) / kBuildTile;
   for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {  // CTA-uniform trip counts
     unsigned changed = 0;
-    for (int j = 0; j < kBuildTile; j += kThreads * kU) {
+    for (int j = 0; j < kBuildTile; j += kThreads * kBuildU) {
       const long long i0 = tile * kBuildTile + j;
-      ulonglong2 u[kU];
-      unsigned hb[kU];
-      int pv[kU];
+      ulonglong2 u[kBuildU];
+      unsigned hb[kBuildU];
+      int pv[kBuildU];
 #pragma unroll
-      for (int k = 0; k < kU; k++) {
+      for (int k = 0; k < kBuildU; k++) {
         const long long i = i0 + (long long)k * kThreads + t;
         u[k] = make_ulonglong2(0ull, 0ull);
         hb[k] = UST_STATE_EXCLUDED;
@@ -837,64 +862,26 @@ __global__ void __launch_bounds__(kThreads) ust_build_state_delta_kernel(long lo
         if (i < n) { u[k] = __ldcs(owner + i); hb[k] = __ldg(hot + i); pv[k] = __ldcs(prev + i); }
       }
 #pragma unroll
-      for (int k = 0; k < kU; k++) {
+      for (int k = 0; k < kBuildU; k++) {
         const long long i = i0 + (long long)k * kThreads + t;
-        const bool valid = i < n;
         int d = -2;
-        if (valid) {
-          if ((u[k].x | u[k].y) == 0ull) {
-            d = -1;  // IsOrphanedPod
-          } else {
-            unsigned slot = ust_uid_hash(u[k].x, u[k].y) & slot_mask;
-            for (;;) {
-              const ulonglong2 e = table[slot];
-              if (e.x == u[k].x && e.y == u[k].y) { d = order[slot]; break; }
-              if ((e.x | e.y) == 0ull) break;
-              slot = (slot + 1u) & slot_mask;
-            }
-          }
+        if (i < n) {
+          d = build_join(u[k], table, order, slot_mask);
           __stcs(cur + i, d);
           changed += d != pv[k] ? 1u : 0u;
-          if (d != -2 && (hb[k] & 15u) < 14u) {
-            const unsigned long long v = inc[hb[k]];
-            lo += (uint32_t)v;
-            hi += (uint32_t)(v >> 32);
-          } else {
-            excluded++;
-          }
-          if ((++pending & 7) == 0) widen(lo, hi, B);
+          build_count(hb[k], d != -2, inc, B, lo, hi, pending, excluded);
         }
-        if (n_ds <= 8) {
-          if (d >= 0) dsl += 1ull << (8 * d);
-        } else {
-          const unsigned act = __ballot_sync(kFull, d >= 0);
-          if (d >= 0) {
-            const unsigned peers = __match_any_sync(act, d);
-            if ((t & 31) == __ffs(peers) - 1) {
-              if (in_smem) atomicAdd(&cnt_ds[d], (unsigned)__popc(peers));
-              else atomicAdd(&ds_count[d], (unsigned long long)__popc(peers));
-            }
-          }
-        }
+        build_count_ds(d, dsl, cnt_ds, ds_count, n_ds, in_smem);
       }
-      if (pending >= 240) spill();
+      if (pending >= kBuildSpill) build_spill(B, lo, hi, pending, dsl, cnt, cnt_ds);
     }
-    changed = __reduce_add_sync(kFull, changed);
-    if ((t & 31) == 0 && changed) atomicAdd(&tile_changed, changed);
-    __syncthreads();
+    cta_sum(changed, tile_changed);
     if (t == 0) { tile_count[tile] = tile_changed; tile_changed = 0; }
     __syncthreads();
   }
-  spill();
+  build_spill(B, lo, hi, pending, dsl, cnt, cnt_ds);
   __syncthreads();
-  for (int o = 16; o > 0; o >>= 1) excluded += __shfl_xor_sync(kFull, excluded, o);
-  if ((t & 31) == 0 && excluded) atomicAdd(&ws->bs_acc[UST_STATE_EXCLUDED], (unsigned long long)excluded);
-  if (t < 14) { if (cnt[t]) atomicAdd(&ws->bs_acc[t], (unsigned long long)cnt[t]); }
-  else if (t == 14) { if (cnt[14]) atomicAdd(&ws->bs_acc[16], (unsigned long long)cnt[14]); }
-  else if (t == 15) { if (cnt[15]) atomicAdd(&ws->bs_acc[17], (unsigned long long)cnt[15]); }
-  if (in_smem)
-    for (int i = t; i < n_ds; i += kThreads)
-      if (cnt_ds[i]) atomicAdd(&ds_count[i], (unsigned long long)cnt_ds[i]);
+  build_finish(t, excluded, cnt, cnt_ds, ds_count, n_ds, in_smem, ws);
 }
 
 // The ordered write of ust_build_state_delta's sparse outputs: tile b's changed pods go to positions tile_off[b] .. (the
@@ -903,8 +890,7 @@ __global__ void __launch_bounds__(kThreads) ust_build_state_write_kernel(long lo
                                                                          const int32_t* __restrict__ prev,
                                                                          const unsigned int* __restrict__ tile_off, long long cap,
                                                                          long long* __restrict__ out_idx, int32_t* __restrict__ out_ds) {
-  __shared__ unsigned int wtot[kWarps];
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int t = threadIdx.x;
   const long long i0 = (long long)blockIdx.x * kBuildTile + 16 * t;
   int c16[16];
   unsigned m = 0;
@@ -923,18 +909,7 @@ __global__ void __launch_bounds__(kThreads) ust_build_state_write_kernel(long lo
       if (i0 + k < n) { c16[k] = cur[i0 + k]; m |= (unsigned)(c16[k] != prev[i0 + k]) << k; }
     }
   }
-  const unsigned c = __popc(m);
-  unsigned incl = c;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const unsigned u = __shfl_up_sync(kFull, incl, o);
-    if (lane >= o) incl += u;
-  }
-  if (lane == 31) wtot[warp] = incl;
-  __syncthreads();
-  unsigned before = 0;
-  for (int w = 0; w < warp; w++) before += wtot[w];
-  long long pos = (long long)tile_off[blockIdx.x] + before + incl - c;
+  long long pos = cta_first_pos(__popc(m), tile_off);
 #pragma unroll
   for (int k = 0; k < 16; k++) {
     if (!((m >> k) & 1u)) continue;
@@ -991,6 +966,27 @@ __device__ __forceinline__ long long splice_lower_bound(const long long* __restr
     if (__ldg(a + mid) < v) lo = mid + 1; else hi = mid;
   }
   return lo;
+}
+// The last index r in [0, len) with a[r] <= v over a sorted array in global memory (0 when there is none; every caller
+// searches a v >= a[0]). Run and segment starts: long long for node positions, int32_t for pod positions.
+template <class T>
+__device__ __forceinline__ long long last_le(const T* __restrict__ a, long long len, T v) {
+  long long lo = 0, hi = len;
+  while (hi - lo > 1) {
+    const long long mid = (lo + hi) >> 1;
+    if (__ldg(a + mid) <= v) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+// ... and over a staged slice a[0, len), from a hint r with a[r] <= v (0, or the answer for a smaller v)
+template <class T>
+__device__ __forceinline__ int last_le_from(const T* a, int r, int len, T v) {
+  int hi = len;
+  while (hi - r > 1) {
+    const int mid = (r + hi) >> 1;
+    if (a[mid] <= v) r = mid; else hi = mid;
+  }
+  return r;
 }
 
 __global__ void __launch_bounds__(kThreads) ust_splice_kernel(long long n, long long n_rm, const long long* __restrict__ rm,
@@ -1104,15 +1100,7 @@ __device__ __forceinline__ void gather_runs(long long n, long long n_runs, const
   const long long b0 = (long long)blockIdx.x * kGatherTile;
   if (b0 >= n) return;  // n == 0: the one CTA of the launch has nothing to do
   const long long b1 = b0 + kGatherTile < n ? b0 + kGatherTile : n;
-  if (t < 2) {  // the last run that starts at or before b0 (t = 0) / b1 - 1 (t = 1)
-    const long long v = t ? b1 - 1 : b0;
-    long long lo = 0, hi = n_runs;
-    while (hi - lo > 1) {
-      const long long mid = (lo + hi) >> 1;
-      if (__ldg(run_off + mid) <= v) lo = mid; else hi = mid;
-    }
-    s_runs[t] = lo;
-  }
+  if (t < 2) s_runs[t] = last_le(run_off, n_runs, t ? b1 - 1 : b0);  // the last run that starts at or before b0 / b1 - 1
   __syncthreads();
   const long long r0 = s_runs[0];
   const int nr = (int)(s_runs[1] - r0 + 1);
@@ -1123,11 +1111,7 @@ __device__ __forceinline__ void gather_runs(long long n, long long n_runs, const
 #pragma unroll 4
   for (int j = t; j < len; j += kThreads) {
     const long long p = b0 + j;
-    int hi = nr;
-    while (hi - r > 1) {
-      const int mid = (r + hi) >> 1;
-      if (s_off[mid] <= p) r = mid; else hi = mid;
-    }
+    r = last_le_from(s_off, r, nr, p);
     copy(p, s_src[r], p - s_off[r]);
   }
 }
@@ -1206,8 +1190,8 @@ __global__ void __launch_bounds__(kThreads) ust_pods_scatter_kernel(long long n_
 }
 
 // The new CSR as 2 n_lists + 1 runs of new pod positions [run_start[r], run_start[r + 1]) (run_start[2 n_lists + 1] =
-// new_total): even r = 2k, the unchanged nodes between list k - 1 and list k, old pods from run_src[r] on; odd r = 2k + 1,
-// new list k, from new_flags[run_src[r]] on. Runs may be empty.
+// new_total), in the encoding of gather_pods: run 2k, the unchanged nodes between list k - 1 and list k, old pods from
+// run_src[2k] on; run 2k + 1, new list k, run_src[2k + 1] = -1 - new_off[k]. Runs may be empty.
 __global__ void __launch_bounds__(kThreads) ust_pods_runs_kernel(long long n_lists, const long long* __restrict__ node_idx,
                                                                  const int32_t* __restrict__ new_off, const int32_t* __restrict__ shift,
                                                                  const int32_t* __restrict__ off, int new_total,
@@ -1220,7 +1204,7 @@ __global__ void __launch_bounds__(kThreads) ust_pods_runs_kernel(long long n_lis
     run_src[2 * k] = prev_end;
     if (k < n_lists) {
       run_start[2 * k + 1] = __ldg(off + __ldg(node_idx + k)) + d;
-      run_src[2 * k + 1] = __ldg(new_off + k);
+      run_src[2 * k + 1] = -1 - __ldg(new_off + k);
     } else {
       run_start[2 * k + 1] = new_total;
     }
@@ -1240,8 +1224,64 @@ __device__ __forceinline__ uint4 pods8_at(const uint16_t* __restrict__ src, int 
   return make_uint4(__funnelshift_r(v0, v1, sh), __funnelshift_r(v1, v2, sh), __funnelshift_r(v2, v3, sh), __funnelshift_r(v3, v4, sh));
 }
 
+// The runs of a pod tile, staged in shared memory by gather_pods
+struct PodRunsSmem {
+  int32_t start[kRelayRuns + 1];
+  int32_t src[kRelayRuns];
+};
+
+// The pod half of ust_pods_relayout_kernel and ust_pods_reorder_kernel: new pod_flags [q0, q1), tile blockIdx.x of
+// kRelayTile positions, from n_runs runs. Run r covers new positions [run_start[r], run_start[r + 1]) and reads old pods
+// run_src[r], run_src[r] + 1, ... (run_src >= 0) or new-list pods -1 - run_src[r], ... (run_src < 0). The CTA finds its
+// tile's runs once, by binary search, and stages them in shared memory (a tile that meets more than kRelayRuns of them,
+// empty ones included, searches them in global memory instead). A chunk of 8 pods inside one run is one shifted 16-byte
+// copy (pods8_at), a chunk across runs goes pod by pod; 16-byte stores.
+__device__ __forceinline__ void gather_pods(long long n_runs, const int32_t* __restrict__ run_start, const int32_t* __restrict__ run_src,
+                                            const uint16_t* __restrict__ flags, const uint16_t* __restrict__ new_flags,
+                                            uint16_t* __restrict__ o_flags, int new_total, PodRunsSmem& sm, long long (&bounds)[2]) {
+  const int t = threadIdx.x;
+  const int q0 = blockIdx.x * kRelayTile;
+  const int q1 = q0 + kRelayTile < new_total ? q0 + kRelayTile : new_total;
+  if (t < 2) bounds[t] = last_le(run_start, n_runs, t ? q1 - 1 : q0);  // the last run that starts at or before q0 / q1 - 1
+  __syncthreads();
+  const long long r0 = bounds[0];
+  const int nr = (int)(bounds[1] - r0 + 1);
+  const bool staged = nr <= kRelayRuns;  // empty runs are not bounded by the tile
+  if (staged) {
+    for (int j = t; j <= nr; j += kThreads) sm.start[j] = __ldg(run_start + r0 + j);
+    for (int j = t; j < nr; j += kThreads) sm.src[j] = __ldg(run_src + r0 + j);
+  }
+  __syncthreads();
+  const int32_t* S = staged ? sm.start : run_start + r0;
+  const int32_t* R = staged ? sm.src : run_src + r0;
+  const int chunks = (q1 - q0 + 7) >> 3;
+#pragma unroll 2
+  for (int c = t; c < chunks; c += kThreads) {
+    const int q = q0 + 8 * c;
+    int r = last_le_from(S, 0, nr, q);  // the run that holds q
+    uint4 v;
+    if (q + 8 <= S[r + 1] && q + 8 <= new_total) {  // the chunk lies in one run: one shifted 16-byte copy
+      const int src = R[r];
+      v = pods8_at(src >= 0 ? flags : new_flags, (src >= 0 ? src : -1 - src) + (q - S[r]));
+    } else {  // it straddles runs (or the end of the array): pod by pod
+      uint32_t w[4] = {0u, 0u, 0u, 0u};
+#pragma unroll
+      for (int e = 0; e < 8; e++) {
+        const int p = q + e;
+        if (p >= new_total) break;
+        while (S[r + 1] <= p) r++;
+        const int src = R[r];
+        const uint16_t x = __ldg((src >= 0 ? flags : new_flags) + (src >= 0 ? src : -1 - src) + (p - S[r]));
+        w[e >> 1] |= (uint32_t)x << (16 * (e & 1));
+      }
+      v = make_uint4(w[0], w[1], w[2], w[3]);
+    }
+    *reinterpret_cast<uint4*>(o_flags + q) = v;
+  }
+}
+
 union RelayoutSmem {
-  struct { int32_t start[kRelayRuns + 1]; int32_t src[kRelayRuns]; } pods;
+  PodRunsSmem pods;
   struct { long long idx[kOffTile]; int32_t shift[kOffTile + 1]; } offs;
 };
 
@@ -1279,57 +1319,8 @@ __global__ void __launch_bounds__(kThreads) ust_pods_relayout_kernel(long long n
     }
     return;
   }
-  // ---- pods: the runs that cover new positions [q0, q1)
-  const long long n_runs = 2 * n_lists + 1;
-  const int q0 = blockIdx.x * kRelayTile;
-  const int q1 = q0 + kRelayTile < new_total ? q0 + kRelayTile : new_total;
-  if (t < 2) {  // the last run that starts at or before q0 (t = 0) / q1 - 1 (t = 1)
-    const int v = t ? q1 - 1 : q0;
-    long long lo = 0, hi = n_runs;
-    while (hi - lo > 1) {
-      const long long mid = (lo + hi) >> 1;
-      if (__ldg(run_start + mid) <= v) lo = mid; else hi = mid;
-    }
-    s_bounds[t] = lo;
-  }
-  __syncthreads();
-  const long long r0 = s_bounds[0];
-  const int nr = (int)(s_bounds[1] - r0 + 1);
-  // empty runs are not bounded by the tile: a tile that meets more runs than fit reads them from global memory
-  const bool staged = nr <= kRelayRuns;
-  if (staged) {
-    for (int j = t; j <= nr; j += kThreads) sm.pods.start[j] = __ldg(run_start + r0 + j);
-    for (int j = t; j < nr; j += kThreads) sm.pods.src[j] = __ldg(run_src + r0 + j);
-  }
-  __syncthreads();
-  const int32_t* S = staged ? sm.pods.start : run_start + r0;
-  const int32_t* R = staged ? sm.pods.src : run_src + r0;
-  const int chunks = (q1 - q0 + 7) >> 3;
-#pragma unroll 2
-  for (int c = t; c < chunks; c += kThreads) {
-    const int q = q0 + 8 * c;
-    int r = 0, hi = nr;  // the run that holds q
-    while (hi - r > 1) {
-      const int mid = (r + hi) >> 1;
-      if (S[mid] <= q) r = mid; else hi = mid;
-    }
-    uint4 v;
-    if (q + 8 <= S[r + 1] && q + 8 <= new_total) {  // the chunk lies in one run: one shifted 16-byte copy
-      v = pods8_at(((r0 + r) & 1) ? new_flags : flags, R[r] + (q - S[r]));
-    } else {  // it straddles runs (or the end of the array): pod by pod
-      uint32_t w[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-      for (int e = 0; e < 8; e++) {
-        const int p = q + e;
-        if (p >= new_total) break;
-        while (S[r + 1] <= p) r++;
-        const uint16_t* src = ((r0 + r) & 1) ? new_flags : flags;
-        w[e >> 1] |= (uint32_t)__ldg(src + R[r] + (p - S[r])) << (16 * (e & 1));
-      }
-      v = make_uint4(w[0], w[1], w[2], w[3]);
-    }
-    *reinterpret_cast<uint4*>(o_flags + q) = v;
-  }
+  // ---- pods
+  gather_pods(2 * n_lists + 1, run_start, run_src, flags, new_flags, o_flags, new_total, sm.pods, s_bounds);
 }
 
 // The pod-list CSR of the resident pod-list snapshot in a new node order, with replaced and inserted lists
@@ -1353,7 +1344,7 @@ __global__ void __launch_bounds__(kThreads) ust_pods_reorder_runs_kernel(long lo
 }
 
 union PodsReorderSmem {
-  struct { int32_t start[kRelayRuns + 1]; int32_t src[kRelayRuns]; } pods;
+  PodRunsSmem pods;
   struct { long long node[kReorderOffTile]; long long src[kReorderOffTile]; int32_t start[kReorderOffTile]; int32_t psrc[kReorderOffTile]; } offs;
 };
 
@@ -1376,15 +1367,7 @@ __global__ void __launch_bounds__(kThreads) ust_pods_reorder_kernel(long long n,
     const long long b0 = (long long)(blockIdx.x - pod_ctas) * kReorderOffTile;
     const long long b1 = b0 + kReorderOffTile < n ? b0 + kReorderOffTile : n;  // nodes [b0, b1) of [0, n)
     if (b1 > b0) {
-      if (t < 2) {  // the last segment that starts at or before b0 (t = 0) / b1 - 1 (t = 1)
-        const long long v = t ? b1 - 1 : b0;
-        long long lo = 0, hi = n_segs;
-        while (hi - lo > 1) {
-          const long long mid = (lo + hi) >> 1;
-          if (__ldg(seg_node + mid) <= v) lo = mid; else hi = mid;
-        }
-        s_bounds[t] = lo;
-      }
+      if (t < 2) s_bounds[t] = last_le(seg_node, n_segs, t ? b1 - 1 : b0);  // the last segment that starts at or before b0 / b1 - 1
       __syncthreads();
       const long long s0 = s_bounds[0];
       const int ns = (int)(s_bounds[1] - s0 + 1);  // every segment holds a node: at most kReorderOffTile of them
@@ -1398,11 +1381,7 @@ __global__ void __launch_bounds__(kThreads) ust_pods_reorder_kernel(long long n,
       int r = 0;
       for (int j = t; j < (int)(b1 - b0); j += kThreads) {
         const long long i = b0 + j;
-        int hi = ns;
-        while (hi - r > 1) {
-          const int mid = (r + hi) >> 1;
-          if (sm.offs.node[mid] <= i) r = mid; else hi = mid;
-        }
+        r = last_le_from(sm.offs.node, r, ns, i);
         const long long src = sm.offs.src[r];
         o_off[i] = src >= 0 ? sm.offs.start[r] + (__ldcs(off + src + (i - sm.offs.node[r])) - sm.offs.psrc[r]) : sm.offs.start[r];
       }
@@ -1410,58 +1389,8 @@ __global__ void __launch_bounds__(kThreads) ust_pods_reorder_kernel(long long n,
     if (b0 <= n && n < b0 + kReorderOffTile && t == 0) o_off[n] = new_total;
     return;
   }
-  // ---- pods: the segments that cover new positions [q0, q1) (empty ones included)
-  const int q0 = blockIdx.x * kRelayTile;
-  const int q1 = q0 + kRelayTile < new_total ? q0 + kRelayTile : new_total;
-  if (t < 2) {  // the last segment that starts at or before q0 (t = 0) / q1 - 1 (t = 1)
-    const int v = t ? q1 - 1 : q0;
-    long long lo = 0, hi = n_segs;
-    while (hi - lo > 1) {
-      const long long mid = (lo + hi) >> 1;
-      if (__ldg(pod_start + mid) <= v) lo = mid; else hi = mid;
-    }
-    s_bounds[t] = lo;
-  }
-  __syncthreads();
-  const long long r0 = s_bounds[0];
-  const int nr = (int)(s_bounds[1] - r0 + 1);
-  // empty segments are not bounded by the tile: a tile that meets more of them than fit reads them from global memory
-  const bool staged = nr <= kRelayRuns;
-  if (staged) {
-    for (int j = t; j <= nr; j += kThreads) sm.pods.start[j] = __ldg(pod_start + r0 + j);
-    for (int j = t; j < nr; j += kThreads) sm.pods.src[j] = __ldg(pod_src + r0 + j);
-  }
-  __syncthreads();
-  const int32_t* S = staged ? sm.pods.start : pod_start + r0;
-  const int32_t* R = staged ? sm.pods.src : pod_src + r0;
-  const int chunks = (q1 - q0 + 7) >> 3;
-#pragma unroll 2
-  for (int c = t; c < chunks; c += kThreads) {
-    const int q = q0 + 8 * c;
-    int r = 0, hi = nr;  // the segment that holds q
-    while (hi - r > 1) {
-      const int mid = (r + hi) >> 1;
-      if (S[mid] <= q) r = mid; else hi = mid;
-    }
-    uint4 v;
-    if (q + 8 <= S[r + 1] && q + 8 <= new_total) {  // the chunk lies in one segment: one shifted 16-byte copy
-      const int src = R[r];
-      v = src >= 0 ? pods8_at(flags, src + (q - S[r])) : pods8_at(new_flags, -1 - src + (q - S[r]));
-    } else {  // it straddles segments (or the end of the array): pod by pod
-      uint32_t w[4] = {0u, 0u, 0u, 0u};
-#pragma unroll
-      for (int e = 0; e < 8; e++) {
-        const int p = q + e;
-        if (p >= new_total) break;
-        while (S[r + 1] <= p) r++;
-        const int src = R[r];
-        const uint16_t x = src >= 0 ? __ldg(flags + src + (p - S[r])) : __ldg(new_flags + (-1 - src) + (p - S[r]));
-        w[e >> 1] |= (uint32_t)x << (16 * (e & 1));
-      }
-      v = make_uint4(w[0], w[1], w[2], w[3]);
-    }
-    *reinterpret_cast<uint4*>(o_flags + q) = v;
-  }
+  // ---- pods: the segments are the runs of gather_pods
+  gather_pods(n_segs, pod_start, pod_src, flags, new_flags, o_flags, new_total, sm.pods, s_bounds);
 }
 
 // Rollout simulation (SURVEY 8f.3): the state feedback between two reconciles. Untimed (sp.timed == 0): "ideal actuators" - every call
@@ -1634,10 +1563,8 @@ __global__ void __launch_bounds__(kThreads) ust_diff_count_kernel(long long n, c
   if (threadIdx.x == 0) tot = 0;
   __syncthreads();
   const long long i0 = (long long)blockIdx.x * kDiffBlock + 16 * threadIdx.x;
-  unsigned c = i0 < n ? __popc(diff_mask16<OUTCOME>(next, act, oc, pnext, pact, poc, i0, n)) : 0u;
-  c = __reduce_add_sync(kFull, c);
-  if ((threadIdx.x & 31) == 0 && c) atomicAdd(&tot, c);
-  __syncthreads();
+  const unsigned c = i0 < n ? __popc(diff_mask16<OUTCOME>(next, act, oc, pnext, pact, poc, i0, n)) : 0u;
+  cta_sum(c, tot);
   if (threadIdx.x == 0) block_count[blockIdx.x] = tot;
 }
 // exclusive scan of the block counts in place (one CTA); total -> *n_out
@@ -1675,22 +1602,10 @@ __global__ void __launch_bounds__(kThreads) ust_diff_write_kernel(long long n, c
                                                                   const unsigned int* __restrict__ block_off, long long cap,
                                                                   long long* __restrict__ out_idx, uint8_t* __restrict__ out_next,
                                                                   uint16_t* __restrict__ out_act, uint8_t* __restrict__ out_oc) {
-  __shared__ unsigned int wtot[kWarps];
-  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int t = threadIdx.x;
   const long long i0 = (long long)blockIdx.x * kDiffBlock + 16 * t;
   const unsigned m = i0 < n ? diff_mask16<OUTCOME>(next, act, oc, pnext, pact, poc, i0, n) : 0u;
-  const unsigned c = __popc(m);
-  unsigned incl = c;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const unsigned u = __shfl_up_sync(kFull, incl, o);
-    if (lane >= o) incl += u;
-  }
-  if (lane == 31) wtot[warp] = incl;
-  __syncthreads();
-  unsigned before = 0;
-  for (int w = 0; w < warp; w++) before += wtot[w];
-  long long pos = (long long)block_off[blockIdx.x] + before + incl - c;
+  long long pos = cta_first_pos(__popc(m), block_off);
   unsigned mm = m;
   while (mm) {
     const int k = __ffs(mm) - 1;

@@ -91,20 +91,13 @@ static_assert(UST_STREAM_CTAS_PER_SM * ((kStreamWarps + 3) / 4) * 32 * UST_STREA
                       ((kVerifyWarps + 3) / 4) * 32 * UST_VERIFY_MAXREG <= kRegsPerSubPartition,
               "registers: the streaming CTAs and a verification CTA must fit on one SM sub-partition");
 
-// Byte-sliced SIMD-in-register counting. The hot-byte table maps a hot byte to sixteen 4-bit one-hot increments packed
-// in 64 bits (fields 0-13: state code, 14: unavailable, 15: upgrade candidate) next to the node's table window; a
-// thread sums the entries of its nodes of two groups (no field can exceed 8), widens the nibbles to byte lanes,
-// and keeps going. No atomics until the byte lanes fill up or the CTA runs out of tiles.
+// Byte-sliced SIMD-in-register counting (hot_increments, ust_common.cuh). The hot-byte table holds a hot byte's 64-bit
+// increment word next to the node's table window; a thread sums the entries of its nodes of two groups (no field can
+// exceed 8), widens the nibbles to byte lanes, and keeps going. No atomics until the byte lanes fill up or the CTA runs
+// out of tiles.
 __device__ __forceinline__ uint4 hot_entry(unsigned b) {
-  // GetCurrentUnavailableNodes (common_manager.go:146-165) counts every snapshot entry that is cordoned or
-  // not ready; an upgrade candidate is upgrade-required and not marked skip (upgrade_inplace.go:82)
   const unsigned code = b & 15u;
-  unsigned long long v = 0;
-  if (code < 14) {
-    v = 1ull << (4 * code);
-    if (b & (UST_HOT_UNSCHEDULABLE | UST_HOT_NOT_READY)) v |= 1ull << 56;
-    if (code == UST_STATE_UPGRADE_REQUIRED && !(b & UST_HOT_SKIP)) v |= 1ull << 60;
-  }
+  const unsigned long long v = hot_increments(b);
   uint32_t x = 0, y = 0;  // the state's lookup constants (ust_lut.h): 16 compile-time pairs
 #pragma unroll
   for (int s = 0; s < 16; s++)
@@ -112,17 +105,6 @@ __device__ __forceinline__ uint4 hot_entry(unsigned b) {
   return make_uint4(x, y, (uint32_t)v, (uint32_t)(v >> 32));
 }
 
-// byte lanes: B[0] = fields 0,2,4,6  B[1] = fields 1,3,5,7  B[2] = fields 8,10,12,14  B[3] = fields 9,11,13,15
-__device__ __forceinline__ unsigned field_of(const uint32_t (&B)[4], int f) {
-  return (B[(f >> 3) * 2 + (f & 1)] >> (8 * ((f & 7) >> 1))) & 0xFFu;
-}
-__device__ __forceinline__ void widen(uint32_t& lo, uint32_t& hi, uint32_t (&B)[4]) {
-  B[0] += lo & 0x0F0F0F0Fu;
-  B[1] += (lo >> 4) & 0x0F0F0F0Fu;
-  B[2] += hi & 0x0F0F0F0Fu;
-  B[3] += (hi >> 4) & 0x0F0F0F0Fu;
-  lo = hi = 0;
-}
 template <bool PODS>
 __device__ __forceinline__ void flush_counts(SS<PODS>& S, uint32_t (&B)[4]) {  // whole warp, converged
 #pragma unroll
