@@ -69,8 +69,9 @@ enum {
 
 /* ------------------------------------------------------------------------------------------------
  * flags[i] (uint32): one bit per reference predicate on the node / its driver pod.
- * Bits 0-4, 9, 10 and 22-31 are reserved for values the kernel derives itself (skip / unschedulable
- * from the hot byte, slot grant, pod-in-sync, pod-list summaries) and are ignored on input. The
+ * Bits 0-4, 9, 10, 22-24 and 28-31 are reserved for values the kernel derives itself (skip / unschedulable
+ * from the hot byte, slot grant, pod-in-sync, pod-list summaries) and are ignored on input; bits 25-27 are the
+ * validation start-time bits below. The
  * positions are chosen so that the bits each state's transition reads are contiguous (the kernel
  * indexes a per-state table with a 9-bit window of this word).
  * ---------------------------------------------------------------------------------------------- */
@@ -90,6 +91,12 @@ enum {
 #define UST_F_NM_PRESENT (1u << 20)        /* NodeUpgradeState.NodeMaintenance != nil            upgrade_requestor.go:420 */
 #define UST_F_NM_READY (1u << 21)          /* NodeMaintenance Ready condition with Reason Ready  upgrade_requestor.go:437-439 */
 #define UST_F_INPUT_MASK 0x003FF9E0u
+/* Validation start-time annotation of a validation-required node (validation_manager.go:139-175). Read only when the
+ * policy asks for UST_EVAL_VALIDATION (then by the pass that walks the validation pods, never through the transition
+ * table, so they stay outside UST_F_INPUT_MASK); ignored otherwise. */
+#define UST_F_VALIDATION_START_ANNO (1u << 25)    /* annotation ...-driver-upgrade-validation-start-time PRESENT  validation_manager.go:142 */
+#define UST_F_VALIDATION_START_INVALID (1u << 26) /* ... and strconv.ParseInt(value, 10, 64) fails                validation_manager.go:155-160 */
+#define UST_F_VALIDATION_TIMED_OUT (1u << 27)     /* ... parses and now > start + 600, evaluated by the encoder   validation_manager.go:32, :161 */
 
 /* ------------------------------------------------------------------------------------------------
  * pod_flags[p] (uint16): one entry per workload pod of a node (CSR by pod_off), used to evaluate
@@ -106,6 +113,12 @@ enum { UST_PHASE_OTHER = 0, UST_PHASE_PENDING = 1, UST_PHASE_RUNNING = 2, UST_PH
 #define UST_POD_MATCH_DELETION_FILTER (1u << 8) /* PodDeletionFilter(pod) == true     pod_manager.go:76,139,179 */
 #define UST_POD_MATCH_WAIT_SELECTOR (1u << 9)  /* matches WaitForCompletionSpec.PodSelector   pod_manager.go:263 */
 #define UST_POD_MATCH_DRAIN_SELECTOR (1u << 10) /* matches DrainSpec.PodSelector       drain_manager.go:86 */
+/* Validation pods (read only with UST_EVAL_VALIDATION; every other path ignores these two bits). A node's pods that
+ * match the validation selector must appear in the order the API List returns them: Validate walks them in that order
+ * (validation_manager.go:99-115), and the order can change its answer (INTEGRATION.md). */
+#define UST_POD_MATCH_VALIDATION_SELECTOR (1u << 11) /* matches the ValidationManager's podSelector      validation_manager.go:78-80 */
+#define UST_POD_READY (1u << 12)               /* Phase==Running && len(ContainerStatuses)!=0 && all Ready (init containers not
+                                                  considered)                                       validation_manager.go:118-136 */
 
 /* ------------------------------------------------------------------------------------------------
  * actions[i] (uint16): the actuator / provider calls ApplyState makes for node i, in addition to the
@@ -124,6 +137,10 @@ enum { UST_PHASE_OTHER = 0, UST_PHASE_PENDING = 1, UST_PHASE_RUNNING = 2, UST_PH
 #define UST_A_UNBLOCK_SAFE_LOAD (1u << 10)      /* safe_driver_load_manager.go:57-71 */
 #define UST_A_SET_WAIT_START (1u << 11)         /* pod_manager.go:336-345 (actuator evaluation only) */
 #define UST_A_CLEAR_WAIT_START (1u << 12)       /* pod_manager.go:301-302, :360 (actuator evaluation only) */
+/* ^ On a validation-required node (only with UST_EVAL_VALIDATION) these two name the VALIDATION start-time annotation
+ *   instead: SET = ChangeNodeUpgradeAnnotation(key, now) (validation_manager.go:145-146), CLEAR = set it to "null", i.e.
+ *   delete it (:106-113, :164-169). When both are set the clear comes first. Validate deletes the annotation once per
+ *   ready pod; the deletes are idempotent, so they are reported as one CLEAR. */
 #define UST_A_REQUESTOR_ANNO_CHANGE (1u << 13)  /* upgrade_requestor.go:302-306 (set), :476-480 (clear) */
 #define UST_A_NM_CREATE_OR_DELETE (1u << 14)    /* upgrade_requestor.go:296, :482 */
 #define UST_A_ERROR (1u << 15)                  /* ApplyState returns an error at this node */
@@ -152,9 +169,31 @@ typedef struct ust_policy {
   int32_t wait_selector_set;       /* WaitForCompletion != nil && PodSelector != ""   common_manager.go:392 */
   int32_t wait_timeout_nonzero;    /* WaitForCompletionSpec.TimeoutSecond != 0       pod_manager.go:290 */
   int32_t use_maintenance_operator; /* StateOptions.Requestor.UseMaintenanceOperator  upgrade_state.go:291,302,321 */
-  int32_t evaluate_actuators;      /* 1: also fill actuator_outcome / wait-start actions from the
-                                         WAIT_* flag bits and, when given, the pod lists */
+  int32_t evaluate_actuators;      /* bit set, UST_EVAL_* below (0: neither) */
 } ust_policy;
+
+/* ust_policy.evaluate_actuators:
+ *   UST_EVAL_ACTUATORS   also fill actuator_outcome / wait-start actions from the WAIT_* flag bits and, when given, the
+ *                        pod lists. (Any non-zero value without UST_EVAL_VALIDATION means this, as it always has.)
+ *   UST_EVAL_VALIDATION  also answer ValidationManager.Validate (validation_manager.go:71-175) for every
+ *                        validation-required node from its pod lists instead of taking UST_F_VALIDATION_DONE: the pods
+ *                        with UST_POD_MATCH_VALIDATION_SELECTOR, walked in list order, and the UST_F_VALIDATION_START_*
+ *                        / _TIMED_OUT bits. Requires UST_EVAL_ACTUATORS and pod lists (value 3): UST_EVAL_VALIDATION
+ *                        alone (value 2), or on a call without pod lists (ust_apply_state* without pods, _packed, _delta,
+ *                        _delta_sparse, _delta_splice, _delta_reorder and both simulations), returns
+ *                        UST_ERR_INVALID_ARGUMENT before any device work. With policy->validation_enabled == 0 Validate
+ *                        is true without looking at any pod (the default manager's empty selector, common_manager.go:128).
+ *   For such a node, in ApplyState's order (common_manager.go:573-604): UST_A_UNBLOCK_SAFE_LOAD when UST_F_SAFE_LOAD, then
+ *     - no matching pod: not done, no annotation call;
+ *     - every matching pod ready: done (uncordon-required / upgrade-done as without the mode) + UST_A_CLEAR_WAIT_START;
+ *     - a ready pod before the first not-ready one: UST_A_CLEAR_WAIT_START + UST_A_SET_WAIT_START, not done (the delete
+ *       makes handleTimeout find no annotation, so such a node never times out);
+ *     - the first matching pod not ready: no annotation => UST_A_SET_WAIT_START; annotation invalid => ApplyState returns
+ *       UST_ERR_VALIDATION at this node (error_pass 10; it keeps its UST_A_UNBLOCK_SAFE_LOAD); timed out => next state
+ *       upgrade-failed + UST_A_CLEAR_WAIT_START; otherwise nothing.
+ *   actuator_outcome stays UST_OUTCOME_NONE for these nodes: Validate is synchronous. */
+#define UST_EVAL_ACTUATORS (1u << 0)
+#define UST_EVAL_VALIDATION (1u << 1)
 
 /* ------------------------------------------------------------------------------------------------
  * Cluster-wide results of one call (what CommonUpgradeStateManager's getters return,
@@ -170,7 +209,9 @@ enum {
   UST_ERR_POD_DELETION_SPEC = -6, /* "pod deletion spec should not be empty"     pod_manager.go:132-134 */
   UST_ERR_DS_UNSCHEDULED = -7,  /* "driver DaemonSet should not have Unscheduled pods"  upgrade_state.go:128-131 */
   UST_ERR_COMM = -8,            /* multi-GPU exchange failed */
-  UST_ERR_TRUNCATED = -9        /* ust_apply_state_delta_sparse: more changed outputs than the caller's arrays hold */
+  UST_ERR_TRUNCATED = -9,       /* ust_apply_state_delta_sparse: more changed outputs than the caller's arrays hold */
+  UST_ERR_VALIDATION = -10      /* UST_EVAL_VALIDATION: a validation start-time annotation does not parse
+                                   (validation_manager.go:155-160): per-node abort in pass 10   common_manager.go:587-590 */
 };
 
 typedef struct ust_counters {
@@ -539,9 +580,13 @@ int ust_fetch_build_state(ust_handle* h, int64_t n_pods, int32_t* ds_idx);
  * no device needed) so that it can be audited entry by entry:
  *   ust_table_entry: bits 0-15 actions, 16-23 next state, 24-31 actuator outcome (0xFF = none) for a
  *   node in state `state_code` whose predicate word is `w` (only the bits of the state's window matter);
- *   ust_table_window_shift: first bit of the window that state reads. */
+ *   ust_table_window_shift: first bit of the window that state reads (the layout without UST_EVAL_VALIDATION);
+ *   ust_table_window: the same for the table of `policy`, and its width in bits (`width` nullable). With
+ *   UST_EVAL_VALIDATION, validation-required reads bits 22..28: the node's pod-list summary byte (bits 1-7), which
+ *   carries Validate's outcome and the SAFE_LOAD / INITIAL_STATE_ANNO / REQUESTOR_MODE bits the pass reads. */
 uint32_t ust_table_entry(const ust_policy* policy, unsigned state_code, uint32_t w);
 int ust_table_window_shift(unsigned state_code);
+int ust_table_window(const ust_policy* policy, unsigned state_code, int* width);
 
 /* ---- multi-GPU (one process per GPU) ----------------------------------------------------------- */
 

@@ -326,6 +326,15 @@ static int pick_static_rounds(const ust_handle* h, int tiles, int grid) {
   return r < 0 ? 0 : r;
 }
 
+// UST_EVAL_VALIDATION answers Validate from the pod lists: it needs them, and the actuator evaluation it is part of
+static int check_eval_mode(ust_handle* h, const ust_policy* p, bool pods) {
+  if (!p || !(p->evaluate_actuators & UST_EVAL_VALIDATION)) return UST_OK;
+  if (!(p->evaluate_actuators & UST_EVAL_ACTUATORS))
+    return h->fail(UST_ERR_INVALID_ARGUMENT, "evaluate_actuators: UST_EVAL_VALIDATION requires UST_EVAL_ACTUATORS");
+  if (!pods) return h->fail(UST_ERR_INVALID_ARGUMENT, "evaluate_actuators: UST_EVAL_VALIDATION requires pod lists, which this call has not");
+  return UST_OK;
+}
+
 static int check_aligned(ust_handle* h, const void* p, const char* what) {
   if (((uintptr_t)p & 15u) != 0) return h->fail(UST_ERR_INVALID_ARGUMENT, "%s must be 16-byte aligned", what);
   return UST_OK;
@@ -476,7 +485,10 @@ static int apply_device(ust_handle* h, const ust_policy* policy, int64_t n, cons
     UST_CUDA(h, h->s_podsum.reserve((size_t)n + 16));
     P.podsum = h->s_podsum.p;
     P.evict_first_inputs = 1;  // the pod-list pass was not measured faster with evict-normal inputs
-    int e = ust_launch_pod_summary(n, P.active, P.hot, P.pod_off, P.pod_flags, n_pods, P.podlut, P.podsum, h->num_sms * 6, st);
+    // UST_EVAL_VALIDATION: the validation-required nodes get their byte too (ust_lut.h); an empty selector reads no pod
+    const int validation = !ust_validation_mode(policy) ? 0 : (policy->validation_enabled ? 2 : 1);
+    int e = ust_launch_pod_summary(n, P.active, P.hot, P.pod_off, P.pod_flags, n_pods, P.podlut, P.podsum, P.flags, validation,
+                                   &P.ws->errinv[P.parity], h->num_sms * 6, st);
     if (e) return h->fail(UST_ERR_CUDA, "pod-summary kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 1;
   }
@@ -928,6 +940,7 @@ int ust_apply_state_device(ust_handle* h, const ust_policy* policy, int64_t n_no
   cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
   if (pods && (!pods->pod_off || pods->n_pods < 0 || (pods->n_pods > 0 && !pods->pod_flags)))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad pod lists");
+  if (int rc = check_eval_mode(h, policy, pods != nullptr)) return rc;
   return apply_device(h, policy, n_nodes, state, flags, pod_rev, ds_idx, n_ds, ds_rev, pods ? pods->pod_off : nullptr,
                       pods ? pods->pod_flags : nullptr, pods ? pods->n_pods : 0, next_state, actions, actuator_outcome,
                       out_device, st);
@@ -945,6 +958,7 @@ int ust_apply_state(ust_handle* h, const ust_policy* policy, int64_t n, const ui
   if (n_ds < 0 || (n_ds > 0 && !ds_rev)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad DaemonSet table");
   if (pods && (!pods->pod_off || pods->n_pods < 0 || (pods->n_pods > 0 && !pods->pod_flags)))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad pod lists");
+  if (int rc = check_eval_mode(h, policy, pods != nullptr)) return rc;
   if (pods) {
     // a call that may leave the pod-list snapshot notes its list lengths for the checks of ust_apply_state_delta_pods
     int32_t* lens = nullptr;
@@ -1090,6 +1104,7 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
                         const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, bool sparse,
                         uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome, int64_t max_out, int64_t* out_idx,
                         int64_t* n_out, ust_counters* out) {
+  if (int rc = check_eval_mode(h, policy, pods)) return rc;
   const int64_t n_old = pods ? h->pods_n : h->resident_n;
   if (n_old < 0 && pods)
     return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident pod-list snapshot: call ust_apply_state with pod lists and actuator_outcome first");
@@ -1444,12 +1459,14 @@ int ust_apply_state_packed(ust_handle* h, const ust_policy* policy, int64_t n, c
   if (n < 0 || (n > 0 && (!state || !flags || !pod_rev16 || !ds_idx8 || !next_state || !actions)))
     return h->fail(UST_ERR_NIL_STATE, "currentState should not be empty");
   if (n_ds < 0 || n_ds > 127 || (n_ds > 0 && !ds_rev)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad DaemonSet table (the packed format holds at most 127 DaemonSets)");
+  if (int rc = check_eval_mode(h, policy, false)) return rc;
   return apply_host(h, policy, n, HostNodes{state, flags, nullptr, nullptr, pod_rev16, ds_idx8}, n_ds, ds_rev, nullptr,
                     next_state, actions, actuator_outcome, out);
 }
 
 static int simulate_common(ust_handle* h, const ust_policy* policy, const ust_sim_options* opt, int32_t steps, ust_counters* history,
                            uint8_t* final_state, uint32_t* final_flags, int32_t* final_pod_rev, int32_t* steps_done) {
+  if (int rc = check_eval_mode(h, policy, false)) return rc;
   const int64_t n = h->resident_n;
   if (n < 0) return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident snapshot: call ust_apply_state (without pod lists) first");
   if (steps < 0 || steps > (1 << 20)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad step count");
@@ -1732,6 +1749,12 @@ uint32_t ust_table_entry(const ust_policy* policy, unsigned state_code, uint32_t
   return ust_lut_lookup(lut.data(), state_code, w);
 }
 int ust_table_window_shift(unsigned state_code) { return ust_window_shift[state_code & 15u]; }
+int ust_table_window(const ust_policy* policy, unsigned state_code, int* width) {
+  const ust_policy key = table_key(policy);  // the policy the table is built for (an inactive one: the plain layout)
+  const ust_policy* p = policy_active(policy) ? &key : nullptr;
+  if (width) *width = ust_policy_bits_of(p, (int)(state_code & 15u));
+  return ust_policy_shift_of(p, (int)(state_code & 15u));
+}
 
 // audit: entries of the 2048-entry pod table (ust_build_pod_lut) that T[pf & 255] & gate(pf) disagrees with
 int ust_debug_podlut_mismatches(const ust_policy* p) {

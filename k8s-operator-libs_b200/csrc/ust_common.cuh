@@ -142,13 +142,16 @@ __device__ __forceinline__ void pack4(const uint32_t e[4], uint32_t& next4, uint
 
 // pod-list summary byte -> the w bits it stands for (ust_pod_summary_kernel): bit 0 = a wait-selector pod is
 // running, bits 1..3 = UST_W_PD_HAS / UST_W_PD_MISMATCH / UST_W_DRAIN_ERROR, bit 4 = the list overrides the
-// pre-evaluated UST_F_WAIT_PODS_RUNNING of the flags word
+// pre-evaluated UST_F_WAIT_PODS_RUNNING of the flags word. A validation-required node in validation mode uses bits 1-3
+// and 5-7 (ust_lut.h, UST_VALSUM_*): they land at w bits 22-24 and 26-28, state 9's window in that mode. Every other
+// node's bits 5-7 are clear, and no other state reads w bits 25-28.
 __device__ __forceinline__ uint32_t pods_apply(uint32_t fl, uint32_t ps) {
-  return (fl & ~((ps & 0x10u) << 12)) | ((ps & 1u) << 16) | ((ps & 0xEu) << 21);
+  return (fl & ~((ps & 0x10u) << 12)) | ((ps & 1u) << 16) | ((ps & 0xEEu) << 21);
 }
 static_assert(UST_F_WAIT_PODS_RUNNING == (1u << 16) && UST_W_PD_HAS == (UST_PODSUM_TO_DELETE << 21) &&
               UST_W_PD_MISMATCH == (UST_PODSUM_CANNOT_DELETE << 21) && UST_W_DRAIN_ERROR == (UST_PODSUM_DRAIN_ERROR << 21) &&
-              UST_PODSUM_WAIT_RUNNING == 1u, "pod summary byte layout");
+              UST_PODSUM_WAIT_RUNNING == 1u && UST_VAL_SHIFT == UST_VALSUM_OUTCOME_SHIFT + 21 && (UST_F_INPUT_MASK & 0x1FC00000u) == 0,
+              "pod summary byte layout");
 
 // ---- the decision between streaming and verification ------------------------------------------------------------
 struct DecideShared {
@@ -266,7 +269,9 @@ __device__ inline void write_counters(const UstParams& P, const long long* V, co
     pass = (long long)(s.abort_key >> 56);
     const long long idx1 = (long long)(s.abort_key & 0x00FFFFFFFFFFFFFFull);
     index = idx1 - 1;
-    code = idx1 ? UST_ERR_REVISION_HASH : (pass == 2 ? UST_ERR_MAX_UNAVAILABLE : UST_ERR_POD_DELETION_SPEC);
+    // node aborts: pass 10 (validation-required) can only be Validate's; the others are revision-hash lookups
+    code = idx1 ? (pass == 10 ? UST_ERR_VALIDATION : UST_ERR_REVISION_HASH)
+                : (pass == 2 ? UST_ERR_MAX_UNAVAILABLE : UST_ERR_POD_DELETION_SPEC);
   }
   const bool slots = P.active && !P.requestor && !(code && pass < 2) && code != UST_ERR_MAX_UNAVAILABLE;
   if (comm_failed) { code = UST_ERR_COMM; index = -1; pass = -1; }

@@ -158,8 +158,11 @@ int ust_launch_stream(const UstParams& p, int grid, void* stream, int pdl);   //
 int ust_launch_verify(const UstParams& p, int grid, void* stream, int pdl);   // ust_kernels.cu
 // also raises the dynamic shared-memory limit; `ctas_per_sm` = streaming CTAs an SM holds (occupancy API, fewest over the variants)
 int ust_stream_config(int device, int* num_sms, size_t* smem_bytes, int* ctas_per_sm);
+// `validation`: 0 = UST_EVAL_VALIDATION off; 1 = on, empty selector; 2 = on, walk the validation pods. An annotation that
+// does not parse publishes its abort key into `errinv` (the call's UstWorkspace::errinv slot)
 int ust_launch_pod_summary(long long n, int active, const uint8_t* hot, const int32_t* pod_off, const uint16_t* pod_flags,
-                           long long n_pods, const uint8_t* podlut, uint8_t* podsum, int grid, void* stream);
+                           long long n_pods, const uint8_t* podlut, uint8_t* podsum, const uint32_t* flags, int validation,
+                           unsigned long long* errinv, int grid, void* stream);
 int ust_launch_build_state(long long n, const uint8_t* hot, const int32_t* ds_idx, int n_ds, const int32_t* ds_desired,
                            unsigned long long* ds_count, UstWorkspace* ws, ust_counters* out, int grid, void* stream);
 // slot of a 128-bit UID in the DaemonSet hash table (before masking to the table size); host build and device lookup

@@ -78,13 +78,15 @@ __device__ __forceinline__ uint32_t noop_entry(uint32_t hb) { return ((hb & 15u)
 // abort semantics: nodes the sequential passes had not reached when the reference returned its error
 // stay untouched; the aborting node carries UST_A_ERROR; an abort inside ProcessPodRestartNodes also
 // drops the restarts collected so far, SchedulePodsRestart is only called after the loop
-// (common_manager.go:462-523).
+// (common_manager.go:462-523). A node that aborts in ProcessValidationRequiredNodes has already had its driver unblocked
+// (UnblockLoading runs before Validate, common_manager.go:580-590).
 __device__ __forceinline__ uint32_t apply_abort(const Shared& S, uint32_t ent, uint32_t hb, long long gidx) {
   const int pass = pass_of_state(hb & 15u);
   if (pass < 0) return ent;
   const unsigned long long key = UST_KEY(pass, (unsigned long long)gidx + 1ull);
   if (key >= S.abort_key) {
-    ent = noop_entry(hb);
+    const uint32_t kept = (key == S.abort_key && pass == 10) ? (ent & UST_A_UNBLOCK_SAFE_LOAD) : 0u;
+    ent = noop_entry(hb) | kept;
     if (key == S.abort_key) ent |= UST_A_ERROR;
   } else if (pass == 8 && (S.abort_key >> 56) == 8) {
     ent &= ~(uint32_t)UST_A_RESTART_DRIVER_POD;
@@ -169,7 +171,7 @@ __device__ void general_step(const UstParams& P, Shared& S, long long base, long
     if (P.podsum && k < nvalid) {  // pod-list summary of the node (ust_pod_summary_kernel), see pods_apply()
       const uint32_t ps = P.podsum[i0 + k];
       f &= ~((ps & 0x10u) << 12);
-      extra |= ((ps & 1u) << 16) | ((ps & 0xEu) << 21);
+      extra |= ((ps & 1u) << 16) | ((ps & 0xEEu) << 21);
     }
     e[k] = node_entry(P, S, ds_smem, hb[k], f, rev[k], di[k], extra);
     if (aborting) e[k] = apply_abort(S, e[k], hb[k], S.node_offset + i0 + k);
@@ -226,7 +228,7 @@ __device__ __forceinline__ void span_eval(const UstParams& P, Shared& S, const S
     for (int k = 0; k < 4; k++) {
       const uint32_t hb = (T.h[j] >> (8 * k)) & 0xFFu, p = (T.ps[j] >> (8 * k)) & 0xFFu;
       const uint32_t fk = fl[k] & ~((p & 0x10u) << 12);
-      e[k] = node_entry(P, S, ds_smem, hb, fk, (int)rv[k], dv[k], grant | ((p & 1u) << 16) | ((p & 0xEu) << 21));
+      e[k] = node_entry(P, S, ds_smem, hb, fk, (int)rv[k], dv[k], grant | ((p & 1u) << 16) | ((p & 0xEEu) << 21));
     }
     uint32_t next4, out4;
     uint2 act4;
@@ -452,11 +454,61 @@ __global__ void __maxnreg__(UST_VERIFY_MAXREG) ust_verify_kernel(const __grid_co
 // coalesced per block.
 constexpr int kPodBlock = 4096;            // nodes per block = 16 per thread
 constexpr int kPodChunks = 6;              // 16-byte loads in flight per thread and pass (48 pods: a typical list in one pass)
+// `validation` (UST_EVAL_VALIDATION): 0 = off, 1 = on with an empty selector (the byte carries the flag bits only),
+// kValWalk = on: the validation pods are walked as well
+constexpr int kValWalk = 2;
 
+// Validate (validation_manager.go:71-175) for one validation-required node: its pods with the validation-selector bit, in
+// list order, up to the first one that is not ready (the chunks of the list, kPodChunks loads in flight, until then).
+__device__ __forceinline__ uint32_t validation_summary(const uint16_t* __restrict__ pod_flags, const unsigned char* bytes,
+                                                       long long total_bytes, int p0, int p1, uint32_t fl, bool walk) {
+  bool not_ready = false, ready_before = false;
+  const int len = p1 - p0;
+  if (walk && len > 0) {
+    const long long c0 = (2LL * p0) & ~15LL;
+    const int nchunks = (int)((2LL * p1 - c0 + 15) >> 4);
+    if (c0 + 16LL * nchunks <= total_bytes) {
+      const uint4* src = reinterpret_cast<const uint4*>(bytes + c0);
+      int rel = (int)((c0 >> 1) - p0);
+      for (int cb = 0; cb < nchunks && !not_ready; cb += kPodChunks) {
+        uint4 x[kPodChunks];
+#pragma unroll
+        for (int u = 0; u < kPodChunks; u++) x[u] = cb + u < nchunks ? __ldcs(src + cb + u) : make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+        for (int u = 0; u < kPodChunks; u++) {
+          const uint32_t wv[4] = {x[u].x, x[u].y, x[u].z, x[u].w};
+#pragma unroll
+          for (int e = 0; e < 8; e++) {
+            const uint32_t f = (e & 1) ? wv[e >> 1] >> 16 : wv[e >> 1];
+            if (!not_ready && (f & UST_POD_MATCH_VALIDATION_SELECTOR) && (unsigned)(rel + e) < (unsigned)len) {
+              if (f & UST_POD_READY) ready_before = true;
+              else not_ready = true;
+            }
+          }
+          rel += 8;
+        }
+      }
+    } else {  // the list ends within the last 16 bytes of the whole array: plain 2-byte loads
+      for (int p = p0; p < p1 && !not_ready; p++) {
+        const uint32_t f = __ldg(pod_flags + p);
+        if (f & UST_POD_MATCH_VALIDATION_SELECTOR) {
+          if (f & UST_POD_READY) ready_before = true;
+          else not_ready = true;
+        }
+      }
+    }
+  }
+  return ust_validation_byte(not_ready, ready_before, walk, fl);
+}
+
+// VALIDATION: the call has UST_EVAL_VALIDATION (`validation` != 0); the other instantiation is the kernel without it
+template <bool VALIDATION>
 __global__ void __launch_bounds__(kThreads, 6) ust_pod_summary_kernel(long long n, int active, const uint8_t* __restrict__ hot,
                                                                       const int32_t* __restrict__ pod_off,
                                                                       const uint16_t* __restrict__ pod_flags, long long n_pods,
-                                                                      const uint8_t* __restrict__ podlut, uint8_t* __restrict__ podsum) {
+                                                                      const uint8_t* __restrict__ podlut, uint8_t* __restrict__ podsum,
+                                                                      const uint32_t* __restrict__ flags, int validation,
+                                                                      unsigned long long* __restrict__ errinv) {
   __shared__ __align__(16) uint8_t lut[256];   // what a pod raises, by its own eight bits (ust_lut.h: ust_build_pod_lut256)
   __shared__ __align__(16) uint8_t res[kPodBlock];   // summary byte per node of the block (bits 6-7: state - 3 while in work)
   __shared__ unsigned short list[kPodBlock];         // block-local indices of the nodes whose list is read
@@ -486,9 +538,10 @@ __global__ void __launch_bounds__(kThreads, 6) ust_pod_summary_kernel(long long 
 #pragma unroll
     for (int k = 0; k < 16; k++) {
       const unsigned s = (w[k >> 2] >> (8 * (k & 3))) & 15u;
-      const bool need = active && s >= UST_STATE_WAIT_FOR_JOBS_REQUIRED && s <= UST_STATE_DRAIN_REQUIRED;
+      const bool val = VALIDATION && s == UST_STATE_VALIDATION_REQUIRED;  // tag 3 (bits 6-7)
+      const bool need = active && ((s >= UST_STATE_WAIT_FOR_JOBS_REQUIRED && s <= UST_STATE_DRAIN_REQUIRED) || val);
       // wait-for-jobs: the list overrides the pre-evaluated bit (0x10) even when it is empty
-      const uint32_t b = need ? (((s - UST_STATE_WAIT_FOR_JOBS_REQUIRED) << 6) | (s == UST_STATE_WAIT_FOR_JOBS_REQUIRED ? 0x10u : 0u)) : 0u;
+      const uint32_t b = need ? (val ? 0xC0u : (((s - UST_STATE_WAIT_FOR_JOBS_REQUIRED) << 6) | (s == UST_STATE_WAIT_FOR_JOBS_REQUIRED ? 0x10u : 0u))) : 0u;
       if ((k & 3) == 0) init[k >> 2] = 0;
       init[k >> 2] |= b << (8 * (k & 3));
       needbits |= (need ? 1u : 0u) << k;
@@ -522,6 +575,13 @@ __global__ void __launch_bounds__(kThreads, 6) ust_pod_summary_kernel(long long 
       // the node's actuator only asks about pods that match ITS selector: wait-for-completion (bit 9), the deletion
       // filter (bit 8) or the drain selector (bit 10) - the others are not even looked up
       const unsigned tag = res[li];
+      if (VALIDATION && tag == 0xC0u) {  // validation-required (validation mode): the byte of ust_lut.h, and the abort Validate causes
+        const uint32_t v = validation_summary(pod_flags, bytes, total_bytes, p0, p1, __ldg(flags + i), validation == kValWalk);
+        // ~key of pass 10 at this node (shard-local index, like the streaming pass's revision-hash keys)
+        if (((v >> UST_VALSUM_OUTCOME_SHIFT) & 7u) == UST_VAL_ERROR) atomicMax(errinv, ~UST_KEY(10, (unsigned long long)i + 1ull));
+        res[li] = (uint8_t)v;
+        continue;
+      }
       const unsigned s = UST_STATE_WAIT_FOR_JOBS_REQUIRED + (tag >> 6);
       const uint32_t sel = s == UST_STATE_WAIT_FOR_JOBS_REQUIRED ? (uint32_t)UST_POD_MATCH_WAIT_SELECTOR
                          : (s == UST_STATE_POD_DELETION_REQUIRED ? (uint32_t)UST_POD_MATCH_DELETION_FILTER : (uint32_t)UST_POD_MATCH_DRAIN_SELECTOR);
@@ -1636,11 +1696,17 @@ int ust_launch_verify(const UstParams& p, int grid, void* stream, int pdl) {
   return (int)cudaLaunchKernelEx(&cfg, ust_verify_kernel, p);
 }
 int ust_launch_pod_summary(long long n, int active, const uint8_t* hot, const int32_t* pod_off, const uint16_t* pod_flags,
-                           long long n_pods, const uint8_t* podlut, uint8_t* podsum, int grid, void* stream) {
+                           long long n_pods, const uint8_t* podlut, uint8_t* podsum, const uint32_t* flags, int validation,
+                           unsigned long long* errinv, int grid, void* stream) {
   if (n <= 0) return 0;
   const long long blocks = (n + kPodBlock - 1) / kPodBlock;
   if (grid > blocks) grid = (int)blocks;
-  ust_pod_summary_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>(n, active, hot, pod_off, pod_flags, n_pods, podlut, podsum);
+  if (validation)
+    ust_pod_summary_kernel<true><<<grid, kThreads, 0, (cudaStream_t)stream>>>(n, active, hot, pod_off, pod_flags, n_pods, podlut,
+                                                                            podsum, flags, validation, errinv);
+  else
+    ust_pod_summary_kernel<false><<<grid, kThreads, 0, (cudaStream_t)stream>>>(n, active, hot, pod_off, pod_flags, n_pods, podlut,
+                                                                             podsum, flags, validation, errinv);
   return (int)cudaGetLastError();
 }
 int ust_launch_build_state(long long n, const uint8_t* hot, const int32_t* ds_idx, int n_ds, const int32_t* ds_desired,

@@ -83,6 +83,25 @@ UST_HD constexpr int ust_lut_used() {
 UST_HD constexpr uint32_t ust_meta_x(int s) { return (uint32_t)(ust_shift_of(s) - 2) | ((((1u << ust_bits_of(s)) - 1u) << 2) << 16); }
 UST_HD constexpr uint32_t ust_meta_y(int s) { return (uint32_t)ust_base_of(s) * 4u; }
 
+// Validation mode (UST_EVAL_ACTUATORS | UST_EVAL_VALIDATION): the pod-summary kernel answers Validate for a
+// validation-required node and writes everything that node's transition reads into its summary byte, bits 1-3 and 5-7
+// (UST_VALSUM_*), which pods_apply() puts at w bits 22-24 and 26-28. State 9 then reads the 7-bit window 22..28 of its
+// table slot instead of bits 6..13; no other state's window moves.
+#define UST_VAL_SHIFT 22
+#define UST_VAL_BITS 7
+static inline bool ust_validation_mode(const ust_policy* p) {
+  return p && (p->evaluate_actuators & (UST_EVAL_ACTUATORS | UST_EVAL_VALIDATION)) == (UST_EVAL_ACTUATORS | UST_EVAL_VALIDATION);
+}
+static inline int ust_policy_shift_of(const ust_policy* p, int s) {
+  return (s == UST_STATE_VALIDATION_REQUIRED && ust_validation_mode(p)) ? UST_VAL_SHIFT : ust_shift_of(s);
+}
+static inline int ust_policy_bits_of(const ust_policy* p, int s) {
+  return (s == UST_STATE_VALIDATION_REQUIRED && ust_validation_mode(p)) ? UST_VAL_BITS : ust_bits_of(s);
+}
+static inline uint32_t ust_policy_meta_x(const ust_policy* p, int s) {
+  return (uint32_t)(ust_policy_shift_of(p, s) - 2) | ((((1u << ust_policy_bits_of(p, s)) - 1u) << 2) << 16);
+}
+
 static constexpr int ust_window_shift[16] = {ust_shift_of(0), ust_shift_of(1), ust_shift_of(2), ust_shift_of(3), ust_shift_of(4), ust_shift_of(5),
                                              ust_shift_of(6), ust_shift_of(7), ust_shift_of(8), ust_shift_of(9), ust_shift_of(10), ust_shift_of(11),
                                              ust_shift_of(12), ust_shift_of(13), ust_shift_of(14), ust_shift_of(15)};
@@ -102,6 +121,55 @@ static inline void ust_uncordon_or_done(uint32_t w, unsigned* next, unsigned* ac
   *next = UST_STATE_UNCORDON_REQUIRED;
   if ((w & UST_F_INITIAL_STATE_ANNO) && !requestor) *next = UST_STATE_DONE;
   if (*next == UST_STATE_DONE || requestor) *actions |= UST_A_CLEAR_INITIAL_STATE_ANNO;
+}
+
+// Pod-list summary byte of a validation-required node in validation mode (ust_pod_summary_kernel): bits 1-3 the outcome
+// of Validate (validation_manager.go:71-175) for the node's validation pods in list order and its start-time annotation,
+// bits 5-7 the flag bits ProcessValidationRequiredNodes reads (common_manager.go:573-604). Bits 0 and 4 stay clear.
+#define UST_VALSUM_OUTCOME_SHIFT 1
+#define UST_VALSUM_SAFE_LOAD 0x20u
+#define UST_VALSUM_INITIAL_STATE_ANNO 0x40u
+#define UST_VALSUM_REQUESTOR_MODE 0x80u
+enum {
+  UST_VAL_WAIT = 0,         // not done, no annotation call: no matching pod, or the first one is not ready and the
+                            // annotation is present, valid and not timed out
+  UST_VAL_SET_START = 1,    // the first matching pod is not ready and there is no annotation: set it to now (:140-150)
+  UST_VAL_RESTART = 2,      // a ready pod before the first not-ready one: delete (:106-113), then set (:140-150)
+  UST_VAL_DONE = 3,         // every matching pod ready: done, annotation deleted
+  UST_VAL_TIMED_OUT = 4,    // now > start + 600: upgrade-failed, annotation deleted (:161-169)
+  UST_VAL_ERROR = 5         // the annotation does not parse: Validate returns an error (:155-160), ApplyState aborts
+};
+// the byte from the walk's findings and the node's flags word (device and host)
+UST_HD inline uint32_t ust_validation_byte(bool any_not_ready, bool ready_before, bool walked, uint32_t fl) {
+  unsigned o = UST_VAL_WAIT;
+  if (walked) {
+    if (!any_not_ready) o = ready_before ? UST_VAL_DONE : UST_VAL_WAIT;
+    else if (ready_before) o = UST_VAL_RESTART;
+    else if (!(fl & UST_F_VALIDATION_START_ANNO)) o = UST_VAL_SET_START;
+    else if (fl & UST_F_VALIDATION_START_INVALID) o = UST_VAL_ERROR;
+    else if (fl & UST_F_VALIDATION_TIMED_OUT) o = UST_VAL_TIMED_OUT;
+  }
+  return (o << UST_VALSUM_OUTCOME_SHIFT) | ((fl & UST_F_SAFE_LOAD) ? UST_VALSUM_SAFE_LOAD : 0u) |
+         ((fl & UST_F_INITIAL_STATE_ANNO) ? UST_VALSUM_INITIAL_STATE_ANNO : 0u) | ((fl & UST_F_REQUESTOR_MODE) ? UST_VALSUM_REQUESTOR_MODE : 0u);
+}
+
+// validation-required in validation mode: the summary byte sits at w bits 21.. (bits 0 and 4 of it are never set)
+static inline void ust_validation_transition(uint32_t w, const ust_policy* p, unsigned* next, unsigned* a) {
+  const uint32_t b = (w >> (UST_VAL_SHIFT - 1)) & 0xEEu;
+  if (b & UST_VALSUM_SAFE_LOAD) *a |= UST_A_UNBLOCK_SAFE_LOAD;  // UnblockLoading runs before Validate
+  const uint32_t wf = ((b & UST_VALSUM_INITIAL_STATE_ANNO) ? UST_F_INITIAL_STATE_ANNO : 0u) |
+                      ((b & UST_VALSUM_REQUESTOR_MODE) ? UST_F_REQUESTOR_MODE : 0u);
+  if (!p->validation_enabled) {  // empty podSelector: Validate is true without any list (validation_manager.go:72-74)
+    ust_uncordon_or_done(wf, next, a);
+    return;
+  }
+  switch ((b >> UST_VALSUM_OUTCOME_SHIFT) & 7u) {
+    case UST_VAL_SET_START: *a |= UST_A_SET_WAIT_START; break;
+    case UST_VAL_RESTART: *a |= UST_A_CLEAR_WAIT_START | UST_A_SET_WAIT_START; break;
+    case UST_VAL_DONE: *a |= UST_A_CLEAR_WAIT_START; ust_uncordon_or_done(wf, next, a); break;
+    case UST_VAL_TIMED_OUT: *a |= UST_A_CLEAR_WAIT_START; *next = UST_STATE_FAILED; break;
+    default: break;  // UST_VAL_WAIT; UST_VAL_ERROR: the abort (published by the pod-summary kernel) decides the node
+  }
 }
 
 // One node's transition as a function of its state code, predicate word and the policy.
@@ -200,6 +268,7 @@ static inline uint32_t ust_transition(unsigned s, uint32_t w, const ust_policy* 
       }
       break;
     case UST_STATE_VALIDATION_REQUIRED:  // common_manager.go:573-604
+      if (ust_validation_mode(p)) { ust_validation_transition(w, p, &next, &a); break; }
       if (w & UST_F_SAFE_LOAD) a |= UST_A_UNBLOCK_SAFE_LOAD;
       if (w & UST_F_VALIDATION_DONE) ust_uncordon_or_done(w, &next, &a);
       break;
@@ -217,12 +286,13 @@ static inline uint32_t ust_transition(unsigned s, uint32_t w, const ust_policy* 
 static inline void ust_build_lut(const ust_policy* p, uint32_t* lut) {
   for (unsigned i = 0; i < UST_LUT_WORDS; i++) lut[i] = 0;
   for (int s = 0; s < 16; s++) {
-    const int sh = ust_shift_of(s), base = ust_base_of(s);
-    for (uint32_t key = 0; key < (1u << ust_bits_of(s)); key++) {
+    // a policy's window fits its state's slot: validation mode gives state 9 7 of the 8 bits it has
+    const int sh = ust_policy_shift_of(p, s), base = ust_base_of(s);
+    for (uint32_t key = 0; key < (1u << ust_policy_bits_of(p, s)); key++) {
       const uint32_t w = (uint32_t)(((uint64_t)key << sh) & 0xFFFFFFFFull);
       lut[base + (int)key] = p ? ust_transition((unsigned)s, w, p) : ust_lut_pack((unsigned)s, (unsigned)s, 0, 0xFF);
     }
-    lut[UST_LUT_ENTRIES + 2 * s] = ust_meta_x(s);
+    lut[UST_LUT_ENTRIES + 2 * s] = ust_policy_meta_x(p, s);
     lut[UST_LUT_ENTRIES + 2 * s + 1] = ust_meta_y(s);
   }
 }

@@ -403,6 +403,16 @@ __global__ void __maxnreg__(UST_STREAM_MAXREG) ust_stream_kernel(const __grid_co
     }
     __syncthreads();
     mbar_wait(&S.lutbar, 0);
+    if (PODS && S.meta[UST_STATE_VALIDATION_REQUIRED].x != ust_meta_x(UST_STATE_VALIDATION_REQUIRED)) {
+      // validation mode moves state 9's window (ust_lut.h): then state 9's lookup pair is the table's, not the compile-time
+      // one of hot_entry. Consumer warps only (named barrier 1; the condition is the same for all of them), once per CTA.
+      if (ct < 8 * kHotRep) {
+        uint4& e = S.hotent[(UST_STATE_VALIDATION_REQUIRED + 16 * (ct / kHotRep)) * kHotRep + ct % kHotRep];
+        e.x = S.meta[UST_STATE_VALIDATION_REQUIRED].x;
+        e.y = S.meta[UST_STATE_VALIDATION_REQUIRED].y;
+      }
+      asm volatile("bar.sync 1, %0;" ::"n"(kThreads - 32) : "memory");
+    }
     consume<DS_SMEM, OUTCOME, PODS>(P, S, warp - 1);
   }
   // this CTA has run out of tiles: add its counts to the shard's (reductions, nobody waits for them) and leave.

@@ -113,11 +113,12 @@ class PodLists(C.Structure):
 
 def make_policy(auto_upgrade=True, max_parallel_upgrades=0, max_unavailable=None, pod_deletion_enabled=False,
                 validation_enabled=False, pod_deletion=None, drain=None, wait_for_completion=None,
-                use_maintenance_operator=False, evaluate_actuators=False):
+                use_maintenance_operator=False, evaluate_actuators=False, evaluate_validation=False):
     """Flatten a DriverUpgradePolicySpec-like description (api/upgrade/v1alpha1/upgrade_spec.go:27-110).
 
     max_unavailable: None | int | "NN%" | any other string (=> intstr parse error).
     pod_deletion / drain / wait_for_completion: None or dicts with the spec's json field names.
+    evaluate_validation: also answer Validate from the pod lists (UST_EVAL_VALIDATION; needs evaluate_actuators and pods).
     """
     p = Policy()
     p.auto_upgrade = int(bool(auto_upgrade))
@@ -148,5 +149,5 @@ def make_policy(auto_upgrade=True, max_parallel_upgrades=0, max_unavailable=None
         p.wait_selector_set = int(bool(wait_for_completion.get("podSelector", "")))
         p.wait_timeout_nonzero = int(wait_for_completion.get("timeoutSeconds", 0) != 0)
     p.use_maintenance_operator = int(bool(use_maintenance_operator))
-    p.evaluate_actuators = int(bool(evaluate_actuators))
+    p.evaluate_actuators = int(bool(evaluate_actuators)) | (K["UST_EVAL_VALIDATION"] if evaluate_validation else 0)
     return p

@@ -81,6 +81,7 @@ def load():
         lib.ust_table_entry.argtypes = [C.c_void_p, C.c_uint, C.c_uint32]
         lib.ust_table_entry.restype = C.c_uint32
         lib.ust_table_window_shift.argtypes = [C.c_uint]
+        lib.ust_table_window.argtypes = [C.c_void_p, C.c_uint, C.c_void_p]
         _lib = lib
     return _lib
 
@@ -88,7 +89,7 @@ def load():
 EXPORTS = ["ust_abi_version", "ust_create", "ust_destroy", "ust_last_error", "ust_create_error", "ust_launch_count",
            "ust_host_alloc", "ust_host_free", "ust_apply_state", "ust_apply_state_device", "ust_stream", "ust_apply_state_packed", "ust_apply_state_delta", "ust_apply_state_delta_sparse", "ust_apply_state_delta_splice", "ust_apply_state_delta_reorder", "ust_apply_state_delta_pods", "ust_apply_state_delta_pods_reorder", "ust_fetch_outputs", "ust_fetch_outputs_pods", "ust_simulate_rollout", "ust_simulate_rollout_timed", "ust_sync",
            "ust_build_state", "ust_build_state_uids", "ust_build_state_delta", "ust_fetch_build_state", "ust_get_unique_id", "ust_comm_init", "ust_comm_set_mode", "ust_table_entry",
-           "ust_table_window_shift"]
+           "ust_table_window_shift", "ust_table_window"]
 
 
 def _p(a):

@@ -136,6 +136,37 @@ def make_pods_blocked(n, seed, start=0, block=500_000):
     return {"pod_off": off.astype(np.int32), "pod_flags": np.concatenate(flags) if flags else np.zeros(0, np.uint16)}
 
 
+def make_validation_pods(soa, pods, seed, start=0, invalid_pct=0.0):
+    """Validation pods for the validation-required nodes of a snapshot (UST_EVAL_VALIDATION): each such node gets 0-3 pods
+    matching the validation selector ahead of its workload pods (only their order among themselves matters), each ready
+    with 80 % probability, and the validation start-time bits (annotation present 50 %, timed out 20 % of those,
+    unparsable `invalid_pct` % of those). Returns (flags, pods) for the same nodes; other nodes keep flags and lists."""
+    n = int(soa["state"].shape[0])
+    idx = np.arange(start, start + n, dtype=np.uint64)
+    f = _fields(seed ^ 0x7A11D, idx, 1)
+    val = (soa["state"] & np.uint8(15)) == abi.UST_STATE_VALIDATION_REQUIRED
+    anno = val & _bern(f[0], 50)
+    flags = soa["flags"] | np.where(anno, np.uint32(abi.UST_F_VALIDATION_START_ANNO), np.uint32(0))
+    flags |= np.where(anno & _bern(f[1], 20), np.uint32(abi.UST_F_VALIDATION_TIMED_OUT), np.uint32(0))
+    flags |= np.where(anno & _bern(f[2], invalid_pct), np.uint32(abi.UST_F_VALIDATION_START_INVALID), np.uint32(0))
+    k = np.where(val, (f[3] & np.uint32(3)).astype(np.int64), 0)
+    old_off = pods["pod_off"].astype(np.int64)
+    cnt = np.diff(old_off) + k
+    off = np.zeros(n + 1, dtype=np.int64)
+    np.cumsum(cnt, out=off[1:])
+    total = int(off[-1])
+    node_of = np.repeat(np.arange(n), cnt)
+    slot = np.arange(total, dtype=np.int64) - off[:-1][node_of]
+    is_val = slot < k[node_of]
+    pf = np.zeros(total, dtype=np.uint16)
+    pf[~is_val] = pods["pod_flags"][(old_off[:-1][node_of] + slot - k[node_of])[~is_val]]
+    # a validation pod is a pure function of (node index, slot), like make_pods' pods
+    g = _fields(seed ^ 0xA11D8, (idx[node_of] << np.uint64(2)) + slot.astype(np.uint64), 1)
+    vf = np.where(_bern(g[0], 80), abi.UST_PHASE_RUNNING | abi.UST_POD_READY, abi.UST_PHASE_PENDING).astype(np.uint16)
+    pf[is_val] = (vf | np.uint16(abi.UST_POD_MATCH_VALIDATION_SELECTOR))[is_val]
+    return flags.astype(np.uint32), {"pod_off": off.astype(np.int32), "pod_flags": pf}
+
+
 # BASELINE.json configs as concrete inputs (BASELINE.md §3)
 CONFIGS = {
     "C1": dict(n=100, seed=0x5EED0001, policy=dict(max_parallel_upgrades=1)),
