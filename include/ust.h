@@ -97,6 +97,8 @@ enum {
 #define UST_F_VALIDATION_START_ANNO (1u << 25)    /* annotation ...-driver-upgrade-validation-start-time PRESENT  validation_manager.go:142 */
 #define UST_F_VALIDATION_START_INVALID (1u << 26) /* ... and strconv.ParseInt(value, 10, 64) fails                validation_manager.go:155-160 */
 #define UST_F_VALIDATION_TIMED_OUT (1u << 27)     /* ... parses and now > start + 600, evaluated by the encoder   validation_manager.go:32, :161 */
+/* Bits 18 and 27 depend on the wall clock: the clocked pod-list calls (ust_apply_state_clocked) derive them on the device
+ * from per-node start times instead of taking them from the encoder. */
 
 /* ------------------------------------------------------------------------------------------------
  * pod_flags[p] (uint16): one entry per workload pod of a node (CSR by pod_off), used to evaluate
@@ -470,6 +472,62 @@ int ust_apply_state_delta_pods_reorder(ust_handle* h, const ust_policy* policy, 
                                        uint8_t* out_outcome, int64_t* n_out, ust_counters* out);
 /* The full outputs of the last call on the resident pod-list snapshot (n_nodes entries each). */
 int ust_fetch_outputs_pods(ust_handle* h, uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome);
+
+/* ---- Clocked pod-list calls: the two timeouts derived on the device ----------------------------------------------
+ * UST_F_WAIT_TIMED_OUT and UST_F_VALIDATION_TIMED_OUT depend on the wall clock as well as on an API object: when a node's
+ * deadline passes, no object changes, so a delta reconcile would send nothing for it and the stale bit would stay
+ * resident. The clocked calls keep one start time per node resident beside the pod-list snapshot; the caller passes
+ * `now` with each call and the device derives both bits afresh (in both directions: a clock that moves backwards
+ * clears them again). A reconcile in which only time passed sends no node and gets back exactly the nodes whose
+ * timeouts fired.
+ *
+ * start[i] (int64, what the encoder parsed; it no longer needs time.Now()):
+ *   wait-for-jobs-required  the wait-for-pod-completion start-time annotation    pod_manager.go:336, :348
+ *   validation-required     the validation start-time annotation                 validation_manager.go:142-160
+ * It is read only when that state's *_START_ANNO bit is set and its *_START_INVALID bit is clear, and ignored in every
+ * other case, whatever it holds. Derivation (Go int64 semantics: the sum wraps, so a start near INT64_MAX counts as
+ * timed out):
+ *   wait-for-jobs-required  UST_F_WAIT_TIMED_OUT       = now > start + wait_timeout_seconds    (pod_manager.go:354)
+ *                           UST_F_VALIDATION_TIMED_OUT = 0
+ *   validation-required     UST_F_VALIDATION_TIMED_OUT = now > start + UST_VALIDATION_TIMEOUT_SECONDS  (validation_manager.go:161)
+ *                           UST_F_WAIT_TIMED_OUT       = 0
+ * Input bits 18 and 27 are ignored by clocked calls (no other state reads them). */
+#define UST_VALIDATION_TIMEOUT_SECONDS 600 /* validation_manager.go:32 */
+typedef struct ust_clock {
+  int64_t now;                  /* time.Now().Unix() of this reconcile */
+  int64_t wait_timeout_seconds; /* WaitForCompletionSpec.TimeoutSecond (pod_manager.go:290-291); policy->wait_timeout_nonzero
+                                   must say whether it is non-zero */
+  const int64_t* start;         /* one per node the call carries: all n_nodes (full call) / aligned with idx (delta) */
+  const int64_t* insert_start;  /* one per inserted node of a reorder (aligned with reorder->state); NULL when n_insert == 0 */
+} ust_clock;
+
+/* ust_apply_state with pod lists (required) and actuator_outcome (required), with the two timeouts derived on the device
+ * from clock->now and clock->start. Returns exactly what ust_apply_state returns on the same arrays when bits 18 and 27
+ * have been set from the same `now` as above (outputs, actuator_outcome, counters, aborts). Leaves the resident pod-list
+ * snapshot as ust_apply_state with pods does, plus a resident start column: a clocked pod-list snapshot, which only
+ * ust_apply_state_delta_pods_clocked uses. UST_ERR_INVALID_ARGUMENT before any device work, with nothing resident changed,
+ * for everything ust_apply_state rejects, pods or actuator_outcome NULL, clock NULL, clock->start NULL with n_nodes > 0,
+ * and policy->wait_timeout_nonzero != (clock->wait_timeout_seconds != 0). */
+int ust_apply_state_clocked(ust_handle* h, const ust_policy* policy, const ust_clock* clock, int64_t n_nodes,
+                            const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx,
+                            int32_t n_ds, const int32_t* ds_rev, const ust_pods* pods, uint8_t* next_state,
+                            uint16_t* actions, uint8_t* actuator_outcome, ust_counters* out);
+/* ust_apply_state_delta_pods_reorder on a clocked pod-list snapshot (reorder == NULL: ust_apply_state_delta_pods), with the
+ * two timeouts derived on the device. A reorder moves each node's start with it, the n_changed nodes overwrite theirs
+ * from clock->start, inserted nodes bring theirs in clock->insert_start. Everything else - outputs, sparse outputs,
+ * counters, aborts, UST_ERR_TRUNCATED, ust_fetch_outputs_pods, residency - works as in the unclocked call. A time-only
+ * reconcile (n_changed == 0, no lists, no reorder) does no O(n) host work. Clocked and unclocked calls do not mix on one
+ * snapshot: this call on a snapshot an unclocked call left, or ust_apply_state_delta_pods / _pods_reorder on one a clocked
+ * call left, returns UST_ERR_INVALID_ARGUMENT. UST_ERR_INVALID_ARGUMENT before any device work, with the snapshot left as
+ * it was, for that, everything ust_apply_state_delta_pods_reorder rejects, clock NULL, clock->start NULL with
+ * n_changed > 0, clock->insert_start NULL with reorder->n_insert > 0, and policy->wait_timeout_nonzero !=
+ * (clock->wait_timeout_seconds != 0). */
+int ust_apply_state_delta_pods_clocked(ust_handle* h, const ust_policy* policy, const ust_clock* clock,
+                                       const ust_reorder* reorder /* nullable */, const ust_pod_lists* lists /* nullable */,
+                                       int64_t n_changed, const int64_t* idx, const uint8_t* state, const uint32_t* flags,
+                                       const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev,
+                                       int64_t max_out, int64_t* out_idx, uint8_t* out_next_state, uint16_t* out_actions,
+                                       uint8_t* out_outcome, int64_t* n_out, ust_counters* out);
 
 /* Rollout simulation (SURVEY 8f.3) on the resident snapshot (see ust_apply_state_delta): `steps` reconciles in a row,
  * entirely on the device. After each ApplyState the decisions are fed back into the snapshot under "ideal

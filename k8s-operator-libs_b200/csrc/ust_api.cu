@@ -160,6 +160,7 @@ struct ust_handle {
   // outputs in `outs` and s_outcome. Only the pod-list entry points see it.
   int64_t pods_n = -1;      // its nodes (-1 = none)
   int64_t pods_total = 0;   // its pods
+  bool pods_clocked = false;  // it was left by a clocked call: its start times are in s_start (ust_apply_state_clocked)
   DevBuf<ust_counters> sim_hist;  // rollout simulation: one ust_counters per simulated reconcile
   int segments = 6;      // upload / compute / download pipeline depth of the host path (UST_SEGMENTS, tuning)
   bool no_hint = false;  // UST_NO_HINT=1 (tuning): every call speculates from the policy default, never from the previous call
@@ -224,6 +225,9 @@ struct ust_handle {
   std::vector<int32_t> seg_pod;
   long long pod_pass_ns = 0;  // diagnostics: host time of the last pods_reorder_segments
   DevBuf<int32_t> sim_entered, sim_wait, sim_valid;  // timed rollout simulation: per-node clocks
+  // clocked pod-list calls: the start time of every node of the pod-list snapshot, the gather target of a reorder (swapped
+  // with it afterwards), the starts of the changed and of the inserted nodes as uploaded. Only clocked calls allocate them.
+  DevBuf<long long> s_start, s_start2, chg_start, ins_start;
   // the resident driver-pod list of ust_build_state_delta (bs_n pods, 0 until the first call; nothing else reads or drops
   // it): state bytes, owner UIDs and the owner indices of the last call in `bs`. `bs2` is the gather target of a reorder
   // (hot / uid allocated on the first reorder; swapped with `bs` afterwards); bs2.owner receives a call's owner indices
@@ -610,12 +614,15 @@ static void drop_resident(ust_handle* h) {
 // The snapshot in `staged` stays resident after a call that produced counters (a reference-level abort and
 // UST_ERR_TRUNCATED included), with the call's outputs unless `outputs` is false. A call that failed keeps nothing.
 // n_pods >= 0: the call evaluated pod lists of that many pods and their actuator outcomes; its snapshot is the pod-list
-// snapshot, which only ust_apply_state_delta_pods and ust_fetch_outputs_pods use.
-static int adopt_resident(ust_handle* h, int rc, int64_t n, int32_t n_ds, bool outputs = true, int64_t n_pods = -1) {
+// snapshot, which only ust_apply_state_delta_pods and ust_fetch_outputs_pods use (`clocked`: with its start times, which
+// only the clocked pod-list calls use).
+static int adopt_resident(ust_handle* h, int rc, int64_t n, int32_t n_ds, bool outputs = true, int64_t n_pods = -1,
+                          bool clocked = false) {
   if (rc != UST_ERR_CUDA && rc != UST_ERR_INVALID_ARGUMENT && rc != UST_ERR_COMM && rc != UST_ERR_NIL_STATE) {
     if (n_pods >= 0) {
       h->pods_n = n;
       h->pods_total = n_pods;
+      h->pods_clocked = clocked;
       return rc;
     }
     h->resident_n = n;
@@ -697,13 +704,33 @@ static int apply_pipelined(ust_handle* h, const ust_policy* policy, int64_t n, c
   return rc;
 }
 
-// ust_apply_state and ust_apply_state_packed after their argument checks: upload, evaluate, download. Snapshots of
-// 2^19 nodes or more take the pipelined path unless they come with pod lists. A call with pod lists and actuator_outcome
-// leaves the pod-list snapshot (its list lengths are in h->pod_len_next, filled by the offset check); one with pod lists
-// but no outcome leaves nothing resident.
+// Clocked pod-list calls: the clock must come with the start times of the nodes the call carries, and agree with the policy
+// about whether the wait has a timeout at all.
+static int check_clock(ust_handle* h, const ust_policy* policy, const ust_clock* clock, bool carried) {
+  if (!clock) return h->fail(UST_ERR_INVALID_ARGUMENT, "clock: required");
+  if (carried && !clock->start) return h->fail(UST_ERR_INVALID_ARGUMENT, "clock: start is NULL while the call carries nodes");
+  if (policy && (policy->wait_timeout_nonzero != 0) != (clock->wait_timeout_seconds != 0))
+    return h->fail(UST_ERR_INVALID_ARGUMENT, "policy.wait_timeout_nonzero must say whether clock.wait_timeout_seconds != 0");
+  return UST_OK;
+}
+
+// Clocked calls: bits 18 and 27 of the staged flags from the resident start column, just before the evaluation reads them
+static int launch_clock(ust_handle* h, const ust_clock* clock, int64_t n, cudaStream_t st) {
+  int e = ust_launch_clock((long long)n, h->staged.hot.p, h->staged.flags.p, h->s_start.p, (long long)clock->now,
+                           (long long)clock->wait_timeout_seconds, 8 * h->num_sms, st);
+  if (e) return h->fail(UST_ERR_CUDA, "clock kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+  h->launches += n > 0 ? 1 : 0;
+  return UST_OK;
+}
+
+// ust_apply_state, ust_apply_state_clocked and ust_apply_state_packed after their argument checks: upload, evaluate,
+// download. Snapshots of 2^19 nodes or more take the pipelined path unless they come with pod lists. A call with pod lists
+// and actuator_outcome leaves the pod-list snapshot (its list lengths are in h->pod_len_next, filled by the offset check);
+// one with pod lists but no outcome leaves nothing resident. `clock` (nullable; pod lists and outcome given): the start
+// times are uploaded beside the snapshot and the two timeouts derived from them.
 static int apply_host(ust_handle* h, const ust_policy* policy, int64_t n, const HostNodes& in, int32_t n_ds,
                       const int32_t* ds_rev, const ust_pods* pods, uint8_t* next_state, uint16_t* actions,
-                      uint8_t* outcome, ust_counters* out) {
+                      uint8_t* outcome, ust_counters* out, const ust_clock* clock = nullptr) {
   drop_resident(h);  // the staging arrays are overwritten from here on
   UST_CUDA(h, cudaSetDevice(h->device));
   StreamDrain drain(h);
@@ -734,6 +761,12 @@ static int apply_host(ust_handle* h, const ust_policy* policy, int64_t n, const 
     UST_CUDA(h, cudaMemcpyAsync(h->s_podoff.p, pods->pod_off, (N + 1) * 4, cudaMemcpyHostToDevice, st));
     if (pods->n_pods) UST_CUDA(h, cudaMemcpyAsync(h->s_podflags.p, pods->pod_flags, (size_t)pods->n_pods * 2, cudaMemcpyHostToDevice, st));
   }
+  if (clock) {
+    UST_CUDA(h, h->s_start.reserve(N + 1));
+    if (N) UST_CUDA(h, cudaMemcpyAsync(h->s_start.p, clock->start, N * 8, cudaMemcpyHostToDevice, st));
+    rc = launch_clock(h, clock, n, st);
+    if (rc) return rc;
+  }
   rc = apply_device(h, policy, n, h->staged.hot.p, h->staged.flags.p, h->staged.rev.p, h->staged.ds.p, n_ds, h->s_dsrev.p,
                     pods ? h->s_podoff.p : nullptr, pods ? h->s_podflags.p : nullptr, pods ? pods->n_pods : 0, h->outs.next.p,
                     h->outs.actions.p, outcome ? h->s_outcome.p : nullptr, nullptr, st);
@@ -747,7 +780,7 @@ static int apply_host(ust_handle* h, const ust_policy* policy, int64_t n, const 
   if (!pods) return adopt_resident(h, rc, n, n_ds);
   if (!outcome) return rc;
   std::swap(h->pod_len, h->pod_len_next);
-  return adopt_resident(h, rc, n, n_ds, true, pods->n_pods);
+  return adopt_resident(h, rc, n, n_ds, true, pods->n_pods, clock != nullptr);
 }
 
 // The launch of ust_build_state / _uids once their inputs are enqueued: `launch(grid)` starts the counting kernel and
@@ -946,12 +979,11 @@ int ust_apply_state_device(ust_handle* h, const ust_policy* policy, int64_t n_no
                       out_device, st);
 }
 
-int ust_apply_state(ust_handle* h, const ust_policy* policy, int64_t n, const uint8_t* state, const uint32_t* flags,
-                    const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev,
-                    const ust_pods* pods, uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome,
-                    ust_counters* out) {
-  if (!h) return UST_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> g(h->mu);
+// ust_apply_state and ust_apply_state_clocked (`clock` non-null: pod lists and actuator_outcome required)
+static int apply_state_common(ust_handle* h, const ust_policy* policy, const ust_clock* clock, int64_t n, const uint8_t* state,
+                              const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds,
+                              const int32_t* ds_rev, const ust_pods* pods, uint8_t* next_state, uint16_t* actions,
+                              uint8_t* actuator_outcome, ust_counters* out) {
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   if (n < 0 || (n > 0 && (!state || !flags || !pod_rev || !ds_idx || !next_state || !actions)))
     return h->fail(UST_ERR_NIL_STATE, "currentState should not be empty");
@@ -959,6 +991,11 @@ int ust_apply_state(ust_handle* h, const ust_policy* policy, int64_t n, const ui
   if (pods && (!pods->pod_off || pods->n_pods < 0 || (pods->n_pods > 0 && !pods->pod_flags)))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad pod lists");
   if (int rc = check_eval_mode(h, policy, pods != nullptr)) return rc;
+  if (clock) {  // (ust_apply_state_clocked has checked that it was given one)
+    if (!pods || !actuator_outcome)
+      return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_clocked: pod lists and actuator_outcome are required");
+    if (int rc = check_clock(h, policy, clock, n > 0)) return rc;
+  }
   if (pods) {
     // a call that may leave the pod-list snapshot notes its list lengths for the checks of ust_apply_state_delta_pods
     int32_t* lens = nullptr;
@@ -970,7 +1007,29 @@ int ust_apply_state(ust_handle* h, const ust_policy* policy, int64_t n, const ui
     if (prc) return prc;
   }
   return apply_host(h, policy, n, HostNodes{state, flags, pod_rev, ds_idx, nullptr, nullptr}, n_ds, ds_rev, pods, next_state,
-                    actions, actuator_outcome, out);
+                    actions, actuator_outcome, out, clock);
+}
+
+int ust_apply_state(ust_handle* h, const ust_policy* policy, int64_t n, const uint8_t* state, const uint32_t* flags,
+                    const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev,
+                    const ust_pods* pods, uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome,
+                    ust_counters* out) {
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  return apply_state_common(h, policy, nullptr, n, state, flags, pod_rev, ds_idx, n_ds, ds_rev, pods, next_state, actions,
+                            actuator_outcome, out);
+}
+
+int ust_apply_state_clocked(ust_handle* h, const ust_policy* policy, const ust_clock* clock, int64_t n, const uint8_t* state,
+                            const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds,
+                            const int32_t* ds_rev, const ust_pods* pods, uint8_t* next_state, uint16_t* actions,
+                            uint8_t* actuator_outcome, ust_counters* out) {
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  h->prev_n = -1;
+  if (!clock) return h->fail(UST_ERR_INVALID_ARGUMENT, "clock: required");
+  return apply_state_common(h, policy, clock, n, state, flags, pod_rev, ds_idx, n_ds, ds_rev, pods, next_state, actions,
+                            actuator_outcome, out);
 }
 
 // The runs of a reorder as the gather kernel reads them (ust_launch_reorder): h->run_off holds the exclusive prefix of
@@ -1099,16 +1158,26 @@ static int pods_reorder_segments(ust_handle* h, const ust_pod_lists* pl, int64_t
 // evaluate everything, return all outputs (dense) or the outputs that differ from the previous call's (sparse). `pods`:
 // the pod-list snapshot, whose lists `pl` (nullable) replaces first (after its reorder, `ro`, which moves the lists and
 // the previous outcome with the nodes); its sparse outputs include actuator_outcome (written to `actuator_outcome`).
+// `clock` (pod-list snapshot left by a clocked call only): the start times move with the nodes, the changed and inserted
+// nodes bring theirs, and the two timeouts are derived before the evaluation.
 static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splice* sp, const ust_reorder* ro, bool pods,
                         const ust_pod_lists* pl, int64_t n_changed, const int64_t* idx, const uint8_t* state, const uint32_t* flags,
                         const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, bool sparse,
                         uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome, int64_t max_out, int64_t* out_idx,
-                        int64_t* n_out, ust_counters* out) {
+                        int64_t* n_out, ust_counters* out, const ust_clock* clock = nullptr) {
   if (int rc = check_eval_mode(h, policy, pods)) return rc;
   const int64_t n_old = pods ? h->pods_n : h->resident_n;
   if (n_old < 0 && pods)
     return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident pod-list snapshot: call ust_apply_state with pod lists and actuator_outcome first");
   if (n_old < 0) return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident snapshot: call ust_apply_state (without pod lists) first");
+  if (pods && h->pods_clocked != (clock != nullptr))
+    return h->fail(UST_ERR_INVALID_ARGUMENT, clock ? "the resident pod-list snapshot has no start times: it was left by an unclocked call"
+                                                   : "the resident pod-list snapshot was left by a clocked call: use ust_apply_state_delta_pods_clocked");
+  if (clock) {
+    if (int rc = check_clock(h, policy, clock, n_changed > 0)) return rc;
+    if (ro && ro->n_insert > 0 && !clock->insert_start)
+      return h->fail(UST_ERR_INVALID_ARGUMENT, "clock: insert_start is NULL while the reorder inserts nodes");
+  }
   if (sparse && !pods && !h->outputs_resident)
     return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident outputs to compare with: the previous call must be an ApplyState on this snapshot");
   // the new node order, checked in full before anything is touched
@@ -1226,6 +1295,13 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
   }
   UST_CUDA(h, h->changed.idx.reserve(M + 1));
   UST_CUDA(h, h->changed.cols.reserve(M));
+  if (clock) {
+    UST_CUDA(h, h->chg_start.reserve(M + 1));
+    if (ro) {
+      UST_CUDA(h, h->s_start2.reserve(N + 1));
+      UST_CUDA(h, h->ins_start.reserve(I + 1));
+    }
+  }
   if (sparse) {  // the pair this call writes holds the new size as well
     UST_CUDA(h, h->outs_prev.reserve(N));
     UST_CUDA(h, h->sp_blocks.reserve((size_t)ust_diff_blocks(n) + 1));
@@ -1276,11 +1352,14 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
       long long* src = h->runs.p + NR + 1;
       UST_CUDA(h, cudaMemcpyAsync(off, h->run_off.data(), (NR + 1) * 8, cudaMemcpyHostToDevice, st));
       if (NR) UST_CUDA(h, cudaMemcpyAsync(src, h->run_src.data(), NR * 8, cudaMemcpyHostToDevice, st));
+      if (clock && I) UST_CUDA(h, cudaMemcpyAsync(h->ins_start.p, clock->insert_start, I * 8, cudaMemcpyHostToDevice, st));
       e = ust_launch_reorder((long long)n, (long long)NR, off, src, in.hot.p, in.flags.p, in.rev.p, in.ds.p, s.hot.p, s.flags.p, s.rev.p,
                              s.ds.p, h->outs.next.p, h->outs.actions.p, pods ? h->s_outcome.p : nullptr, x.hot.p, x.flags.p, x.rev.p,
-                             x.ds.p, h->splice_outs.next.p, h->splice_outs.actions.p, pods ? h->splice_outcome.p : nullptr, st);
+                             x.ds.p, h->splice_outs.next.p, h->splice_outs.actions.p, pods ? h->splice_outcome.p : nullptr, st,
+                             clock ? h->ins_start.p : nullptr, clock ? h->s_start.p : nullptr, clock ? h->s_start2.p : nullptr);
       if (e) return h->fail(UST_ERR_CUDA, "reorder kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
       if (pods) std::swap(h->s_outcome, h->splice_outcome);  // the previous outcome in the new order
+      if (clock) std::swap(h->s_start, h->s_start2);          // the start times in the new order
     } else {
       // a splice keeps its own kernel: the gather kernel measured slower on splices (DESIGN.md §3.4)
       if (R) UST_CUDA(h, cudaMemcpyAsync(h->removed.p, sp->remove_idx, R * 8, cudaMemcpyHostToDevice, st));
@@ -1299,11 +1378,16 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
     static_assert(sizeof(long long) == sizeof(int64_t), "index width");
     UST_CUDA(h, cudaMemcpyAsync(h->changed.idx.p, idx, M * 8, cudaMemcpyHostToDevice, st));
     UST_CUDA(h, h->changed.cols.upload(state, flags, pod_rev, ds_idx, 0, M, st));
+    if (clock) UST_CUDA(h, cudaMemcpyAsync(h->chg_start.p, clock->start, M * 8, cudaMemcpyHostToDevice, st));
     const Columns &d = h->changed.cols, &s = h->staged;
     int e = ust_launch_patch((long long)n_changed, h->changed.idx.p, d.hot.p, d.flags.p, d.rev.p, d.ds.p, s.hot.p, s.flags.p,
-                             s.rev.p, s.ds.p, st);
+                             s.rev.p, s.ds.p, st, clock ? h->chg_start.p : nullptr, clock ? h->s_start.p : nullptr);
     if (e) return h->fail(UST_ERR_CUDA, "patch kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 1;
+  }
+  if (clock) {
+    int rc = launch_clock(h, clock, n, st);
+    if (rc) return rc;
   }
   if (sparse) std::swap(h->outs, h->outs_prev);  // the previous call's outputs step aside; this call writes the other pair
   if (sparse && pods) std::swap(h->s_outcome, h->s_outcome_prev);
@@ -1335,7 +1419,7 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
       if (pods) UST_CUDA(h, cudaMemcpyAsync(actuator_outcome, h->sp_outcome.p, (size_t)cnt, cudaMemcpyDeviceToHost, st));
     }
   }
-  rc = adopt_resident(h, finish_with_counters(h, st, out), n, n_ds, true, pods ? new_total : -1);
+  rc = adopt_resident(h, finish_with_counters(h, st, out), n, n_ds, true, pods ? new_total : -1, clock != nullptr);
   if (sparse && (rc == UST_OK) && *n_out > max_out)
     return h->fail(UST_ERR_TRUNCATED, "%lld outputs changed, the caller's arrays hold %lld: fetch them with %s", (long long)*n_out,
                    (long long)max_out, pods ? "ust_fetch_outputs_pods" : "ust_fetch_outputs");
@@ -1415,6 +1499,20 @@ int ust_apply_state_delta_pods_reorder(ust_handle* h, const ust_policy* policy, 
   if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_pods_reorder runs on one GPU");
   return delta_common(h, policy, nullptr, reorder, true, lists, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true,
                       out_next_state, out_actions, out_outcome, max_out, out_idx, n_out, out);
+}
+
+int ust_apply_state_delta_pods_clocked(ust_handle* h, const ust_policy* policy, const ust_clock* clock, const ust_reorder* reorder,
+                                       const ust_pod_lists* lists, int64_t n_changed, const int64_t* idx, const uint8_t* state,
+                                       const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds,
+                                       const int32_t* ds_rev, int64_t max_out, int64_t* out_idx, uint8_t* out_next_state,
+                                       uint16_t* out_actions, uint8_t* out_outcome, int64_t* n_out, ust_counters* out) {
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
+  if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_pods_clocked runs on one GPU");
+  if (!clock) return h->fail(UST_ERR_INVALID_ARGUMENT, "clock: required");
+  return delta_common(h, policy, nullptr, reorder, true, lists, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true,
+                      out_next_state, out_actions, out_outcome, max_out, out_idx, n_out, out, clock);
 }
 
 int ust_fetch_outputs_pods(ust_handle* h, uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome) {

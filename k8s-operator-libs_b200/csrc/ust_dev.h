@@ -192,8 +192,14 @@ int ust_launch_build_state_reorder(long long n, long long n_runs, const long lon
                                    const int32_t* prev, uint8_t* o_hot, void* o_uid, int32_t* o_prev, void* stream);
 int ust_launch_build_state_patch(long long m, const long long* idx, const uint8_t* state, const void* uid, uint8_t* hot_out,
                                  void* uid_out, void* stream);
+// with start_out non-null (clocked pod-list deltas) the changed nodes' start times are scattered as well
 int ust_launch_patch(long long m, const long long* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
-                     const int32_t* ds_idx, uint8_t* hot_out, uint32_t* flags_out, int32_t* rev_out, int32_t* ds_out, void* stream);
+                     const int32_t* ds_idx, uint8_t* hot_out, uint32_t* flags_out, int32_t* rev_out, int32_t* ds_out, void* stream,
+                     const long long* start = nullptr, long long* start_out = nullptr);
+// clocked pod-list calls: bits 18 and 27 of the wait-for-jobs-required and validation-required nodes' flags, derived in place
+// from their start times (include/ust.h, ust_clock); hot carries 16 bytes of padding
+int ust_launch_clock(long long n, const uint8_t* hot, uint32_t* flags, const long long* start, long long now, long long wait_timeout,
+                     int grid, void* stream);
 // membership splice (ust_apply_state_delta_splice): the resident columns and the previous outputs, rewritten in the new node
 // order into the o_* arrays (n - n_rm + n_ins entries); rm / ib sorted and checked by the caller
 int ust_launch_splice(long long n, long long n_rm, const long long* rm, long long n_ins, const long long* ib, const uint8_t* ins_hot,
@@ -203,11 +209,13 @@ int ust_launch_splice(long long n, long long n_rm, const long long* rm, long lon
 // new node order of the resident snapshot (ust_apply_state_delta_reorder): the resident columns and the previous
 // outputs, gathered into the o_* arrays (n entries). Run r covers new positions [run_off[r], run_off[r + 1]) and reads old
 // nodes from run_src[r] on, or inserted nodes from -1 - run_src[r] on (run_src[r] < 0); checked by the caller. With `oc`
-// non-null (ust_apply_state_delta_pods_reorder) the previous actuator_outcome is gathered into o_oc as well
+// non-null (ust_apply_state_delta_pods_reorder) the previous actuator_outcome is gathered into o_oc as well, and with o_start
+// non-null as well (clocked) the start times into o_start (inserted nodes from ins_start)
 int ust_launch_reorder(long long n, long long n_runs, const long long* run_off, const long long* run_src, const uint8_t* ins_hot,
                        const uint32_t* ins_flags, const int32_t* ins_rev, const int32_t* ins_ds, const uint8_t* hot, const uint32_t* flags,
                        const int32_t* rev, const int32_t* ds, const uint8_t* next, const uint16_t* act, const uint8_t* oc, uint8_t* o_hot,
-                       uint32_t* o_flags, int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, uint8_t* o_oc, void* stream);
+                       uint32_t* o_flags, int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, uint8_t* o_oc, void* stream,
+                       const long long* ins_start = nullptr, const long long* start = nullptr, long long* o_start = nullptr);
 // rollout simulation: the clock of the feedback between two reconciles (include/ust.h, ust_sim_options)
 struct UstSimParams {
   int timed;            // 0: whatever a node waits for has happened by the next reconcile

@@ -991,11 +991,14 @@ __global__ void __launch_bounds__(kThreads) ust_build_state_patch_kernel(long lo
   }
 }
 
-// Delta update of the resident snapshot (SURVEY 8f.2): scatter the re-encoded nodes into the SoA arrays.
+// Delta update of the resident snapshot (SURVEY 8f.2): scatter the re-encoded nodes into the SoA arrays. CLOCK (clocked
+// pod-list deltas): their start times too.
+template <bool CLOCK>
 __global__ void __launch_bounds__(kThreads) ust_patch_kernel(long long m, const long long* __restrict__ idx,
                                                              const uint8_t* __restrict__ state, const uint32_t* __restrict__ flags,
                                                              const int32_t* __restrict__ pod_rev, const int32_t* __restrict__ ds_idx,
-                                                             uint8_t* hot_out, uint32_t* flags_out, int32_t* rev_out, int32_t* ds_out) {
+                                                             uint8_t* hot_out, uint32_t* flags_out, int32_t* rev_out, int32_t* ds_out,
+                                                             const long long* __restrict__ start, long long* start_out) {
   const long long stride = (long long)gridDim.x * kThreads;
   for (long long k = (long long)blockIdx.x * kThreads + threadIdx.x; k < m; k += stride) {
     const long long i = __ldg(idx + k);
@@ -1003,6 +1006,7 @@ __global__ void __launch_bounds__(kThreads) ust_patch_kernel(long long m, const 
     flags_out[i] = __ldg(flags + k);
     rev_out[i] = __ldg(pod_rev + k);
     ds_out[i] = __ldg(ds_idx + k);
+    if (CLOCK) start_out[i] = __ldg(start + k);
   }
 }
 
@@ -1144,7 +1148,8 @@ __global__ void __launch_bounds__(kThreads) ust_splice_kernel(long long n, long 
 // (every run is at least one position long, so at most kGatherTile of them meet a tile). Each thread then finds its
 // positions' runs in that range, walking forward from the run of its previous position.
 // 16 B read + 16 B written per node, 16 B per run; a run is read contiguously. OUTCOME (ust_apply_state_delta_pods_reorder):
-// the previous actuator_outcome travels too (1 B more each way; 0xFF for inserted nodes).
+// the previous actuator_outcome travels too (1 B more each way; 0xFF for inserted nodes). CLOCK
+// (ust_apply_state_delta_pods_clocked): the start time too (8 B more each way; inserted nodes bring theirs).
 constexpr int kGatherTile = 2048;
 
 // The run lookup of the gather kernels (ust_reorder_kernel, ust_build_state_reorder_kernel): copy(p, src, k) for every new
@@ -1176,7 +1181,7 @@ __device__ __forceinline__ void gather_runs(long long n, long long n_runs, const
   }
 }
 
-template <bool OUTCOME>
+template <bool OUTCOME, bool CLOCK>
 __global__ void __launch_bounds__(kThreads) ust_reorder_kernel(long long n, long long n_runs, const long long* __restrict__ run_off,
                                                                const long long* __restrict__ run_src,
                                                                const uint8_t* __restrict__ ins_hot, const uint32_t* __restrict__ ins_flags,
@@ -1188,20 +1193,54 @@ __global__ void __launch_bounds__(kThreads) ust_reorder_kernel(long long n, long
                                                                uint8_t* __restrict__ o_hot, uint32_t* __restrict__ o_flags,
                                                                int32_t* __restrict__ o_rev, int32_t* __restrict__ o_ds,
                                                                uint8_t* __restrict__ o_next, uint16_t* __restrict__ o_act,
-                                                               uint8_t* __restrict__ o_oc) {
+                                                               uint8_t* __restrict__ o_oc, const long long* __restrict__ ins_start,
+                                                               const long long* __restrict__ start, long long* __restrict__ o_start) {
   gather_runs(n, n_runs, run_off, run_src, [=](long long p, long long src, long long k) {
     if (src >= 0) {
       const long long i = src + k;
       o_hot[p] = __ldcs(hot + i); o_flags[p] = __ldcs(flags + i); o_rev[p] = __ldcs(rev + i); o_ds[p] = __ldcs(ds + i);
       o_next[p] = __ldcs(next + i); o_act[p] = __ldcs(act + i);
       if (OUTCOME) o_oc[p] = __ldcs(oc + i);
+      if (CLOCK) o_start[p] = __ldcs(start + i);
     } else {
       const long long i = -1 - src + k;
       o_hot[p] = __ldg(ins_hot + i); o_flags[p] = __ldg(ins_flags + i); o_rev[p] = __ldg(ins_rev + i); o_ds[p] = __ldg(ins_ds + i);
       o_next[p] = 0xFF; o_act[p] = 0;
       if (OUTCOME) o_oc[p] = 0xFF;
+      if (CLOCK) o_start[p] = __ldg(ins_start + i);
     }
   });
+}
+
+// Clocked pod-list calls (ust_apply_state_clocked, ust_apply_state_delta_pods_clocked): bits 18 and 27 of the resident flags,
+// derived from the resident start column and the call's clock just before the evaluation reads them (include/ust.h,
+// ust_clock). A thread reads 16 hot bytes in one load; only wait-for-jobs-required and validation-required nodes read their
+// flags word - and, with a valid start annotation, their start - and write the word back when it changes. 1 B per node,
+// plus up to 12 B read and 4 B written per such node. (A variant that issued the flags loads of all 16 nodes first, then
+// their start loads, measured slower at C4: 67 against 53 us, DESIGN.md.)
+__global__ void __launch_bounds__(kThreads) ust_clock_kernel(long long n, const uint8_t* __restrict__ hot, uint32_t* __restrict__ flags,
+                                                             const long long* __restrict__ start, long long now, long long wait_timeout) {
+  const long long chunks = (n + 15) / 16;  // the hot column carries 16 bytes of padding
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long c = (long long)blockIdx.x * kThreads + threadIdx.x; c < chunks; c += stride) {
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(hot) + c);
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int j = 0; j < 16; j++) {
+      const unsigned s = (w[j >> 2] >> (8 * (j & 3))) & UST_HOT_STATE_MASK;
+      const long long i = c * 16 + j;
+      if ((s != UST_STATE_WAIT_FOR_JOBS_REQUIRED && s != UST_STATE_VALIDATION_REQUIRED) || i >= n) continue;
+      const bool wait = s == UST_STATE_WAIT_FOR_JOBS_REQUIRED;
+      const uint32_t anno = wait ? UST_F_WAIT_START_ANNO : UST_F_VALIDATION_START_ANNO;
+      const uint32_t invalid = wait ? UST_F_WAIT_START_INVALID : UST_F_VALIDATION_START_INVALID;
+      const uint32_t f = flags[i];
+      const bool timed_out = (f & (anno | invalid)) == anno &&
+                             ust_timed_out(now, __ldg(start + i), wait ? wait_timeout : (long long)UST_VALIDATION_TIMEOUT_SECONDS);
+      const uint32_t g = (f & ~(UST_F_WAIT_TIMED_OUT | UST_F_VALIDATION_TIMED_OUT)) |
+                         (timed_out ? (wait ? UST_F_WAIT_TIMED_OUT : UST_F_VALIDATION_TIMED_OUT) : 0u);
+      if (g != f) flags[i] = g;
+    }
+  }
 }
 
 // The resident driver-pod list of ust_build_state_delta in a new order: state byte, owner UID and previous owner index of
@@ -1520,7 +1559,7 @@ __global__ void __launch_bounds__(kThreads) ust_feedback_kernel(long long n, uin
       // Validate() of a node whose validation pod is not ready runs handleTimeout (validation_manager.go:139-175)
       if (s == UST_STATE_VALIDATION_REQUIRED && ns == UST_STATE_VALIDATION_REQUIRED && !(f & UST_F_VALIDATION_DONE)) {
         if (vs == kSimNone) vs = (int)now;
-        else if (now > (long long)vs + sp.validation_timeout) { ns = UST_STATE_FAILED; vs = kSimNone; }
+        else if (ust_timed_out(now, vs, sp.validation_timeout)) { ns = UST_STATE_FAILED; vs = kSimNone; }
       }
       if (ns != UST_STATE_VALIDATION_REQUIRED) vs = kSimNone;      // the annotation is removed once the pod is ready (:104-110)
       if (ns != s) ent = (int)now;
@@ -1530,7 +1569,7 @@ __global__ void __launch_bounds__(kThreads) ust_feedback_kernel(long long n, uin
       else {
         if (ns != s) f = sp.job_seconds > 0 ? (f | UST_F_WAIT_PODS_RUNNING) : (f & ~UST_F_WAIT_PODS_RUNNING);
         if (now_next >= (long long)ent + sp.job_seconds) f &= ~UST_F_WAIT_PODS_RUNNING;
-        const bool timed_out = ws != kSimNone && now_next > (long long)ws + sp.wait_timeout;
+        const bool timed_out = ws != kSimNone && ust_timed_out(now_next, ws, sp.wait_timeout);
         f = timed_out ? (f | UST_F_WAIT_TIMED_OUT) : (f & ~UST_F_WAIT_TIMED_OUT);
       }
     }
@@ -1724,11 +1763,24 @@ int ust_launch_widen(long long n, const uint16_t* rev16, const int8_t* ds8, int3
   return (int)cudaGetLastError();
 }
 int ust_launch_patch(long long m, const long long* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
-                     const int32_t* ds_idx, uint8_t* hot_out, uint32_t* flags_out, int32_t* rev_out, int32_t* ds_out, void* stream) {
+                     const int32_t* ds_idx, uint8_t* hot_out, uint32_t* flags_out, int32_t* rev_out, int32_t* ds_out, void* stream,
+                     const long long* start, long long* start_out) {
   if (m <= 0) return 0;
   const long long grid = (m + kThreads - 1) / kThreads;
-  ust_patch_kernel<<<(unsigned)(grid > 65535 * 16 ? 65535 * 16 : grid), kThreads, 0, (cudaStream_t)stream>>>(
-      m, idx, state, flags, pod_rev, ds_idx, hot_out, flags_out, rev_out, ds_out);
+  const unsigned g = (unsigned)(grid > 65535 * 16 ? 65535 * 16 : grid);
+  if (start_out)
+    ust_patch_kernel<true><<<g, kThreads, 0, (cudaStream_t)stream>>>(m, idx, state, flags, pod_rev, ds_idx, hot_out, flags_out, rev_out,
+                                                                    ds_out, start, start_out);
+  else
+    ust_patch_kernel<false><<<g, kThreads, 0, (cudaStream_t)stream>>>(m, idx, state, flags, pod_rev, ds_idx, hot_out, flags_out, rev_out,
+                                                                     ds_out, nullptr, nullptr);
+  return (int)cudaGetLastError();
+}
+int ust_launch_clock(long long n, const uint8_t* hot, uint32_t* flags, const long long* start, long long now, long long wait_timeout,
+                     int grid, void* stream) {
+  if (n <= 0) return 0;
+  const long long want = ((n + 15) / 16 + kThreads - 1) / kThreads;
+  ust_clock_kernel<<<(unsigned)(want < grid ? want : grid), kThreads, 0, (cudaStream_t)stream>>>(n, hot, flags, start, now, wait_timeout);
   return (int)cudaGetLastError();
 }
 int ust_launch_splice(long long n, long long n_rm, const long long* rm, long long n_ins, const long long* ib, const uint8_t* ins_hot,
@@ -1743,16 +1795,22 @@ int ust_launch_splice(long long n, long long n_rm, const long long* rm, long lon
 int ust_launch_reorder(long long n, long long n_runs, const long long* run_off, const long long* run_src, const uint8_t* ins_hot,
                        const uint32_t* ins_flags, const int32_t* ins_rev, const int32_t* ins_ds, const uint8_t* hot, const uint32_t* flags,
                        const int32_t* rev, const int32_t* ds, const uint8_t* next, const uint16_t* act, const uint8_t* oc, uint8_t* o_hot,
-                       uint32_t* o_flags, int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, uint8_t* o_oc, void* stream) {
+                       uint32_t* o_flags, int32_t* o_rev, int32_t* o_ds, uint8_t* o_next, uint16_t* o_act, uint8_t* o_oc, void* stream,
+                       const long long* ins_start, const long long* start, long long* o_start) {
   const long long grid = n > 0 ? (n + kGatherTile - 1) / kGatherTile : 1;  // one launch also for the empty snapshot
-  if (oc)
-    ust_reorder_kernel<true><<<(unsigned)grid, kThreads, 0, (cudaStream_t)stream>>>(n, n_runs, run_off, run_src, ins_hot, ins_flags, ins_rev,
+  if (oc && o_start)
+    ust_reorder_kernel<true, true><<<(unsigned)grid, kThreads, 0, (cudaStream_t)stream>>>(
+        n, n_runs, run_off, run_src, ins_hot, ins_flags, ins_rev, ins_ds, hot, flags, rev, ds, next, act, oc, o_hot, o_flags, o_rev, o_ds,
+        o_next, o_act, o_oc, ins_start, start, o_start);
+  else if (oc)
+    ust_reorder_kernel<true, false><<<(unsigned)grid, kThreads, 0, (cudaStream_t)stream>>>(n, n_runs, run_off, run_src, ins_hot, ins_flags, ins_rev,
                                                                                   ins_ds, hot, flags, rev, ds, next, act, oc, o_hot, o_flags,
-                                                                                  o_rev, o_ds, o_next, o_act, o_oc);
+                                                                                  o_rev, o_ds, o_next, o_act, o_oc, nullptr, nullptr, nullptr);
   else
-    ust_reorder_kernel<false><<<(unsigned)grid, kThreads, 0, (cudaStream_t)stream>>>(n, n_runs, run_off, run_src, ins_hot, ins_flags, ins_rev,
+    ust_reorder_kernel<false, false><<<(unsigned)grid, kThreads, 0, (cudaStream_t)stream>>>(n, n_runs, run_off, run_src, ins_hot, ins_flags, ins_rev,
                                                                                    ins_ds, hot, flags, rev, ds, next, act, nullptr, o_hot,
-                                                                                   o_flags, o_rev, o_ds, o_next, o_act, nullptr);
+                                                                                   o_flags, o_rev, o_ds, o_next, o_act, nullptr, nullptr, nullptr,
+                                                                                   nullptr);
   return (int)cudaGetLastError();
 }
 int ust_launch_pods_scatter(long long n_lists, const long long* node_idx, const int32_t* new_off, const uint16_t* new_flags,

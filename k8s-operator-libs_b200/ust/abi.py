@@ -111,6 +111,11 @@ class PodLists(C.Structure):
                 ("n_pods", C.c_int64)]
 
 
+class Clock(C.Structure):
+    """ust_clock: the time of a clocked pod-list call and the start times of the nodes it carries (raw host addresses)."""
+    _fields_ = [("now", C.c_int64), ("wait_timeout_seconds", C.c_int64), ("start", C.c_void_p), ("insert_start", C.c_void_p)]
+
+
 def make_policy(auto_upgrade=True, max_parallel_upgrades=0, max_unavailable=None, pod_deletion_enabled=False,
                 validation_enabled=False, pod_deletion=None, drain=None, wait_for_completion=None,
                 use_maintenance_operator=False, evaluate_actuators=False, evaluate_validation=False):

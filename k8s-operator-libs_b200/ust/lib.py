@@ -64,6 +64,11 @@ def load():
                                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                                            C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                            C.c_void_p]
+        lib.ust_apply_state_clocked.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p] + apply_args[2:]
+        lib.ust_apply_state_delta_pods_clocked.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                           C.c_void_p, C.c_void_p]
         lib.ust_fetch_outputs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         lib.ust_fetch_outputs_pods.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.ust_simulate_rollout.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -87,7 +92,7 @@ def load():
 
 
 EXPORTS = ["ust_abi_version", "ust_create", "ust_destroy", "ust_last_error", "ust_create_error", "ust_launch_count",
-           "ust_host_alloc", "ust_host_free", "ust_apply_state", "ust_apply_state_device", "ust_stream", "ust_apply_state_packed", "ust_apply_state_delta", "ust_apply_state_delta_sparse", "ust_apply_state_delta_splice", "ust_apply_state_delta_reorder", "ust_apply_state_delta_pods", "ust_apply_state_delta_pods_reorder", "ust_fetch_outputs", "ust_fetch_outputs_pods", "ust_simulate_rollout", "ust_simulate_rollout_timed", "ust_sync",
+           "ust_host_alloc", "ust_host_free", "ust_apply_state", "ust_apply_state_device", "ust_stream", "ust_apply_state_packed", "ust_apply_state_delta", "ust_apply_state_delta_sparse", "ust_apply_state_delta_splice", "ust_apply_state_delta_reorder", "ust_apply_state_delta_pods", "ust_apply_state_delta_pods_reorder", "ust_apply_state_clocked", "ust_apply_state_delta_pods_clocked", "ust_fetch_outputs", "ust_fetch_outputs_pods", "ust_simulate_rollout", "ust_simulate_rollout_timed", "ust_sync",
            "ust_build_state", "ust_build_state_uids", "ust_build_state_delta", "ust_fetch_build_state", "ust_get_unique_id", "ust_comm_init", "ust_comm_set_mode", "ust_table_entry",
            "ust_table_window_shift", "ust_table_window"]
 
@@ -417,6 +422,72 @@ class Handle:
             C.addressof(pl) if pl is not None else None, int(idx.shape[0]), _p(idx), _p(ch["state"]), _p(ch["flags"]),
             _p(ch["pod_rev"]), _p(ch["ds_idx"]), int(ds_rev.shape[0]), _p(ds_rev), C.c_int64(int(max_out)), _p(out[0]),
             _p(out[1]), _p(out[2]), _p(out[3]), C.addressof(n_out), C.addressof(cnt))
+        return rc, int(n_out.value), out[0], out[1], out[2], out[3], cnt.as_dict()
+
+    def apply_state_clocked(self, policy, now, wait_timeout_seconds, start, soa, pods, out=None, clock_start=True):
+        """ust_apply_state_clocked: apply_state with pod lists, the two timeouts derived on the device from `now` and the
+        per-node start times `start` (int64). clock_start=False passes a NULL start (a rejection test); now=None a NULL
+        clock. Returns (rc, next_state, actions, outcome, counters-dict)."""
+        n = int(soa["state"].shape[0])
+        nxt, act, oc = out if out is not None else (np.zeros(n, np.uint8), np.zeros(n, np.uint16), np.full(n, 0xFF, np.uint8))
+        st = np.ascontiguousarray(start, dtype=np.int64) if start is not None else None
+        ck = abi.Clock(int(now), int(wait_timeout_seconds), _p(st) if clock_start else None, None) if now is not None else None
+        ps = None
+        if pods is not None:
+            off = np.ascontiguousarray(pods["pod_off"], dtype=np.int32)
+            pf = np.ascontiguousarray(pods["pod_flags"], dtype=np.uint16)
+            ps = abi.Pods(off.ctypes.data, pf.ctypes.data, int(pf.shape[0]))
+        cnt = abi.Counters()
+        rc = self._lib.ust_apply_state_clocked(
+            self._h, C.addressof(policy) if policy is not None else None, C.addressof(ck) if ck is not None else None, n,
+            _p(soa["state"]), _p(soa["flags"]), _p(soa["pod_rev"]), _p(soa["ds_idx"]), int(soa["ds_rev"].shape[0]),
+            _p(soa["ds_rev"]), C.addressof(ps) if ps is not None else None, _p(nxt), _p(act), _p(oc), C.addressof(cnt))
+        return rc, nxt, act, oc, cnt.as_dict()
+
+    def apply_state_delta_pods_clocked(self, policy, now, wait_timeout_seconds, reorder, lists, idx, changed, start, ds_rev,
+                                       max_out, insert_start=None, out=None, clock=True):
+        """ust_apply_state_delta_pods_clocked: apply_state_delta_pods_reorder on a clocked snapshot. `start` holds the start
+        times of the nodes at `idx`, `insert_start` those of the reorder's inserted nodes (None: NULL); clock=False passes a
+        NULL clock. Returns what apply_state_delta_pods returns."""
+        keep = []
+
+        def arr(a, dt):
+            a = np.ascontiguousarray(a, dtype=dt)
+            keep.append(a)
+            return a
+
+        ro = None
+        if reorder is not None:
+            src = arr(reorder.get("run_src", np.zeros(0)), np.int64)
+            ln = arr(reorder.get("run_len", np.zeros(0)), np.int64)
+            ins = {k: arr(reorder[k], dt) if k in reorder else None
+                   for k, dt in (("state", np.uint8), ("flags", np.uint32), ("pod_rev", np.int32), ("ds_idx", np.int32))}
+            n_ins = reorder.get("n_insert", 0 if ins["state"] is None else int(ins["state"].shape[0]))
+            ro = abi.Reorder(int(src.shape[0]), _p(src), _p(ln), int(n_ins), _p(ins["state"]), _p(ins["flags"]),
+                             _p(ins["pod_rev"]), _p(ins["ds_idx"]))
+        pl = None
+        if lists is not None:
+            ni = arr(lists["node_idx"], np.int64)
+            off = arr(lists["pod_off"], np.int32)
+            pf = arr(lists["pod_flags"], np.uint16)
+            pl = abi.PodLists(int(ni.shape[0]), _p(ni), _p(off), _p(pf), int(pf.shape[0]))
+        idx = arr(idx, np.int64)
+        ch = {"state": arr(changed["state"], np.uint8), "flags": arr(changed["flags"], np.uint32),
+              "pod_rev": arr(changed["pod_rev"], np.int32), "ds_idx": arr(changed["ds_idx"], np.int32)}
+        st = arr(start, np.int64) if start is not None else None
+        ist = arr(insert_start, np.int64) if insert_start is not None else None
+        ck = abi.Clock(int(now), int(wait_timeout_seconds), _p(st), _p(ist)) if clock else None
+        ds_rev = arr(ds_rev, np.int32)
+        if out is None:
+            out = (np.zeros(max_out + 1, np.int64), np.zeros(max_out + 1, np.uint8), np.zeros(max_out + 1, np.uint16),
+                   np.zeros(max_out + 1, np.uint8))
+        n_out = C.c_int64(0)
+        cnt = abi.Counters()
+        rc = self._lib.ust_apply_state_delta_pods_clocked(
+            self._h, C.addressof(policy) if policy is not None else None, C.addressof(ck) if ck is not None else None,
+            C.addressof(ro) if ro is not None else None, C.addressof(pl) if pl is not None else None, int(idx.shape[0]), _p(idx),
+            _p(ch["state"]), _p(ch["flags"]), _p(ch["pod_rev"]), _p(ch["ds_idx"]), int(ds_rev.shape[0]), _p(ds_rev),
+            C.c_int64(int(max_out)), _p(out[0]), _p(out[1]), _p(out[2]), _p(out[3]), C.addressof(n_out), C.addressof(cnt))
         return rc, int(n_out.value), out[0], out[1], out[2], out[3], cnt.as_dict()
 
     def fetch_outputs_pods(self, n):
