@@ -28,12 +28,12 @@ static const char* const kNullString = "null";  // consts.go:90
 static const char* const kTrueString = "true";  // consts.go:92
 static std::string g_driver_name;                 // util.go:91-99
 
-// The seven keys are functions of the driver name only (util.go:101-133). The reference formats them on every use; an
+// The eight keys are functions of the driver name only (util.go:101-133). The reference formats them on every use; an
 // encoder that walks a million nodes cannot (six formatted strings per node were a third of Encode's time), so they are
 // built once per SetDriverName.
 struct DriverKeys {
   bool valid = false;
-  std::string state, skip, safeLoad, requested, requestorMode, initialState, waitStart;
+  std::string state, skip, safeLoad, requested, requestorMode, initialState, waitStart, validationStart;
 };
 static DriverKeys g_keys;
 static std::string key(const char* tail) { return "nvidia.com/" + g_driver_name + tail; }
@@ -46,6 +46,7 @@ static const DriverKeys& keys() {
     g_keys.requestorMode = key("-driver-upgrade-requestor-mode");
     g_keys.initialState = key("-driver-upgrade.node-initial-state.unschedulable");
     g_keys.waitStart = key("-driver-upgrade-wait-for-pod-completion-start-time");
+    g_keys.validationStart = key("-driver-upgrade-validation-start-time");
     g_keys.valid = true;
   }
   return g_keys;
@@ -58,6 +59,7 @@ std::string GetUpgradeRequestedAnnotationKey() { return keys().requested; }
 std::string GetUpgradeRequestorModeAnnotationKey() { return keys().requestorMode; }
 std::string GetUpgradeInitialStateAnnotationKey() { return keys().initialState; }
 std::string GetWaitForPodCompletionStartTimeAnnotationKey() { return keys().waitStart; }
+std::string GetValidationStartTimeAnnotationKey() { return keys().validationStart; }
 
 bool IsOrphanedPod(const Pod& pod) { return pod.OwnerReferences.empty(); }
 bool IsNodeInRequestorMode(const Node& node) { return node.Annotations.count(keys().requestorMode) != 0; }
@@ -457,12 +459,104 @@ static void flatten_policy(const DriverUpgradePolicySpec& p, bool podDeletionEna
   c->use_maintenance_operator = useMaintenanceOperator;
 }
 
+// strconv.ParseInt(s, 10, 64) (Go 1.x): an optional sign, then decimal digits only; the error text is Go's. The input is
+// quoted as strconv.Quote does: \", \\, \a \b \f \n \r \t \v, other ASCII controls and bytes that are not valid UTF-8
+// as \xhh, C1 controls (U+0080-U+009F) as \u00hh. Other runes are copied: Go also escapes the non-printable ones among
+// them (format characters such as U+200B, unassigned code points), which this does not.
+static void goQuoteTo(const std::string& s, std::string* q) {
+  static const char* hex = "0123456789abcdef";
+  auto esc = [&](const char* pfx, unsigned v) { *q += pfx; *q += hex[(v >> 4) & 15]; *q += hex[v & 15]; };
+  *q += '"';
+  for (size_t i = 0; i < s.size();) {
+    const unsigned char ch = (unsigned char)s[i];
+    if (ch < 0x80) {
+      switch (ch) {
+        case '"': *q += "\\\""; break;
+        case '\\': *q += "\\\\"; break;
+        case '\a': *q += "\\a"; break;
+        case '\b': *q += "\\b"; break;
+        case '\f': *q += "\\f"; break;
+        case '\n': *q += "\\n"; break;
+        case '\r': *q += "\\r"; break;
+        case '\t': *q += "\\t"; break;
+        case '\v': *q += "\\v"; break;
+        default:
+          if (ch < 0x20 || ch == 0x7f) esc("\\x", ch); else *q += (char)ch;
+      }
+      i++;
+      continue;
+    }
+    // one UTF-8 sequence: its length and code point, or an invalid byte (overlong forms, surrogates and > U+10FFFF too)
+    const size_t len = ch >= 0xF0 ? 4 : ch >= 0xE0 ? 3 : ch >= 0xC0 ? 2 : 0;
+    uint32_t cp = len == 4 ? ch & 7u : len == 3 ? ch & 15u : ch & 31u;
+    bool ok = len > 0 && i + len <= s.size();
+    for (size_t k = 1; ok && k < len; k++) {
+      const unsigned char c = (unsigned char)s[i + k];
+      ok = (c & 0xC0) == 0x80;
+      cp = (cp << 6) | (c & 0x3Fu);
+    }
+    ok = ok && !(len == 2 && cp < 0x80) && !(len == 3 && cp < 0x800) && !(len == 4 && (cp < 0x10000 || cp > 0x10FFFF)) &&
+         !(cp >= 0xD800 && cp <= 0xDFFF);
+    if (!ok) { esc("\\x", ch); i++; continue; }
+    if (cp <= 0x9F) esc("\\u00", cp); else q->append(s, i, len);
+    i += len;
+  }
+  *q += '"';
+}
+static bool parseInt64(const std::string& s, int64_t* out, std::string* err) {
+  auto fail = [&](const char* what) {
+    *err = "strconv.ParseInt: parsing ";
+    goQuoteTo(s, err);
+    *err += ": ";
+    *err += what;
+    return false;
+  };
+  size_t i = 0;
+  bool neg = false;
+  if (!s.empty() && (s[0] == '+' || s[0] == '-')) { neg = s[0] == '-'; i = 1; }
+  if (i == s.size()) return fail("invalid syntax");
+  uint64_t u = 0;
+  for (; i < s.size(); i++) {
+    if (s[i] < '0' || s[i] > '9') return fail("invalid syntax");
+    const uint64_t d = (uint64_t)(s[i] - '0');
+    if (u > (UINT64_MAX - d) / 10) return fail("value out of range");  // ParseUint stops at the first overflow
+    u = u * 10 + d;
+  }
+  if (u > (neg ? (uint64_t)INT64_MAX + 1 : (uint64_t)INT64_MAX)) return fail("value out of range");
+  *out = neg ? (int64_t)(0 - u) : (int64_t)u;
+  return true;
+}
+
+// A validation pod as Validate sees it (validation_manager.go:95-136): it matched the selector, and it is ready when it
+// is Running, has container statuses and all of them are Ready.
+static uint16_t validationPodFlags(const Pod& p) {
+  bool ready = p.Phase == "Running" && !p.ContainerStatuses.empty();
+  for (const auto& cs : p.ContainerStatuses) ready = ready && cs.Ready;
+  return (uint16_t)(UST_POD_MATCH_VALIDATION_SELECTOR | (ready ? UST_POD_READY : 0));
+}
+
+// The one List of a ValidateOnDevice reconcile, grouped by node. The reference lists per node, with the selector and the
+// field selector spec.nodeName=<node> (validation_manager.go:77-79); this takes one cluster-wide List and keeps its
+// order within each node. That rests on one assumption: the API server returns a node's pods in the same relative order
+// in both Lists (it sorts a List by namespace and name). Validate's answer depends on that order: a ready pod listed
+// before a not-ready one resets the start time (INTEGRATION.md, "Encoding the validation pods").
+using PodsByNode = std::unordered_map<std::string, std::vector<const Pod*>>;
+static Error listValidationPods(K8sClient* client, const std::string& selector, PodsByNode* byNode) {
+  if (client == nullptr) return Errorf("no K8sClient to list the validation pods with");
+  std::vector<Pod*> pods;
+  if (Error e = client->ListPodsBySelector(selector, "", &pods)) return e;
+  for (const Pod* p : pods)
+    if (!p->NodeName.empty()) (*byNode)[p->NodeName].push_back(p);
+  return std::nullopt;
+}
+
 // One snapshot entry -> its four SoA values. `ds` / `dsErr`: index of its DaemonSet in the table (-1 = orphaned) and
 // whether that DaemonSet's revision-hash lookup failed; `deferred` receives an error the reference would raise when
-// its pass reaches the node.
+// its pass reaches the node; `validationStart` (ValidateOnDevice only, else nullptr) the parsed validation start time.
 Error ClusterUpgradeStateManagerImpl::encodeOne(const NodeUpgradeState* ns, int code, int32_t ds, bool dsErr,
                                                 std::map<std::string, int32_t>* intern, const std::vector<int32_t>& ds_rev,
-                                                uint8_t* hot_out, uint32_t* flags_out, int32_t* rev_out, std::string* deferred) {
+                                                uint8_t* hot_out, uint32_t* flags_out, int32_t* rev_out, std::string* deferred,
+                                                int64_t* validationStart) {
   auto internHash = [&](const std::string& h) {  // find first: emplace would build (and throw away) a map node per node
     auto it = intern->find(h);
     return it != intern->end() ? it->second : intern->emplace(h, (int32_t)intern->size() + 1).first->second;
@@ -521,6 +615,20 @@ Error ClusterUpgradeStateManagerImpl::encodeOne(const NodeUpgradeState* ns, int 
     f |= UST_F_NM_PRESENT;
     if (ns->NodeMaintenance->ReadyConditionWithReasonReady) f |= UST_F_NM_READY;
   }
+  if (validationStart) {  // StateOptions::ValidateOnDevice: the start-time annotation handleTimeout reads (validation_manager.go:142-160)
+    *validationStart = 0;
+    auto it = n.Annotations.find(keys().validationStart);
+    if (it != n.Annotations.end()) {
+      f |= UST_F_VALIDATION_START_ANNO;
+      std::string err;
+      if (!parseInt64(it->second, validationStart, &err)) {
+        f |= UST_F_VALIDATION_START_INVALID;
+        *validationStart = 0;
+        // Validate's error when it reaches the node (:97-101); the device returns UST_ERR_VALIDATION there
+        if (code == UST_STATE_VALIDATION_REQUIRED) *deferred = "unable to handle timeout for validation state: " + err;
+      }
+    }
+  }
   *hot_out = hot;
   *flags_out = f;
   *rev_out = rev;
@@ -573,6 +681,8 @@ Error ClusterUpgradeStateManagerImpl::Encode(const ClusterUpgradeState& s, const
   e.state.assign(n, 0);
   e.flags.assign(n, 0);
   e.pod_rev.assign(n, 0);
+  e.validateOnDevice = validateOnDevice();
+  if (e.validateOnDevice) e.start.assign(n, 0);
   const int32_t base = (int32_t)intern.size();
   const size_t workers = (size_t)std::max(1, std::min(opts_.EncodeThreads, (int)(n / 4096 + 1)));
   struct Part { std::map<std::string, int32_t> intern; std::vector<std::pair<size_t, std::string>> deferred; Error err; size_t errAt = 0; };
@@ -584,7 +694,8 @@ Error ClusterUpgradeStateManagerImpl::Encode(const ClusterUpgradeState& s, const
     for (size_t i = i0; i < i1; i++) {
       const int32_t ds = e.ds_idx[i];
       uint8_t hot; uint32_t f; int32_t rev; std::string deferred;
-      if (Error err = encodeOne(e.entries[i], codes[i], ds, ds >= 0 && dsHashError[(size_t)ds], &p.intern, e.ds_rev, &hot, &f, &rev, &deferred)) {
+      if (Error err = encodeOne(e.entries[i], codes[i], ds, ds >= 0 && dsHashError[(size_t)ds], &p.intern, e.ds_rev, &hot, &f, &rev, &deferred,
+                                e.validateOnDevice ? &e.start[i] : nullptr)) {
         p.err = err; p.errAt = i;
         return;
       }
@@ -620,6 +731,20 @@ Error ClusterUpgradeStateManagerImpl::Encode(const ClusterUpgradeState& s, const
         if (e.pod_rev[i] > base) e.pod_rev[i] = remap[(size_t)e.pod_rev[i]];
     }
   }
+  // 4. ValidateOnDevice: every entry's validation pods (an empty list when it has none), from one List
+  if (e.validateOnDevice) {
+    e.policy.evaluate_actuators = UST_EVAL_ACTUATORS | UST_EVAL_VALIDATION;
+    e.now = opts_.Now();
+    PodsByNode byNode;
+    e.listError = listValidationPods(K8sClient, validationSelector_, &byNode);
+    e.pod_off.assign(n + 1, 0);
+    for (size_t i = 0; i < n; i++) {
+      auto it = e.listError ? byNode.end() : byNode.find(e.entries[i]->Node->Name);
+      if (it != byNode.end())
+        for (const Pod* p : it->second) e.pod_flags.push_back(validationPodFlags(*p));
+      e.pod_off[i + 1] = (int32_t)e.pod_flags.size();
+    }
+  }
   return std::nullopt;
 }
 
@@ -632,6 +757,7 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
   const bool requestor = opts_.Requestor.UseMaintenanceOperator;
   auto setState = [&](size_t i) { return NodeUpgradeStateProvider->ChangeNodeUpgradeState(enc.entries[i]->Node, StateNameOfCode(next_state[i])); };
   auto anno = [&](size_t i, const std::string& k, const char* v) { return NodeUpgradeStateProvider->ChangeNodeUpgradeAnnotation(enc.entries[i]->Node, k, v); };
+  auto validationError = [](const Error& e) { return Errorf("unable to handle timeout for validation state: " + *e); };  // :97-101
   auto abortError = [&](long long idx = -1) -> Error {
     if (idx >= 0) { auto it = enc.deferred.find((size_t)idx); if (it != enc.deferred.end()) return Errorf(it->second); }
     return Errorf(ust_last_error(handle_));
@@ -653,7 +779,8 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
       if (code == UST_STATE_UNCORDON_REQUIRED) continue;  // two sub-passes below
       const unsigned a = actions[i];
       Node* node = enc.entries[i]->Node;
-      if (a & UST_A_ERROR) return abortError((long long)i);
+      const bool onDevice = code == UST_STATE_VALIDATION_REQUIRED && enc.validateOnDevice;
+      if ((a & UST_A_ERROR) && !onDevice) return abortError((long long)i);
       if (a & UST_A_CLEAR_UPGRADE_REQUESTED)
         if (Error e = anno(i, GetUpgradeRequestedAnnotationKey(), kNullString)) return e;
       if (a & UST_A_SET_INITIAL_STATE_ANNO)
@@ -662,7 +789,22 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
         if (Error e = CordonManager->Cordon(node)) return e;
       if (a & UST_A_UNBLOCK_SAFE_LOAD)
         if (Error e = SafeDriverLoadManager->UnblockLoading(node)) return e;
-      if (code == UST_STATE_VALIDATION_REQUIRED) {
+      if (onDevice) {
+        // the calls Validate makes (validation_manager.go:71-175), as the device answered it
+        if (enc.listError) return enc.listError;  // its List failed (:79-83)
+        if (a & UST_A_ERROR) return abortError((long long)i);  // the start time does not parse (:155-160)
+        const std::string& key = GetValidationStartTimeAnnotationKey();
+        if (next_state[i] == UST_STATE_FAILED) {  // handleTimeout: timed out (:161-172)
+          (void)NodeUpgradeStateProvider->ChangeNodeUpgradeState(node, UpgradeStateFailed);  // error ignored (:163)
+          if (Error e = anno(i, key, kNullString)) return validationError(e);
+          continue;
+        }
+        if (a & UST_A_CLEAR_WAIT_START)  // a ready pod (:106-113)
+          if (Error e = anno(i, key, kNullString)) return e;
+        if (a & UST_A_SET_WAIT_START)    // handleTimeout: no start time yet (:143-152)
+          if (Error e = anno(i, key, std::to_string(enc.now).c_str())) return validationError(e);
+        if (!(a & UST_A_SET_STATE)) continue;  // "Validations not complete on the node"
+      } else if (code == UST_STATE_VALIDATION_REQUIRED) {
         bool done = false;
         if (Error e = ValidationManager->Validate(node, &done)) return e;
         if (!done) continue;  // "Validations not complete on the node"
@@ -749,9 +891,19 @@ Error ClusterUpgradeStateManagerImpl::ApplyState(ClusterUpgradeState* currentSta
   std::vector<uint16_t> actions(n + 1);
   enc.state.push_back(0); enc.flags.push_back(0); enc.pod_rev.push_back(0); enc.ds_idx.push_back(0);  // never pass NULL for n == 0
   enc.ds_rev.push_back(0);
-  const int rc = ust_apply_state(handle_, &enc.policy, (int64_t)n, enc.state.data(), enc.flags.data(), enc.pod_rev.data(),
-                                 enc.ds_idx.data(), (int32_t)enc.ds_rev.size() - 1, enc.ds_rev.data(), nullptr, next.data(),
-                                 actions.data(), nullptr, &last_);
+  int rc;
+  if (enc.validateOnDevice) {  // Validate on the device: the validation pods, the start times and `now` go with the call
+    std::vector<uint8_t> outcome(n + 1);
+    enc.pod_flags.push_back(0); enc.start.push_back(0);
+    const ust_pods pods = {enc.pod_off.data(), enc.pod_flags.data(), (int64_t)enc.pod_flags.size() - 1};
+    const ust_clock clock = {enc.now, upgradePolicy->WaitForCompletion ? upgradePolicy->WaitForCompletion->TimeoutSecond : 0, enc.start.data(), nullptr};
+    rc = ust_apply_state_clocked(handle_, &enc.policy, &clock, (int64_t)n, enc.state.data(), enc.flags.data(), enc.pod_rev.data(),
+                                 enc.ds_idx.data(), (int32_t)enc.ds_rev.size() - 1, enc.ds_rev.data(), &pods, next.data(), actions.data(),
+                                 outcome.data(), &last_);
+  } else {
+    rc = ust_apply_state(handle_, &enc.policy, (int64_t)n, enc.state.data(), enc.flags.data(), enc.pod_rev.data(), enc.ds_idx.data(),
+                         (int32_t)enc.ds_rev.size() - 1, enc.ds_rev.data(), nullptr, next.data(), actions.data(), nullptr, &last_);
+  }
   if (rc == UST_ERR_CUDA || rc == UST_ERR_INVALID_ARGUMENT || rc == UST_ERR_NIL_STATE) return Errorf(ust_last_error(handle_));
   return Replay(enc, *upgradePolicy, next.data(), actions.data(), rc, last_);
 }
@@ -827,6 +979,91 @@ int ClusterUpgradeStateManagerImpl::EvaluateCached(const ust_policy& policy, boo
   return rc;
 }
 
+int ClusterUpgradeStateManagerImpl::EvaluateCachedPods(const ust_policy& policy, int64_t now, int64_t waitTimeout, bool full,
+                                                       const std::vector<int64_t>& changed, Cache* cache, ust_counters* c) {
+  Cache& k = *cache;
+  const size_t n = k.slots.size();
+  if (handle_ == nullptr) return UST_ERR_CUDA;
+  // never pass NULL for empty arrays
+  std::vector<int32_t> dsrev = k.ds_rev;
+  dsrev.push_back(0);
+  std::vector<int32_t> off;
+  std::vector<uint16_t> pf;
+  auto csr = [&](size_t m, const int64_t* rows) {  // the lists of `rows` (nullptr: every slot) as one CSR
+    off.assign(m + 1, 0);
+    for (size_t j = 0; j < m; j++) {
+      const auto& l = k.lists[rows ? (size_t)rows[j] : j];
+      pf.insert(pf.end(), l.begin(), l.end());
+      off[j + 1] = (int32_t)pf.size();
+    }
+    pf.push_back(0);
+  };
+  std::vector<uint8_t> outcome(n + 1);
+  if (full) {
+    k.next.assign(n + 1, 0);
+    k.actions.assign(n + 1, 0);
+    std::vector<uint8_t> st = k.state; st.push_back(0);
+    std::vector<uint32_t> fl = k.flags; fl.push_back(0);
+    std::vector<int32_t> rv = k.pod_rev; rv.push_back(0);
+    std::vector<int32_t> di = k.ds_idx; di.push_back(0);
+    std::vector<int64_t> sv = k.start; sv.push_back(0);
+    csr(n, nullptr);
+    const ust_pods pods = {off.data(), pf.data(), (int64_t)pf.size() - 1};
+    const ust_clock clock = {now, waitTimeout, sv.data(), nullptr};
+    return ust_apply_state_clocked(handle_, &policy, &clock, (int64_t)n, st.data(), fl.data(), rv.data(), di.data(), (int32_t)k.ds_rev.size(),
+                                   dsrev.data(), &pods, k.next.data(), k.actions.data(), outcome.data(), c);
+  }
+  const size_t m = changed.size();
+  std::vector<uint8_t> st(m + 1);
+  std::vector<uint32_t> fl(m + 1);
+  std::vector<int32_t> rv(m + 1), di(m + 1);
+  std::vector<int64_t> sv(m + 1), ix(changed);
+  ix.push_back(0);
+  for (size_t j = 0; j < m; j++) {
+    const size_t i = (size_t)changed[j];
+    st[j] = k.state[i]; fl[j] = k.flags[i]; rv[j] = k.pod_rev[i]; di[j] = k.ds_idx[i]; sv[j] = k.start[i];
+  }
+  // nodes that joined: their columns and start times from the cache, at the positions the runs give them
+  const Cache::Splice& ps = k.pending;
+  const size_t ni = ps.insert_at.size();
+  std::vector<uint8_t> ist(ni + 1);
+  std::vector<uint32_t> ifl(ni + 1);
+  std::vector<int32_t> irv(ni + 1), idi(ni + 1);
+  std::vector<int64_t> isv(ni + 1);
+  for (size_t j = 0; j < ni; j++) {
+    const size_t i = (size_t)ps.insert_at[j];
+    ist[j] = k.state[i]; ifl[j] = k.flags[i]; irv[j] = k.pod_rev[i]; idi[j] = k.ds_idx[i]; isv[j] = k.start[i];
+  }
+  const ust_reorder reorder = {(int64_t)ps.run_src.size(), ps.run_src.data(), ps.run_len.data(), (int64_t)ni,
+                               ist.data(), ifl.data(), irv.data(), idi.data()};
+  std::vector<int64_t> li(k.listChanged);
+  li.push_back(0);
+  csr(k.listChanged.size(), k.listChanged.data());
+  const ust_pod_lists lists = {(int64_t)k.listChanged.size(), li.data(), off.data(), pf.data(), (int64_t)pf.size() - 1};
+  const ust_clock clock = {now, waitTimeout, sv.data(), isv.data()};
+  const int64_t cap = (int64_t)(n / 4 + 1024);
+  std::vector<int64_t> oi((size_t)cap + 1);
+  std::vector<uint8_t> on((size_t)cap + 1), oo((size_t)cap + 1);
+  std::vector<uint16_t> oa((size_t)cap + 1);
+  int64_t n_out = 0;
+  const int rc = ust_apply_state_delta_pods_clocked(handle_, &policy, &clock, ps.empty() ? nullptr : &reorder,
+                                                    k.listChanged.empty() ? nullptr : &lists, (int64_t)m, ix.data(), st.data(), fl.data(),
+                                                    rv.data(), di.data(), (int32_t)k.ds_rev.size(), dsrev.data(), cap, oi.data(), on.data(),
+                                                    oa.data(), oo.data(), &n_out, c);
+  if (rc == UST_ERR_CUDA || rc == UST_ERR_INVALID_ARGUMENT || rc == UST_ERR_COMM) return rc;
+  if (n_out > cap) {  // UST_ERR_TRUNCATED or a reference-level abort with more outputs than the arrays hold: fetch them all
+    stats_.outputs_received += (int64_t)n;
+    k.next.resize(n + 1);
+    k.actions.resize(n + 1);
+    const int frc = ust_fetch_outputs_pods(handle_, k.next.data(), k.actions.data(), outcome.data());
+    if (frc != UST_OK) return frc;
+    return rc == UST_ERR_TRUNCATED ? UST_OK : rc;
+  }
+  for (int64_t j = 0; j < n_out; j++) { k.next[(size_t)oi[(size_t)j]] = on[(size_t)j]; k.actions[(size_t)oi[(size_t)j]] = oa[(size_t)j]; }
+  stats_.outputs_received += n_out;
+  return rc;
+}
+
 Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState* currentState, const DriverUpgradePolicySpec* upgradePolicy) {
   if (currentState == nullptr) return Errorf("currentState should not be empty");  // upgrade_state.go:175-177
   if (upgradePolicy == nullptr || !upgradePolicy->AutoUpgrade) return std::nullopt;  // upgrade_state.go:179-182
@@ -834,6 +1071,18 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
   flatten_policy(*upgradePolicy, podDeletionStateEnabled_, validationStateEnabled_, opts_.Requestor.UseMaintenanceOperator, &pol);
   Cache& k = cache_;
   stats_.reconciles++;
+  // ValidateOnDevice: the cache holds the clocked pod-list snapshot; a change of mode starts it over
+  const bool dev = validateOnDevice();
+  if (k.valid && k.pods != dev) ResetIncremental();
+  k.pods = dev;
+  int64_t now = 0;
+  PodsByNode byNode;
+  Error listErr;
+  if (dev) {
+    pol.evaluate_actuators = UST_EVAL_ACTUATORS | UST_EVAL_VALIDATION;
+    now = opts_.Now();
+    listErr = listValidationPods(K8sClient, validationSelector_, &byNode);
+  }
   const bool full = !k.valid;
   for (auto& sl : k.slots) sl.seen = false;
   // the DaemonSet table: identities are cached by UID, revision hashes are looked up once per DaemonSet per reconcile
@@ -902,7 +1151,8 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
   }
   for (size_t i = 0; i < nOld; i++)
     if (!present[i]) sp.remove_idx.push_back((int64_t)i);
-  if (moved) {  // maximal runs of consecutive old slots, joins as inserted runs
+  if (moved || (dev && !sp.empty())) {  // maximal runs of consecutive old slots, joins as inserted runs (the pod-list calls
+                                        // take no splice)
     sp.insert_before.clear();
     orderRuns(from, &sp.run_src, &sp.run_len);
   }
@@ -930,6 +1180,7 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
         nk.slots.back().id = id;
         nk.state.push_back(UST_STATE_EXCLUDED); nk.flags.push_back(0); nk.pod_rev.push_back(0); nk.ds_idx.push_back(-1);
         nk.next.push_back(0); nk.actions.push_back(0); nk.deferredMsg.emplace_back();
+        if (dev) { nk.lists.emplace_back(); nk.listSig.emplace_back("\x01"); nk.start.push_back(0); }
         continue;
       }
       const size_t q = (size_t)from[p];
@@ -937,9 +1188,11 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
       nk.state.push_back(k.state[q]); nk.flags.push_back(k.flags[q]); nk.pod_rev.push_back(k.pod_rev[q]); nk.ds_idx.push_back(k.ds_idx[q]);
       nk.next.push_back(q < k.next.size() ? k.next[q] : 0); nk.actions.push_back(q < k.actions.size() ? k.actions[q] : 0);
       nk.deferredMsg.push_back(std::move(k.deferredMsg[q]));
+      if (dev) { nk.lists.push_back(std::move(k.lists[q])); nk.listSig.push_back(std::move(k.listSig[q])); nk.start.push_back(k.start[q]); }
     }
     k.slots.swap(nk.slots); k.state.swap(nk.state); k.flags.swap(nk.flags); k.pod_rev.swap(nk.pod_rev); k.ds_idx.swap(nk.ds_idx);
     k.next.swap(nk.next); k.actions.swap(nk.actions); k.deferredMsg.swap(nk.deferredMsg);
+    k.lists.swap(nk.lists); k.listSig.swap(nk.listSig); k.start.swap(nk.start);
     for (size_t i = 0; i < k.slots.size(); i++) k.slotOfId[k.slots[i].id] = i;
   }
   if (!full) {
@@ -952,6 +1205,10 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
   // this reconcile's view in pass order (what Replay walks): entry, its slot
   EncodedSnapshot view;
   view.policy = pol;
+  view.validateOnDevice = dev;
+  view.now = now;
+  view.listError = listErr;
+  std::vector<char> sendList(dev ? k.slots.size() : 0, 0);
   std::vector<size_t> slotOfView;
   bool orderBroken = false;
   auto visit = [&](NodeUpgradeState* ns, int code) -> Error {
@@ -970,10 +1227,12 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
                       (ns->NodeMaintenance ? (ns->NodeMaintenance->ReadyConditionWithReasonReady ? "R" : "P") : "-");
     if (!versioned || sig != sl.sig || sl.code != code) {
       uint8_t hot; uint32_t f; int32_t rev; std::string deferred;
-      if (Error err = encodeOne(ns, code, ds, dsErr, &k.intern, k.ds_rev, &hot, &f, &rev, &deferred)) return err;
+      int64_t start = 0;
+      if (Error err = encodeOne(ns, code, ds, dsErr, &k.intern, k.ds_rev, &hot, &f, &rev, &deferred, dev ? &start : nullptr)) return err;
       stats_.encoded++;
-      if (hot != k.state[i] || f != k.flags[i] || rev != k.pod_rev[i] || ds != k.ds_idx[i]) {
+      if (hot != k.state[i] || f != k.flags[i] || rev != k.pod_rev[i] || ds != k.ds_idx[i] || (dev && start != k.start[i])) {
         k.state[i] = hot; k.flags[i] = f; k.pod_rev[i] = rev; k.ds_idx[i] = ds;
+        if (dev) k.start[i] = start;
         if (joined.empty() || !joined[i]) changed.push_back((int64_t)i);  // a joined node travels with the splice / reorder
       }
       k.deferredMsg[i] = deferred;
@@ -981,6 +1240,30 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
       sl.code = code;
     } else {
       stats_.reused++;
+    }
+    if (dev) {
+      // the node's validation pods: rebuilt when the (pod, resourceVersion) sequence changed, sent when the bits did (or the
+      // node joined: an inserted node brings its list). After a failed List the resident lists stay as they are.
+      const bool joinedNode = !joined.empty() && joined[i];
+      if (!listErr) {
+        auto it = byNode.find(n.Name);
+        std::string lsig;
+        bool lversioned = true;
+        if (it != byNode.end())
+          for (const Pod* p : it->second) {
+            lversioned = lversioned && !p->ResourceVersion.empty();
+            lsig += p->Namespace + "/" + p->Name + "@" + p->ResourceVersion + ";";
+          }
+        if (!lversioned || lsig != k.listSig[i]) {
+          std::vector<uint16_t> fl;
+          if (it != byNode.end())
+            for (const Pod* p : it->second) fl.push_back(validationPodFlags(*p));
+          if (fl != k.lists[i]) { k.lists[i].swap(fl); sendList[i] = 1; }
+          k.listSig[i] = lversioned ? lsig : std::string("\x01");
+        }
+      }
+      if (joinedNode) sendList[i] = 1;
+      if (code == UST_STATE_VALIDATION_REQUIRED) stats_.validate_avoided++;
     }
     if (!slotOfView.empty() && (int)(view.state.back() & UST_HOT_STATE_MASK) == code && slotOfView.back() > i)
       orderBroken = true;  // within a bucket, slot order must be the slice order: slots are handed out in it
@@ -1013,7 +1296,19 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
   }
   std::sort(changed.begin(), changed.end());
   if (full) stats_.full_uploads++;
-  const int rc = EvaluateCached(pol, full, changed, &k, &last_);
+  int rc;
+  if (dev) {
+    k.listChanged.clear();
+    for (size_t i = 0; i < sendList.size(); i++)
+      if (full || sendList[i]) k.listChanged.push_back((int64_t)i);
+    stats_.lists_sent += (int64_t)k.listChanged.size();
+    stats_.lists_reused += (int64_t)(k.slots.size() - k.listChanged.size());
+    if (!full && changed.empty() && k.listChanged.empty() && k.pending.empty()) stats_.time_only++;
+    rc = EvaluateCachedPods(pol, now, upgradePolicy->WaitForCompletion ? upgradePolicy->WaitForCompletion->TimeoutSecond : 0, full, changed,
+                            &k, &last_);
+  } else {
+    rc = EvaluateCached(pol, full, changed, &k, &last_);
+  }
   if (rc == UST_ERR_CUDA || rc == UST_ERR_INVALID_ARGUMENT || rc == UST_ERR_NIL_STATE || rc == UST_ERR_COMM) {
     ResetIncremental();
     return Errorf(handle_ ? ust_last_error(handle_) : "no H100 device bound to this manager: ApplyState has no CPU path");

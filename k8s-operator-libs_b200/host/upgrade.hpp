@@ -16,6 +16,7 @@
 // in the reference's pass order. Without libust.so / a H100 every ApplyState returns an error.
 #pragma once
 #include <cstdint>
+#include <ctime>
 #include <functional>
 #include <map>
 #include <memory>
@@ -57,6 +58,7 @@ std::string GetUpgradeRequestedAnnotationKey();
 std::string GetUpgradeRequestorModeAnnotationKey();
 std::string GetUpgradeInitialStateAnnotationKey();
 std::string GetWaitForPodCompletionStartTimeAnnotationKey();
+std::string GetValidationStartTimeAnnotationKey();
 
 // ---- the slice of corev1 / appsv1 the path reads --------------------------------------------------------
 using StringMap = std::map<std::string, std::string>;
@@ -181,6 +183,13 @@ struct K8sClient {
   // (:370-414), the NodeMaintenance CRUD of the upgrade-required and uncordon-required passes
   virtual Error CreateOrUpdateNodeMaintenance(NodeUpgradeState* nodeState) { (void)nodeState; return std::nullopt; }
   virtual Error DeleteOrUpdateNodeMaintenance(NodeUpgradeState* nodeState) { (void)nodeState; return std::nullopt; }
+  // The ValidationManager's List (validation_manager.go:77-79): the pods of every namespace that match the label selector
+  // `selector` ("k=v[,k=v]") and run on node `nodeName` ("" = on any node), in the order the API returns them. Used by
+  // StateOptions::ValidateOnDevice, which makes one such List per reconcile with nodeName "".
+  virtual Error ListPodsBySelector(const std::string& selector, const std::string& nodeName, std::vector<Pod*>* out) {
+    (void)selector; (void)nodeName; (void)out;
+    return Errorf("this K8sClient cannot list pods by label selector");
+  }
 };
 
 struct RequestorOptions { bool UseMaintenanceOperator = false; };  // upgrade_requestor.go:527-546 (the switch only)
@@ -191,6 +200,15 @@ struct StateOptions {                                                 // upgrade
   // the injected PodManager::GetPodControllerRevisionHash and SafeDriverLoadManager::IsWaitingForSafeDriverLoad are called
   // concurrently (they are read-only in the reference: pod_manager.go:84-89, safe_driver_load_manager.go:51-57).
   int EncodeThreads = 1;
+  // Not in the reference: answer ValidationManager::Validate on the device (UST_EVAL_VALIDATION) instead of calling it.
+  // With a non-empty WithValidationEnabled selector, ApplyState and ApplyStateIncremental make one
+  // K8sClient::ListPodsBySelector per reconcile, hand every node its validation pods and its parsed validation start-time
+  // annotation to the clocked pod-list calls, and replay the annotation and state calls Validate would have made; the
+  // injected ValidationManager is never called. ApplyStateIncremental then keeps the lists and start times resident too.
+  bool ValidateOnDevice = false;
+  // The reconcile's time.Now().Unix(): read once per ApplyState call; the device derives the validation timeout from it
+  // and a new validation start-time annotation is set to it.
+  std::function<int64_t()> Now = [] { return (int64_t)time(nullptr); };
 };
 
 // ---- the encoded snapshot (include/ust.h layout) and its replay ------------------------------------------
@@ -201,6 +219,15 @@ struct EncodedSnapshot {
   std::vector<int32_t> pod_rev, ds_idx, ds_rev;
   std::map<size_t, std::string> deferred;  // an error the reference raises when it reaches the node (IsWaitingForSafeDriverLoad)
   ust_policy policy{};
+  // StateOptions::ValidateOnDevice (with a validation selector): per entry its validation pods (CSR, UST_POD_* bits in the
+  // List's order) and its parsed validation start-time annotation; the reconcile's `now`; and the List's error, which
+  // Replay returns at the first validation-required node, after its UnblockLoading, as Validate would.
+  bool validateOnDevice = false;
+  std::vector<int32_t> pod_off;
+  std::vector<uint16_t> pod_flags;
+  std::vector<int64_t> start;
+  int64_t now = 0;
+  Error listError;
 };
 
 // ---- common_manager.go:23-41 --------------------------------------------------------------------------------
@@ -296,9 +323,14 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
     int64_t inserted = 0, removed = 0;  // nodes that joined / left the cached snapshot by a splice or reorder
     int64_t reorders = 0;               // reconciles that went to the device as a reorder (a surviving node moved)
     int64_t slots = 0;                  // size of the cached snapshot after the last reconcile
+    // StateOptions::ValidateOnDevice: validation pod lists sent to the device / left resident, reconciles that sent no node
+    // and no list (only time passed), and the ValidationManager::Validate calls (one API List each) not made
+    int64_t lists_sent = 0, lists_reused = 0, time_only = 0, validate_avoided = 0;
   };
   const IncrementalStats& Stats() const { return stats_; }
   void ResetIncremental();
+  // Switches StateOptions::ValidateOnDevice; the incremental cache starts over on the next call when the mode changes.
+  void SetValidateOnDevice(bool on) { opts_.ValidateOnDevice = on; }
 
   // ---- incremental BuildState: the driver-pod list stays on the device (ust_build_state_delta) -----------------------------
   // The same contract, result and errors as BuildState, for a reconcile loop that calls it again and again. The manager keeps
@@ -371,13 +403,30 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
     std::map<std::string, int32_t> dsIndexByUID;
     std::vector<bool> dsHashError;
     bool valid = false;
+    // StateOptions::ValidateOnDevice only (pods == true): per slot its validation pod list, the (pod, resourceVersion)
+    // sequence it was built from ("" = no pods, "\x01" = unknown) and its validation start time; and the slots whose list
+    // goes down with this call, in slot order (every inserted slot among them). In this mode pending never holds a
+    // splice: a change of node order is always run_src / run_len, as the pod-list calls take it.
+    bool pods = false;
+    std::vector<std::vector<uint16_t>> lists;
+    std::vector<std::string> listSig;
+    std::vector<int64_t> start;
+    std::vector<int64_t> listChanged;
   };
   virtual int EvaluateCached(const ust_policy& policy, bool full, const std::vector<int64_t>& changed, Cache* cache, ust_counters* c);
+  // The same on the clocked pod-list snapshot (StateOptions::ValidateOnDevice): full: ust_apply_state_clocked with every
+  // list and start time; else ust_apply_state_delta_pods_clocked with cache->pending as runs, the lists of
+  // cache->listChanged and the start times of `changed` and of the inserted slots. `now` / `waitTimeout` make the ust_clock.
+  virtual int EvaluateCachedPods(const ust_policy& policy, int64_t now, int64_t waitTimeout, bool full,
+                                 const std::vector<int64_t>& changed, Cache* cache, ust_counters* c);
   ClusterUpgradeStateManagerImpl() = default;
+  explicit ClusterUpgradeStateManagerImpl(StateOptions opts) : opts_(std::move(opts)) {}  // a manager without a device
 
  private:
   Error encodeOne(const NodeUpgradeState* ns, int code, int32_t ds, bool dsErr, std::map<std::string, int32_t>* intern,
-                  const std::vector<int32_t>& ds_rev, uint8_t* hot, uint32_t* flags, int32_t* rev, std::string* deferred);
+                  const std::vector<int32_t>& ds_rev, uint8_t* hot, uint32_t* flags, int32_t* rev, std::string* deferred,
+                  int64_t* validationStart);
+  bool validateOnDevice() const { return opts_.ValidateOnDevice && validationStateEnabled_; }
   Error assembleState(const std::vector<Pod*>& podList, const uint8_t* podState, const int32_t* owner_idx,
                       std::map<std::string, DaemonSet*>& daemonSets, std::unique_ptr<ClusterUpgradeState>* out);
   Cache cache_;
