@@ -1153,48 +1153,83 @@ static int pods_reorder_segments(ust_handle* h, const ust_pod_lists* pl, int64_t
   return UST_OK;
 }
 
-// ust_apply_state_delta, _delta_sparse, _delta_splice, _delta_reorder, _delta_pods and _delta_pods_reorder: bring the
-// resident snapshot into a new node order (optional: nodes leave, join and move), scatter the re-encoded nodes into it,
-// evaluate everything, return all outputs (dense) or the outputs that differ from the previous call's (sparse). `pods`:
-// the pod-list snapshot, whose lists `pl` (nullable) replaces first (after its reorder, `ro`, which moves the lists and
-// the previous outcome with the nodes); its sparse outputs include actuator_outcome (written to `actuator_outcome`).
-// `clock` (pod-list snapshot left by a clocked call only): the start times move with the nodes, the changed and inserted
-// nodes bring theirs, and the two timeouts are derived before the evaluation.
-static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splice* sp, const ust_reorder* ro, bool pods,
-                        const ust_pod_lists* pl, int64_t n_changed, const int64_t* idx, const uint8_t* state, const uint32_t* flags,
-                        const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, bool sparse,
-                        uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome, int64_t max_out, int64_t* out_idx,
-                        int64_t* n_out, ust_counters* out, const ust_clock* clock = nullptr) {
-  if (int rc = check_eval_mode(h, policy, pods)) return rc;
-  const int64_t n_old = pods ? h->pods_n : h->resident_n;
-  if (n_old < 0 && pods)
+// One call of ust_apply_state_delta, _delta_sparse, _delta_splice, _delta_reorder, _delta_pods, _delta_pods_reorder or
+// _delta_pods_clocked. The constructors take the arguments every dense or sparse entry point has, in ABI order
+// (actuator_outcome: pod-list calls only among the sparse ones); an entry point then sets the fields of its own structs.
+struct DeltaCall {
+  const ust_policy* policy;
+  int64_t n_changed;                     // the re-encoded nodes: their indices and (wide) columns
+  const int64_t* idx;
+  HostNodes changed;
+  int32_t n_ds;
+  const int32_t* ds_rev;
+  uint8_t* next_state;                   // outputs: n entries each (dense) or max_out entries each and their count (sparse)
+  uint16_t* actions;
+  uint8_t* actuator_outcome;
+  ust_counters* out;
+  bool sparse = false;
+  int64_t max_out = 0;
+  int64_t* out_idx = nullptr;
+  int64_t* n_out = nullptr;
+  const ust_splice* splice = nullptr;    // the new node order: at most one of the two
+  const ust_reorder* reorder = nullptr;
+  bool pods = false;                     // the call is on the pod-list snapshot, `lists` (nullable) replaces some of its lists
+  const ust_pod_lists* lists = nullptr;
+  bool clocked = false;                  // the entry point takes a clock, which must be given
+  const ust_clock* clock = nullptr;
+  DeltaCall(const ust_policy* policy_, int64_t n_changed_, const int64_t* idx_, const uint8_t* state, const uint32_t* flags,
+            const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds_, const int32_t* ds_rev_, uint8_t* next_state_,
+            uint16_t* actions_, uint8_t* actuator_outcome_, ust_counters* out_)
+      : policy(policy_), n_changed(n_changed_), idx(idx_), changed{state, flags, pod_rev, ds_idx, nullptr, nullptr}, n_ds(n_ds_),
+        ds_rev(ds_rev_), next_state(next_state_), actions(actions_), actuator_outcome(actuator_outcome_), out(out_) {}
+  DeltaCall(const ust_policy* policy_, int64_t n_changed_, const int64_t* idx_, const uint8_t* state, const uint32_t* flags,
+            const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds_, const int32_t* ds_rev_, int64_t max_out_, int64_t* out_idx_,
+            uint8_t* next_state_, uint16_t* actions_, uint8_t* actuator_outcome_, int64_t* n_out_, ust_counters* out_)
+      : DeltaCall(policy_, n_changed_, idx_, state, flags, pod_rev, ds_idx, n_ds_, ds_rev_, next_state_, actions_, actuator_outcome_, out_) {
+    sparse = true; max_out = max_out_; out_idx = out_idx_; n_out = n_out_;
+  }
+};
+
+// What the checks of a delta call derive from it. The host scratch they fill besides (the reorder's runs, the pod-list
+// segments, h->pod_len_next, h->pl_shift_host) is overwritten by the next call's checks; nothing resident changes.
+struct DeltaPlan {
+  int64_t n_old = 0, n = 0;            // snapshot size before and after the new node order
+  int64_t n_remove = 0, n_insert = 0;  // nodes removed (splice) and inserted (splice or reorder) ...
+  HostNodes ins = {};                  // ... and the inserted nodes' columns
+  bool gather = false;                 // the node order changes: columns and previous outputs move into the second set
+  int64_t new_total = 0;               // pods of the new pod-list snapshot
+  bool same_len = true;                // every replaced list keeps its length: copied in place
+  bool pods_gather = false;            // a reorder of the pod-list snapshot: its CSR is gathered anew
+};
+
+// Every check of a delta call, before any device work: a call that fails here leaves the resident snapshot as it was.
+static int plan_delta(ust_handle* h, const DeltaCall& c, DeltaPlan* p) {
+  if (c.clocked && !c.clock) return h->fail(UST_ERR_INVALID_ARGUMENT, "clock: required");
+  if (int rc = check_eval_mode(h, c.policy, c.pods)) return rc;
+  const int64_t n_old = c.pods ? h->pods_n : h->resident_n;
+  if (n_old < 0 && c.pods)
     return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident pod-list snapshot: call ust_apply_state with pod lists and actuator_outcome first");
   if (n_old < 0) return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident snapshot: call ust_apply_state (without pod lists) first");
-  if (pods && h->pods_clocked != (clock != nullptr))
-    return h->fail(UST_ERR_INVALID_ARGUMENT, clock ? "the resident pod-list snapshot has no start times: it was left by an unclocked call"
-                                                   : "the resident pod-list snapshot was left by a clocked call: use ust_apply_state_delta_pods_clocked");
-  if (clock) {
-    if (int rc = check_clock(h, policy, clock, n_changed > 0)) return rc;
-    if (ro && ro->n_insert > 0 && !clock->insert_start)
+  if (c.pods && h->pods_clocked != (c.clock != nullptr))
+    return h->fail(UST_ERR_INVALID_ARGUMENT, c.clock ? "the resident pod-list snapshot has no start times: it was left by an unclocked call"
+                                                     : "the resident pod-list snapshot was left by a clocked call: use ust_apply_state_delta_pods_clocked");
+  if (c.clock) {
+    if (int rc = check_clock(h, c.policy, c.clock, c.n_changed > 0)) return rc;
+    if (c.reorder && c.reorder->n_insert > 0 && !c.clock->insert_start)
       return h->fail(UST_ERR_INVALID_ARGUMENT, "clock: insert_start is NULL while the reorder inserts nodes");
   }
-  if (sparse && !pods && !h->outputs_resident)
+  if (c.sparse && !c.pods && !h->outputs_resident)
     return h->fail(UST_ERR_INVALID_ARGUMENT, "no resident outputs to compare with: the previous call must be an ApplyState on this snapshot");
   // the new node order, checked in full before anything is touched
-  int64_t n = n_old, n_ins = 0;
-  const uint8_t* ins_state = nullptr;
-  const uint32_t* ins_flags = nullptr;
-  const int32_t *ins_rev = nullptr, *ins_ds = nullptr;
-  bool gather = false;
-  if (ro) {
+  p->n_old = p->n = n_old;
+  if (const ust_reorder* ro = c.reorder) {
     if (ro->n_insert > 0 && (!ro->state || !ro->flags || !ro->pod_rev || !ro->ds_idx)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad reorder");
-    if (int rc = reorder_runs(h, ro->n_runs, ro->run_src, ro->run_len, ro->n_insert, n_old, &n)) return rc;
-    gather = true;
-    n_ins = ro->n_insert;
-    ins_state = ro->state; ins_flags = ro->flags; ins_rev = ro->pod_rev; ins_ds = ro->ds_idx;
-  } else {
-    const int64_t n_rm = sp ? sp->n_remove : 0;
-    n_ins = sp ? sp->n_insert : 0;
+    if (int rc = reorder_runs(h, ro->n_runs, ro->run_src, ro->run_len, ro->n_insert, n_old, &p->n)) return rc;
+    p->gather = true;
+    p->n_insert = ro->n_insert;
+    p->ins = HostNodes{ro->state, ro->flags, ro->pod_rev, ro->ds_idx, nullptr, nullptr};
+  } else if (const ust_splice* sp = c.splice) {
+    const int64_t n_rm = sp->n_remove, n_ins = sp->n_insert;
     if (n_rm < 0 || n_ins < 0 || n_rm > n_old || (n_rm > 0 && !sp->remove_idx) ||
         (n_ins > 0 && (!sp->insert_before || !sp->state || !sp->flags || !sp->pod_rev || !sp->ds_idx)))
       return h->fail(UST_ERR_INVALID_ARGUMENT, "bad splice");
@@ -1206,27 +1241,27 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
       if (sp->insert_before[k] < (k ? sp->insert_before[k - 1] : 0) || sp->insert_before[k] > n_old)
         return h->fail(UST_ERR_INVALID_ARGUMENT, "splice: insert_before[%lld] = %lld is not non-decreasing in [0, %lld]", (long long)k,
                        (long long)sp->insert_before[k], (long long)n_old);
-    n = n_old - n_rm + n_ins;
-    gather = n_rm || n_ins;
-    if (gather) {
-      ins_state = sp->state; ins_flags = sp->flags; ins_rev = sp->pod_rev; ins_ds = sp->ds_idx;
-    }
+    p->n = n_old - n_rm + n_ins;
+    p->gather = n_rm || n_ins;
+    p->n_remove = n_rm; p->n_insert = n_ins;
+    p->ins = HostNodes{sp->state, sp->flags, sp->pod_rev, sp->ds_idx, nullptr, nullptr};
   }
+  const int64_t n = p->n;
   if (n >= (1LL << 40)) return h->fail(UST_ERR_INVALID_ARGUMENT, "too many nodes");
-  if (n_changed < 0 || (n_changed > 0 && (!idx || !state || !flags || !pod_rev || !ds_idx)))
+  if (c.n_changed < 0 || (c.n_changed > 0 && (!c.idx || !c.changed.state || !c.changed.flags || !c.changed.rev || !c.changed.ds)))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
-  if (!sparse && n > 0 && (!next_state || !actions)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
-  if (sparse && (max_out < 0 || !n_out || (max_out > 0 && (!out_idx || !next_state || !actions || (pods && !actuator_outcome)))))
+  if (!c.sparse && n > 0 && (!c.next_state || !c.actions)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
+  if (c.sparse && (c.max_out < 0 || !c.n_out || (c.max_out > 0 && (!c.out_idx || !c.next_state || !c.actions || (c.pods && !c.actuator_outcome)))))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
-  if (n_ds < 0 || (n_ds > 0 && !ds_rev)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad DaemonSet table");
-  for (int64_t k = 0; k < n_changed; k++)
-    if (idx[k] < 0 || idx[k] >= n) return h->fail(UST_ERR_INVALID_ARGUMENT, "changed node %lld has index %lld outside the snapshot of %lld nodes", (long long)k, (long long)idx[k], (long long)n);
+  if (c.n_ds < 0 || (c.n_ds > 0 && !c.ds_rev)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad DaemonSet table");
+  for (int64_t k = 0; k < c.n_changed; k++)
+    if (c.idx[k] < 0 || c.idx[k] >= n) return h->fail(UST_ERR_INVALID_ARGUMENT, "changed node %lld has index %lld outside the snapshot of %lld nodes", (long long)k, (long long)c.idx[k], (long long)n);
   // replacement pod lists, checked in O(n_lists + n_pods) against the host copy of the resident list lengths; with every
   // length kept they are copied in place, otherwise the CSR is laid out anew (pl_shift_host: prefix of the length changes).
   // Under a reorder the CSR is always gathered anew, from the segments that pods_reorder_segments cuts.
-  const int64_t L = pods && pl ? pl->n_lists : 0;
-  int64_t new_total = pods ? h->pods_total : 0;
-  bool same_len = true;
+  const ust_pod_lists* pl = c.lists;
+  const int64_t L = c.pods && pl ? pl->n_lists : 0;
+  p->new_total = c.pods ? h->pods_total : 0;
   if (L != 0) {
     if (L < 0 || !pl->node_idx || !pl->pod_off || pl->n_pods < 0 || (pl->n_pods > 0 && !pl->pod_flags))
       return h->fail(UST_ERR_INVALID_ARGUMENT, "bad pod lists");
@@ -1236,10 +1271,10 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
                        (long long)pl->node_idx[k], (long long)n);
     if (int rc = check_pod_offsets_host(h, L, pl->pod_off, pl->n_pods)) return rc;
   }
-  const bool pods_gather = pods && ro;
-  if (pods_gather) {
+  p->pods_gather = c.pods && c.reorder;
+  if (p->pods_gather) {
     const auto t0 = std::chrono::steady_clock::now();
-    if (int rc = pods_reorder_segments(h, pl, L, n, &new_total)) return rc;
+    if (int rc = pods_reorder_segments(h, pl, L, n, &p->new_total)) return rc;
     h->pod_pass_ns = std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::steady_clock::now() - t0).count();
   } else if (L != 0) {
     h->pl_shift_host.resize((size_t)L + 1);
@@ -1247,124 +1282,132 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
     for (int64_t k = 0; k < L; k++) {
       h->pl_shift_host[(size_t)k] = (int32_t)d;  // |d| stays below 2^31 when the new total does (checked below)
       const int32_t len = pl->pod_off[k + 1] - pl->pod_off[k];
-      same_len = same_len && len == h->pod_len[(size_t)pl->node_idx[k]];
+      p->same_len = p->same_len && len == h->pod_len[(size_t)pl->node_idx[k]];
       d += (int64_t)len - h->pod_len[(size_t)pl->node_idx[k]];
     }
     h->pl_shift_host[(size_t)L] = (int32_t)d;
-    new_total += d;
-    if (new_total >= (1LL << 31)) return h->fail(UST_ERR_INVALID_ARGUMENT, "pod lists: %lld pods in all, pod_off is int32", (long long)new_total);
+    p->new_total += d;
+    if (p->new_total >= (1LL << 31)) return h->fail(UST_ERR_INVALID_ARGUMENT, "pod lists: %lld pods in all, pod_off is int32", (long long)p->new_total);
   }
+  return UST_OK;
+}
+
+// The device work of a delta call once plan_delta has passed: the new node order (the previous outputs move with the nodes;
+// on the pod-list snapshot their lists, previous outcome and start times too), the replaced lists, the re-encoded nodes,
+// the two timeouts (clocked), the evaluation, then all outputs (dense) or those that differ from the previous call's
+// (sparse), and the new snapshot becomes the resident one.
+static int run_delta(ust_handle* h, const DeltaCall& c, const DeltaPlan& p) {
   UST_CUDA(h, cudaSetDevice(h->device));
   StreamDrain drain(h);
   cudaStream_t st = h->stream;
-  const size_t N = (size_t)n, M = (size_t)n_changed, I = (size_t)n_ins, NR = h->run_src.size();
-  const size_t R = !ro && gather ? (size_t)sp->n_remove : 0;
-  if (gather) {  // the previous outputs travel with the snapshot
+  const int64_t L = c.pods && c.lists ? c.lists->n_lists : 0;
+  const size_t N = (size_t)p.n, M = (size_t)c.n_changed, I = (size_t)p.n_insert, NR = h->run_src.size(), R = (size_t)p.n_remove;
+  if (p.gather) {  // the previous outputs travel with the snapshot
     UST_CUDA(h, h->splice_cols.reserve(N));
     UST_CUDA(h, h->splice_outs.reserve(N));
-    if (ro) UST_CUDA(h, h->runs.reserve(2 * NR + 2));
+    if (c.reorder) UST_CUDA(h, h->runs.reserve(2 * NR + 2));
     else UST_CUDA(h, h->removed.reserve(R + 1));
-    if (!ro) UST_CUDA(h, h->inserted.idx.reserve(I + 1));
+    if (!c.reorder) UST_CUDA(h, h->inserted.idx.reserve(I + 1));
     UST_CUDA(h, h->inserted.cols.reserve(I));
   }
-  UST_CUDA(h, h->s_dsrev.reserve((size_t)n_ds + 1));
+  UST_CUDA(h, h->s_dsrev.reserve((size_t)c.n_ds + 1));
   // (under a reorder s_outcome holds the previous outcome at the old size, which the gather reads: it is not resized)
-  if (pods ? !ro : actuator_outcome != nullptr) UST_CUDA(h, h->s_outcome.reserve(N + 16));
-  if (pods && sparse) {
+  if (c.pods ? !c.reorder : c.actuator_outcome != nullptr) UST_CUDA(h, h->s_outcome.reserve(N + 16));
+  if (c.pods && c.sparse) {
     UST_CUDA(h, h->s_outcome_prev.reserve(N + 16));
-    UST_CUDA(h, h->sp_outcome.reserve((size_t)max_out + 1));
+    UST_CUDA(h, h->sp_outcome.reserve((size_t)c.max_out + 1));
   }
-  const size_t S = pods_gather ? h->seg_src.size() : 0;
-  if (pods_gather) {
+  const size_t S = p.pods_gather ? h->seg_src.size() : 0;
+  if (p.pods_gather) {
     UST_CUDA(h, h->splice_outcome.reserve(N + 16));
     UST_CUDA(h, h->pr_segs.reserve(2 * S + 1));
     UST_CUDA(h, h->pr_pods.reserve(2 * S + 1));
     UST_CUDA(h, h->s_podoff2.reserve(N + 1));
-    UST_CUDA(h, h->s_podflags2.reserve((size_t)new_total + 16));
+    UST_CUDA(h, h->s_podflags2.reserve((size_t)p.new_total + 16));
   }
   if (L) {  // the new lists carry 8 pods of padding for the relayout's 16-byte loads, the new CSR too
     UST_CUDA(h, h->pl_idx.reserve((size_t)L));
     UST_CUDA(h, h->pl_off.reserve((size_t)L + 1));
-    UST_CUDA(h, h->pl_flags.reserve((size_t)pl->n_pods + 16));
-    if (!same_len) {
+    UST_CUDA(h, h->pl_flags.reserve((size_t)c.lists->n_pods + 16));
+    if (!p.same_len) {
       UST_CUDA(h, h->pl_shift.reserve((size_t)L + 1));
       UST_CUDA(h, h->pl_runs.reserve(4 * (size_t)L + 3));
       UST_CUDA(h, h->s_podoff2.reserve(N + 1));
-      UST_CUDA(h, h->s_podflags2.reserve((size_t)new_total + 16));
+      UST_CUDA(h, h->s_podflags2.reserve((size_t)p.new_total + 16));
     }
   }
   UST_CUDA(h, h->changed.idx.reserve(M + 1));
   UST_CUDA(h, h->changed.cols.reserve(M));
-  if (clock) {
+  if (c.clock) {
     UST_CUDA(h, h->chg_start.reserve(M + 1));
-    if (ro) {
+    if (c.reorder) {
       UST_CUDA(h, h->s_start2.reserve(N + 1));
       UST_CUDA(h, h->ins_start.reserve(I + 1));
     }
   }
-  if (sparse) {  // the pair this call writes holds the new size as well
+  if (c.sparse) {  // the pair this call writes holds the new size as well
     UST_CUDA(h, h->outs_prev.reserve(N));
-    UST_CUDA(h, h->sp_blocks.reserve((size_t)ust_diff_blocks(n) + 1));
-    UST_CUDA(h, h->sp_idx.reserve((size_t)max_out + 1));
-    UST_CUDA(h, h->outs_sparse.reserve((size_t)max_out));
+    UST_CUDA(h, h->sp_blocks.reserve((size_t)ust_diff_blocks(p.n) + 1));
+    UST_CUDA(h, h->sp_idx.reserve((size_t)c.max_out + 1));
+    UST_CUDA(h, h->outs_sparse.reserve((size_t)c.max_out));
   }
   drop_resident(h);  // until the patched snapshot has been evaluated
-  if (pods_gather) std::swap(h->pod_len, h->pod_len_next);
-  else for (int64_t k = 0; k < L; k++) h->pod_len[(size_t)pl->node_idx[k]] = pl->pod_off[k + 1] - pl->pod_off[k];
-  if (n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsrev.p, ds_rev, (size_t)n_ds * 4, cudaMemcpyHostToDevice, st));
+  if (p.pods_gather) std::swap(h->pod_len, h->pod_len_next);
+  else for (int64_t k = 0; k < L; k++) h->pod_len[(size_t)c.lists->node_idx[k]] = c.lists->pod_off[k + 1] - c.lists->pod_off[k];
+  if (c.n_ds) UST_CUDA(h, cudaMemcpyAsync(h->s_dsrev.p, c.ds_rev, (size_t)c.n_ds * 4, cudaMemcpyHostToDevice, st));
   if (L) {
-    if (!pods_gather) UST_CUDA(h, cudaMemcpyAsync(h->pl_idx.p, pl->node_idx, (size_t)L * 8, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, cudaMemcpyAsync(h->pl_off.p, pl->pod_off, ((size_t)L + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (pl->n_pods) UST_CUDA(h, cudaMemcpyAsync(h->pl_flags.p, pl->pod_flags, (size_t)pl->n_pods * 2, cudaMemcpyHostToDevice, st));
+    if (!p.pods_gather) UST_CUDA(h, cudaMemcpyAsync(h->pl_idx.p, c.lists->node_idx, (size_t)L * 8, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, cudaMemcpyAsync(h->pl_off.p, c.lists->pod_off, ((size_t)L + 1) * 4, cudaMemcpyHostToDevice, st));
+    if (c.lists->n_pods) UST_CUDA(h, cudaMemcpyAsync(h->pl_flags.p, c.lists->pod_flags, (size_t)c.lists->n_pods * 2, cudaMemcpyHostToDevice, st));
   }
-  if (pods_gather) {  // the run table and the gather of the new CSR, into the second pair
+  if (p.pods_gather) {  // the run table and the gather of the new CSR, into the second pair
     long long* segs = h->pr_segs.p;
     UST_CUDA(h, cudaMemcpyAsync(segs, h->seg_node.data(), (S + 1) * 8, cudaMemcpyHostToDevice, st));
     if (S) UST_CUDA(h, cudaMemcpyAsync(segs + S + 1, h->seg_src.data(), S * 8, cudaMemcpyHostToDevice, st));
     UST_CUDA(h, cudaMemcpyAsync(h->pr_pods.p, h->seg_pod.data(), (S + 1) * 4, cudaMemcpyHostToDevice, st));
-    int e = ust_launch_pods_reorder((long long)n, (long long)S, segs, h->pr_pods.p, h->s_podoff.p, h->s_podflags.p, h->pl_off.p,
-                                    h->pl_flags.p, (int)new_total, h->s_podoff2.p, h->s_podflags2.p, 8 * h->num_sms, st);
+    int e = ust_launch_pods_reorder((long long)p.n, (long long)S, segs, h->pr_pods.p, h->s_podoff.p, h->s_podflags.p, h->pl_off.p,
+                                    h->pl_flags.p, (int)p.new_total, h->s_podoff2.p, h->s_podflags2.p, 8 * h->num_sms, st);
     if (e) return h->fail(UST_ERR_CUDA, "pod-list reorder kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 2;
     std::swap(h->s_podoff, h->s_podoff2);
     std::swap(h->s_podflags, h->s_podflags2);
   } else if (L) {
     int e;
-    if (same_len) {
+    if (p.same_len) {
       e = ust_launch_pods_scatter((long long)L, h->pl_idx.p, h->pl_off.p, h->pl_flags.p, h->s_podoff.p, h->s_podflags.p, 8 * h->num_sms, st);
       h->launches += 1;
     } else {
       UST_CUDA(h, cudaMemcpyAsync(h->pl_shift.p, h->pl_shift_host.data(), ((size_t)L + 1) * 4, cudaMemcpyHostToDevice, st));
-      e = ust_launch_pods_relayout((long long)n, (long long)L, h->pl_idx.p, h->pl_off.p, h->pl_shift.p, h->s_podoff.p, h->s_podflags.p,
-                                   h->pl_flags.p, (int)new_total, h->pl_runs.p, h->s_podoff2.p, h->s_podflags2.p, 8 * h->num_sms, st);
+      e = ust_launch_pods_relayout((long long)p.n, (long long)L, h->pl_idx.p, h->pl_off.p, h->pl_shift.p, h->s_podoff.p, h->s_podflags.p,
+                                   h->pl_flags.p, (int)p.new_total, h->pl_runs.p, h->s_podoff2.p, h->s_podflags2.p, 8 * h->num_sms, st);
       h->launches += 2;
       std::swap(h->s_podoff, h->s_podoff2);
       std::swap(h->s_podflags, h->s_podflags2);
     }
     if (e) return h->fail(UST_ERR_CUDA, "pod-list kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
   }
-  if (gather) {
-    UST_CUDA(h, h->inserted.cols.upload(ins_state, ins_flags, ins_rev, ins_ds, 0, I, st));
+  if (p.gather) {
+    UST_CUDA(h, h->inserted.cols.upload(p.ins.state, p.ins.flags, p.ins.rev, p.ins.ds, 0, I, st));
     const Columns &in = h->inserted.cols, &s = h->staged, &x = h->splice_cols;
     int e;
-    if (ro) {
+    if (c.reorder) {
       long long* off = h->runs.p;
       long long* src = h->runs.p + NR + 1;
       UST_CUDA(h, cudaMemcpyAsync(off, h->run_off.data(), (NR + 1) * 8, cudaMemcpyHostToDevice, st));
       if (NR) UST_CUDA(h, cudaMemcpyAsync(src, h->run_src.data(), NR * 8, cudaMemcpyHostToDevice, st));
-      if (clock && I) UST_CUDA(h, cudaMemcpyAsync(h->ins_start.p, clock->insert_start, I * 8, cudaMemcpyHostToDevice, st));
-      e = ust_launch_reorder((long long)n, (long long)NR, off, src, in.hot.p, in.flags.p, in.rev.p, in.ds.p, s.hot.p, s.flags.p, s.rev.p,
-                             s.ds.p, h->outs.next.p, h->outs.actions.p, pods ? h->s_outcome.p : nullptr, x.hot.p, x.flags.p, x.rev.p,
-                             x.ds.p, h->splice_outs.next.p, h->splice_outs.actions.p, pods ? h->splice_outcome.p : nullptr, st,
-                             clock ? h->ins_start.p : nullptr, clock ? h->s_start.p : nullptr, clock ? h->s_start2.p : nullptr);
+      if (c.clock && I) UST_CUDA(h, cudaMemcpyAsync(h->ins_start.p, c.clock->insert_start, I * 8, cudaMemcpyHostToDevice, st));
+      e = ust_launch_reorder((long long)p.n, (long long)NR, off, src, in.hot.p, in.flags.p, in.rev.p, in.ds.p, s.hot.p, s.flags.p, s.rev.p,
+                             s.ds.p, h->outs.next.p, h->outs.actions.p, c.pods ? h->s_outcome.p : nullptr, x.hot.p, x.flags.p, x.rev.p,
+                             x.ds.p, h->splice_outs.next.p, h->splice_outs.actions.p, c.pods ? h->splice_outcome.p : nullptr, st,
+                             c.clock ? h->ins_start.p : nullptr, c.clock ? h->s_start.p : nullptr, c.clock ? h->s_start2.p : nullptr);
       if (e) return h->fail(UST_ERR_CUDA, "reorder kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
-      if (pods) std::swap(h->s_outcome, h->splice_outcome);  // the previous outcome in the new order
-      if (clock) std::swap(h->s_start, h->s_start2);          // the start times in the new order
+      if (c.pods) std::swap(h->s_outcome, h->splice_outcome);  // the previous outcome in the new order
+      if (c.clock) std::swap(h->s_start, h->s_start2);          // the start times in the new order
     } else {
       // a splice keeps its own kernel: the gather kernel measured slower on splices (DESIGN.md §3.4)
-      if (R) UST_CUDA(h, cudaMemcpyAsync(h->removed.p, sp->remove_idx, R * 8, cudaMemcpyHostToDevice, st));
-      if (I) UST_CUDA(h, cudaMemcpyAsync(h->inserted.idx.p, sp->insert_before, I * 8, cudaMemcpyHostToDevice, st));
-      e = ust_launch_splice((long long)n_old, (long long)R, h->removed.p, (long long)n_ins, h->inserted.idx.p, in.hot.p, in.flags.p,
+      if (R) UST_CUDA(h, cudaMemcpyAsync(h->removed.p, c.splice->remove_idx, R * 8, cudaMemcpyHostToDevice, st));
+      if (I) UST_CUDA(h, cudaMemcpyAsync(h->inserted.idx.p, c.splice->insert_before, I * 8, cudaMemcpyHostToDevice, st));
+      e = ust_launch_splice((long long)p.n_old, (long long)R, h->removed.p, (long long)p.n_insert, h->inserted.idx.p, in.hot.p, in.flags.p,
                             in.rev.p, in.ds.p, s.hot.p, s.flags.p, s.rev.p, s.ds.p, h->outs.next.p, h->outs.actions.p,
                             x.hot.p, x.flags.p, x.rev.p, x.ds.p, h->splice_outs.next.p, h->splice_outs.actions.p, st);
       if (e) return h->fail(UST_ERR_CUDA, "splice kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
@@ -1376,115 +1419,112 @@ static int delta_common(ust_handle* h, const ust_policy* policy, const ust_splic
   }
   if (M) {
     static_assert(sizeof(long long) == sizeof(int64_t), "index width");
-    UST_CUDA(h, cudaMemcpyAsync(h->changed.idx.p, idx, M * 8, cudaMemcpyHostToDevice, st));
-    UST_CUDA(h, h->changed.cols.upload(state, flags, pod_rev, ds_idx, 0, M, st));
-    if (clock) UST_CUDA(h, cudaMemcpyAsync(h->chg_start.p, clock->start, M * 8, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, cudaMemcpyAsync(h->changed.idx.p, c.idx, M * 8, cudaMemcpyHostToDevice, st));
+    UST_CUDA(h, h->changed.cols.upload(c.changed.state, c.changed.flags, c.changed.rev, c.changed.ds, 0, M, st));
+    if (c.clock) UST_CUDA(h, cudaMemcpyAsync(h->chg_start.p, c.clock->start, M * 8, cudaMemcpyHostToDevice, st));
     const Columns &d = h->changed.cols, &s = h->staged;
-    int e = ust_launch_patch((long long)n_changed, h->changed.idx.p, d.hot.p, d.flags.p, d.rev.p, d.ds.p, s.hot.p, s.flags.p,
-                             s.rev.p, s.ds.p, st, clock ? h->chg_start.p : nullptr, clock ? h->s_start.p : nullptr);
+    int e = ust_launch_patch((long long)c.n_changed, h->changed.idx.p, d.hot.p, d.flags.p, d.rev.p, d.ds.p, s.hot.p, s.flags.p,
+                             s.rev.p, s.ds.p, st, c.clock ? h->chg_start.p : nullptr, c.clock ? h->s_start.p : nullptr);
     if (e) return h->fail(UST_ERR_CUDA, "patch kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 1;
   }
-  if (clock) {
-    int rc = launch_clock(h, clock, n, st);
+  if (c.clock) {
+    int rc = launch_clock(h, c.clock, p.n, st);
     if (rc) return rc;
   }
-  if (sparse) std::swap(h->outs, h->outs_prev);  // the previous call's outputs step aside; this call writes the other pair
-  if (sparse && pods) std::swap(h->s_outcome, h->s_outcome_prev);
-  int rc = apply_device(h, policy, n, h->staged.hot.p, h->staged.flags.p, h->staged.rev.p, h->staged.ds.p, n_ds, h->s_dsrev.p,
-                        pods ? h->s_podoff.p : nullptr, pods ? h->s_podflags.p : nullptr, pods ? new_total : 0, h->outs.next.p,
-                        h->outs.actions.p, actuator_outcome || pods ? h->s_outcome.p : nullptr, nullptr, st);
+  if (c.sparse) std::swap(h->outs, h->outs_prev);  // the previous call's outputs step aside; this call writes the other pair
+  if (c.sparse && c.pods) std::swap(h->s_outcome, h->s_outcome_prev);
+  int rc = apply_device(h, c.policy, p.n, h->staged.hot.p, h->staged.flags.p, h->staged.rev.p, h->staged.ds.p, c.n_ds, h->s_dsrev.p,
+                        c.pods ? h->s_podoff.p : nullptr, c.pods ? h->s_podflags.p : nullptr, c.pods ? p.new_total : 0, h->outs.next.p,
+                        h->outs.actions.p, c.actuator_outcome || c.pods ? h->s_outcome.p : nullptr, nullptr, st);
   if (rc) return rc;
-  if (!sparse) {
+  if (!c.sparse) {
     if (N) {
-      UST_CUDA(h, cudaMemcpyAsync(next_state, h->outs.next.p, N, cudaMemcpyDeviceToHost, st));
-      UST_CUDA(h, cudaMemcpyAsync(actions, h->outs.actions.p, N * 2, cudaMemcpyDeviceToHost, st));
-      if (actuator_outcome) UST_CUDA(h, cudaMemcpyAsync(actuator_outcome, h->s_outcome.p, N, cudaMemcpyDeviceToHost, st));
+      UST_CUDA(h, cudaMemcpyAsync(c.next_state, h->outs.next.p, N, cudaMemcpyDeviceToHost, st));
+      UST_CUDA(h, cudaMemcpyAsync(c.actions, h->outs.actions.p, N * 2, cudaMemcpyDeviceToHost, st));
+      if (c.actuator_outcome) UST_CUDA(h, cudaMemcpyAsync(c.actuator_outcome, h->s_outcome.p, N, cudaMemcpyDeviceToHost, st));
     }
   } else {
-    int e = ust_launch_diff((long long)n, h->outs.next.p, h->outs.actions.p, pods ? h->s_outcome.p : nullptr, h->outs_prev.next.p,
-                            h->outs_prev.actions.p, pods ? h->s_outcome_prev.p : nullptr, h->sp_blocks.p, h->sp_count_dev,
-                            (long long)max_out, h->sp_idx.p, h->outs_sparse.next.p, h->outs_sparse.actions.p,
-                            pods ? h->sp_outcome.p : nullptr, st);
+    int e = ust_launch_diff((long long)p.n, h->outs.next.p, h->outs.actions.p, c.pods ? h->s_outcome.p : nullptr, h->outs_prev.next.p,
+                            h->outs_prev.actions.p, c.pods ? h->s_outcome_prev.p : nullptr, h->sp_blocks.p, h->sp_count_dev,
+                            (long long)c.max_out, h->sp_idx.p, h->outs_sparse.next.p, h->outs_sparse.actions.p,
+                            c.pods ? h->sp_outcome.p : nullptr, st);
     if (e) return h->fail(UST_ERR_CUDA, "diff kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
     h->launches += 3;
     UST_CUDA(h, cudaMemcpyAsync(h->sp_count_host, h->sp_count_dev, sizeof(long long), cudaMemcpyDeviceToHost, st));
     UST_CUDA(h, cudaStreamSynchronize(st));
     const int64_t cnt = *h->sp_count_host;
-    *n_out = cnt;
-    if (cnt <= max_out && cnt > 0) {
-      UST_CUDA(h, cudaMemcpyAsync(out_idx, h->sp_idx.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, st));
-      UST_CUDA(h, cudaMemcpyAsync(next_state, h->outs_sparse.next.p, (size_t)cnt, cudaMemcpyDeviceToHost, st));
-      UST_CUDA(h, cudaMemcpyAsync(actions, h->outs_sparse.actions.p, (size_t)cnt * 2, cudaMemcpyDeviceToHost, st));
-      if (pods) UST_CUDA(h, cudaMemcpyAsync(actuator_outcome, h->sp_outcome.p, (size_t)cnt, cudaMemcpyDeviceToHost, st));
+    *c.n_out = cnt;
+    if (cnt <= c.max_out && cnt > 0) {
+      UST_CUDA(h, cudaMemcpyAsync(c.out_idx, h->sp_idx.p, (size_t)cnt * 8, cudaMemcpyDeviceToHost, st));
+      UST_CUDA(h, cudaMemcpyAsync(c.next_state, h->outs_sparse.next.p, (size_t)cnt, cudaMemcpyDeviceToHost, st));
+      UST_CUDA(h, cudaMemcpyAsync(c.actions, h->outs_sparse.actions.p, (size_t)cnt * 2, cudaMemcpyDeviceToHost, st));
+      if (c.pods) UST_CUDA(h, cudaMemcpyAsync(c.actuator_outcome, h->sp_outcome.p, (size_t)cnt, cudaMemcpyDeviceToHost, st));
     }
   }
-  rc = adopt_resident(h, finish_with_counters(h, st, out), n, n_ds, true, pods ? new_total : -1, clock != nullptr);
-  if (sparse && (rc == UST_OK) && *n_out > max_out)
-    return h->fail(UST_ERR_TRUNCATED, "%lld outputs changed, the caller's arrays hold %lld: fetch them with %s", (long long)*n_out,
-                   (long long)max_out, pods ? "ust_fetch_outputs_pods" : "ust_fetch_outputs");
+  rc = adopt_resident(h, finish_with_counters(h, st, c.out), p.n, c.n_ds, true, c.pods ? p.new_total : -1, c.clock != nullptr);
+  if (c.sparse && (rc == UST_OK) && *c.n_out > c.max_out)
+    return h->fail(UST_ERR_TRUNCATED, "%lld outputs changed, the caller's arrays hold %lld: fetch them with %s", (long long)*c.n_out,
+                   (long long)c.max_out, c.pods ? "ust_fetch_outputs_pods" : "ust_fetch_outputs");
   return rc;
+}
+
+// The entry of every delta call. `one_gpu`: the name of an entry point that refuses more than one rank (ust_comm_init): a
+// shard's node indices and pod lists are its own, so a new order or new lists would have to reach every rank.
+static int delta_entry(ust_handle* h, const char* one_gpu, const DeltaCall& c) {
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
+  if (one_gpu && h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "%s runs on one GPU", one_gpu);
+  DeltaPlan p;
+  const int rc = plan_delta(h, c, &p);
+  return rc ? rc : run_delta(h, c, p);
 }
 
 int ust_apply_state_delta(ust_handle* h, const ust_policy* policy, int64_t n_changed, const int64_t* idx, const uint8_t* state,
                           const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds,
                           const int32_t* ds_rev, uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome,
                           ust_counters* out) {
-  if (!h) return UST_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> g(h->mu);
-  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  return delta_common(h, policy, nullptr, nullptr, false, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, false, next_state, actions,
-                      actuator_outcome, 0, nullptr, nullptr, out);
+  return delta_entry(h, nullptr, DeltaCall(policy, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, next_state, actions,
+                                           actuator_outcome, out));
 }
 
 int ust_apply_state_delta_sparse(ust_handle* h, const ust_policy* policy, int64_t n_changed, const int64_t* idx,
                                  const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx,
                                  int32_t n_ds, const int32_t* ds_rev, int64_t max_out, int64_t* out_idx,
                                  uint8_t* out_next_state, uint16_t* out_actions, int64_t* n_out, ust_counters* out) {
-  if (!h) return UST_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> g(h->mu);
-  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  return delta_common(h, policy, nullptr, nullptr, false, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
-                      nullptr, max_out, out_idx, n_out, out);
+  return delta_entry(h, nullptr, DeltaCall(policy, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, max_out, out_idx,
+                                           out_next_state, out_actions, nullptr, n_out, out));
 }
 
 int ust_apply_state_delta_splice(ust_handle* h, const ust_policy* policy, const ust_splice* splice, int64_t n_changed,
                                  const int64_t* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
                                  const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, int64_t max_out, int64_t* out_idx,
                                  uint8_t* out_next_state, uint16_t* out_actions, int64_t* n_out, ust_counters* out) {
-  if (!h) return UST_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> g(h->mu);
-  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  // node indices of a shard are global ranges (ust_comm_init): a splice would have to move them on every rank
-  if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_splice runs on one GPU");
-  return delta_common(h, policy, splice, nullptr, false, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state, out_actions,
-                      nullptr, max_out, out_idx, n_out, out);
+  DeltaCall c(policy, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, max_out, out_idx, out_next_state, out_actions,
+              nullptr, n_out, out);
+  c.splice = splice;
+  return delta_entry(h, "ust_apply_state_delta_splice", c);
 }
 
 int ust_apply_state_delta_reorder(ust_handle* h, const ust_policy* policy, const ust_reorder* reorder, int64_t n_changed,
                                   const int64_t* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
                                   const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, int64_t max_out, int64_t* out_idx,
                                   uint8_t* out_next_state, uint16_t* out_actions, int64_t* n_out, ust_counters* out) {
-  if (!h) return UST_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> g(h->mu);
-  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  // node indices of a shard are global ranges (ust_comm_init): a reorder would have to move them on every rank
-  if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_reorder runs on one GPU");
-  return delta_common(h, policy, nullptr, reorder, false, nullptr, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true, out_next_state,
-                      out_actions, nullptr, max_out, out_idx, n_out, out);
+  DeltaCall c(policy, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, max_out, out_idx, out_next_state, out_actions,
+              nullptr, n_out, out);
+  c.reorder = reorder;
+  return delta_entry(h, "ust_apply_state_delta_reorder", c);
 }
 
 int ust_apply_state_delta_pods(ust_handle* h, const ust_policy* policy, const ust_pod_lists* lists, int64_t n_changed,
                                const int64_t* idx, const uint8_t* state, const uint32_t* flags, const int32_t* pod_rev,
                                const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, int64_t max_out, int64_t* out_idx,
                                uint8_t* out_next_state, uint16_t* out_actions, uint8_t* out_outcome, int64_t* n_out, ust_counters* out) {
-  if (!h) return UST_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> g(h->mu);
-  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  // the pod lists of a shard hold that shard's nodes only; the call keeps to one GPU like the splice and the reorder
-  if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_pods runs on one GPU");
-  return delta_common(h, policy, nullptr, nullptr, true, lists, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true,
-                      out_next_state, out_actions, out_outcome, max_out, out_idx, n_out, out);
+  DeltaCall c(policy, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, max_out, out_idx, out_next_state, out_actions,
+              out_outcome, n_out, out);
+  c.pods = true; c.lists = lists;
+  return delta_entry(h, "ust_apply_state_delta_pods", c);
 }
 
 int ust_apply_state_delta_pods_reorder(ust_handle* h, const ust_policy* policy, const ust_reorder* reorder, const ust_pod_lists* lists,
@@ -1492,13 +1532,10 @@ int ust_apply_state_delta_pods_reorder(ust_handle* h, const ust_policy* policy, 
                                        const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev, int64_t max_out,
                                        int64_t* out_idx, uint8_t* out_next_state, uint16_t* out_actions, uint8_t* out_outcome,
                                        int64_t* n_out, ust_counters* out) {
-  if (!h) return UST_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> g(h->mu);
-  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  // node indices and pod lists of a shard are its own: a reorder would have to move them on every rank
-  if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_pods_reorder runs on one GPU");
-  return delta_common(h, policy, nullptr, reorder, true, lists, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true,
-                      out_next_state, out_actions, out_outcome, max_out, out_idx, n_out, out);
+  DeltaCall c(policy, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, max_out, out_idx, out_next_state, out_actions,
+              out_outcome, n_out, out);
+  c.reorder = reorder; c.pods = true; c.lists = lists;
+  return delta_entry(h, "ust_apply_state_delta_pods_reorder", c);
 }
 
 int ust_apply_state_delta_pods_clocked(ust_handle* h, const ust_policy* policy, const ust_clock* clock, const ust_reorder* reorder,
@@ -1506,13 +1543,10 @@ int ust_apply_state_delta_pods_clocked(ust_handle* h, const ust_policy* policy, 
                                        const uint32_t* flags, const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds,
                                        const int32_t* ds_rev, int64_t max_out, int64_t* out_idx, uint8_t* out_next_state,
                                        uint16_t* out_actions, uint8_t* out_outcome, int64_t* n_out, ust_counters* out) {
-  if (!h) return UST_ERR_INVALID_ARGUMENT;
-  std::lock_guard<std::mutex> g(h->mu);
-  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
-  if (h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_apply_state_delta_pods_clocked runs on one GPU");
-  if (!clock) return h->fail(UST_ERR_INVALID_ARGUMENT, "clock: required");
-  return delta_common(h, policy, nullptr, reorder, true, lists, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, true,
-                      out_next_state, out_actions, out_outcome, max_out, out_idx, n_out, out, clock);
+  DeltaCall c(policy, n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev, max_out, out_idx, out_next_state, out_actions,
+              out_outcome, n_out, out);
+  c.reorder = reorder; c.pods = true; c.lists = lists; c.clocked = true; c.clock = clock;
+  return delta_entry(h, "ust_apply_state_delta_pods_clocked", c);
 }
 
 int ust_fetch_outputs_pods(ust_handle* h, uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome) {

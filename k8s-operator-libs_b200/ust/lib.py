@@ -46,29 +46,19 @@ def load():
         lib.ust_apply_state_device.argtypes = apply_args + [C.c_void_p]
         lib.ust_apply_state_packed.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        lib.ust_apply_state_delta.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                              C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        lib.ust_apply_state_delta_sparse.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                                     C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
-                                                     C.c_void_p, C.c_void_p]
-        lib.ust_apply_state_delta_splice.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
-                                                     C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
-                                                     C.c_void_p, C.c_void_p, C.c_void_p]
-        lib.ust_apply_state_delta_reorder.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
-                                                      C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
-                                                      C.c_void_p, C.c_void_p, C.c_void_p]
-        lib.ust_apply_state_delta_pods.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
-                                                   C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
-                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        lib.ust_apply_state_delta_pods_reorder.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
-                                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
-                                                           C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                                           C.c_void_p]
         lib.ust_apply_state_clocked.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p] + apply_args[2:]
-        lib.ust_apply_state_delta_pods_clocked.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
-                                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
-                                                           C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                                           C.c_void_p, C.c_void_p]
+        # the delta calls: handle, policy, the call's structs (order change, pod lists, clock), the changed nodes and the
+        # DaemonSet table, the outputs; the sparse ones end in out_outcome (pod lists only), n_out and the counters
+        vp = C.c_void_p
+        nodes = [C.c_int64, vp, vp, vp, vp, vp, C.c_int32, vp]  # n_changed, idx, state, flags, pod_rev, ds_idx, n_ds, ds_rev
+        sparse = [C.c_int64, vp, vp, vp]  # max_out, out_idx, out_next_state, out_actions
+        lib.ust_apply_state_delta.argtypes = [vp, vp] + nodes + [vp, vp, vp, vp]
+        lib.ust_apply_state_delta_sparse.argtypes = [vp, vp] + nodes + sparse + [vp, vp]
+        lib.ust_apply_state_delta_splice.argtypes = [vp, vp, vp] + nodes + sparse + [vp, vp]
+        lib.ust_apply_state_delta_reorder.argtypes = [vp, vp, vp] + nodes + sparse + [vp, vp]
+        lib.ust_apply_state_delta_pods.argtypes = [vp, vp, vp] + nodes + sparse + [vp, vp, vp]
+        lib.ust_apply_state_delta_pods_reorder.argtypes = [vp, vp, vp, vp] + nodes + sparse + [vp, vp, vp]
+        lib.ust_apply_state_delta_pods_clocked.argtypes = [vp, vp, vp, vp, vp] + nodes + sparse + [vp, vp, vp]
         lib.ust_fetch_outputs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         lib.ust_fetch_outputs_pods.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.ust_simulate_rollout.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
@@ -103,6 +93,78 @@ def _p(a):
     if isinstance(a, np.ndarray):
         return a.ctypes.data
     return int(a)  # raw address (e.g. torch tensor .data_ptr())
+
+
+def _ref(s):
+    """Address of a ctypes struct, or NULL for None."""
+    return C.addressof(s) if s is not None else None
+
+
+# The ABI structs of the delta calls from the dicts the Handle methods take. Each helper returns the struct (None for None)
+# and the arrays it points into, which must stay alive until the call returns.
+_NODE_COLUMNS = (("state", np.uint8), ("flags", np.uint32), ("pod_rev", np.int32), ("ds_idx", np.int32))
+
+
+def _inserted(d):
+    """The inserted nodes' columns of a splice or reorder dict (None for a column it lacks)."""
+    return [np.ascontiguousarray(d[k], dtype=dt) if k in d else None for k, dt in _NODE_COLUMNS]
+
+
+def _splice(splice):
+    """ust_splice of a dict with remove_idx, insert_before and the inserted nodes' columns."""
+    if splice is None:
+        return None, []
+    rm = np.ascontiguousarray(splice.get("remove_idx", np.zeros(0)), dtype=np.int64)
+    ib = np.ascontiguousarray(splice.get("insert_before", np.zeros(0)), dtype=np.int64)
+    ins = _inserted(splice)
+    return abi.Splice(int(rm.shape[0]), _p(rm), int(ib.shape[0]), _p(ib), *[_p(a) for a in ins]), [rm, ib] + ins
+
+
+def _reorder(reorder):
+    """ust_reorder of a dict with run_src, run_len and the inserted nodes' columns (n_insert defaults to their count)."""
+    if reorder is None:
+        return None, []
+    src = np.ascontiguousarray(reorder.get("run_src", np.zeros(0)), dtype=np.int64)
+    ln = np.ascontiguousarray(reorder.get("run_len", np.zeros(0)), dtype=np.int64)
+    ins = _inserted(reorder)
+    n_ins = reorder.get("n_insert", 0 if ins[0] is None else int(ins[0].shape[0]))
+    return abi.Reorder(int(src.shape[0]), _p(src), _p(ln), int(n_ins), *[_p(a) for a in ins]), [src, ln] + ins
+
+
+def _pod_lists(lists):
+    """ust_pod_lists of a dict with node_idx, pod_off and pod_flags."""
+    if lists is None:
+        return None, []
+    ni = np.ascontiguousarray(lists["node_idx"], dtype=np.int64)
+    off = np.ascontiguousarray(lists["pod_off"], dtype=np.int32)
+    pf = np.ascontiguousarray(lists["pod_flags"], dtype=np.uint16)
+    return abi.PodLists(int(ni.shape[0]), _p(ni), _p(off), _p(pf), int(pf.shape[0])), [ni, off, pf]
+
+
+def _clock(now, wait_timeout_seconds, start, insert_start):
+    """ust_clock; a start array that is None is passed as NULL."""
+    keep = [np.ascontiguousarray(a, dtype=np.int64) if a is not None else None for a in (start, insert_start)]
+    return abi.Clock(int(now), int(wait_timeout_seconds), *[_p(a) for a in keep]), keep
+
+
+def _changed_nodes(idx, changed, ds_rev):
+    """The arguments n_changed .. ds_rev of a delta call: the nodes at `idx` with their columns `changed`, and the
+    DaemonSet table."""
+    idx = np.ascontiguousarray(idx, dtype=np.int64)
+    cols = [np.ascontiguousarray(changed[k], dtype=dt) for k, dt in _NODE_COLUMNS]
+    ds_rev = np.ascontiguousarray(ds_rev, dtype=np.int32)
+    return [int(idx.shape[0]), _p(idx)] + [_p(a) for a in cols] + [int(ds_rev.shape[0]), _p(ds_rev)], [idx, ds_rev] + cols
+
+
+def _sparse_outputs(max_out, out, pods):
+    """The arguments max_out .. out (counters) of a sparse delta call, and what the call writes: the output arrays (`out`
+    reused, or max_out + 1 entries each; out_outcome with pod lists only), n_out and the counters."""
+    k = 4 if pods else 3
+    if out is None:
+        out = [np.zeros(max_out + 1, dt) for dt in (np.int64, np.uint8, np.uint16, np.uint8)[:k]]
+    out = tuple(out[:k])
+    n_out, cnt = C.c_int64(0), abi.Counters()
+    return [C.c_int64(int(max_out))] + [_p(a) for a in out] + [C.addressof(n_out), C.addressof(cnt)], (out, n_out, cnt)
 
 
 def pinned_array(shape, dtype):
@@ -240,189 +302,56 @@ class Handle:
     def apply_state_delta(self, policy, n, idx, changed, ds_rev, want_outcome=True, out=None):
         """ust_apply_state_delta: overwrite nodes `idx` of the resident snapshot (n nodes) with `changed`
         (dict of state / flags / pod_rev / ds_idx arrays of len(idx)) and evaluate it again."""
-        idx = np.ascontiguousarray(idx, dtype=np.int64)
-        ch = {"state": np.ascontiguousarray(changed["state"], dtype=np.uint8),
-              "flags": np.ascontiguousarray(changed["flags"], dtype=np.uint32),
-              "pod_rev": np.ascontiguousarray(changed["pod_rev"], dtype=np.int32),
-              "ds_idx": np.ascontiguousarray(changed["ds_idx"], dtype=np.int32)}
-        ds_rev = np.ascontiguousarray(ds_rev, dtype=np.int32)
+        nodes, keep = _changed_nodes(idx, changed, ds_rev)  # `keep`: the arrays `nodes` points into, alive until the call returns
         if out is None:
-            nxt = np.zeros(n, np.uint8)
-            act = np.zeros(n, np.uint16)
-            oc = np.full(n, 0xFF, np.uint8) if want_outcome else None
-        else:
-            nxt, act, oc = out
+            out = (np.zeros(n, np.uint8), np.zeros(n, np.uint16), np.full(n, 0xFF, np.uint8) if want_outcome else None)
+        nxt, act, oc = out
         cnt = abi.Counters()
-        rc = self._lib.ust_apply_state_delta(
-            self._h, C.addressof(policy) if policy is not None else None, int(idx.shape[0]), _p(idx), _p(ch["state"]),
-            _p(ch["flags"]), _p(ch["pod_rev"]), _p(ch["ds_idx"]), int(ds_rev.shape[0]), _p(ds_rev), _p(nxt), _p(act), _p(oc),
-            C.addressof(cnt))
+        rc = self._lib.ust_apply_state_delta(self._h, _ref(policy), *nodes, _p(nxt), _p(act), _p(oc), C.addressof(cnt))
         return rc, nxt, act, oc, cnt.as_dict()
+
+    def _delta_sparse(self, fn, policy, structs, idx, changed, ds_rev, max_out, out, pods=False):
+        """One sparse delta call fn(handle, policy, structs, changed nodes, outputs); `structs`: (ctypes struct or None,
+        arrays behind it) pairs. Returns (rc, n_out, out_idx, out_next, out_actions[, out_outcome], counters-dict)."""
+        nodes, keep = _changed_nodes(idx, changed, ds_rev)  # `keep`: the arrays `nodes` points into, alive until the call returns
+        outputs, (out, n_out, cnt) = _sparse_outputs(max_out, out, pods)
+        rc = fn(self._h, _ref(policy), *[_ref(s) for s, _ in structs], *nodes, *outputs)
+        return (rc, int(n_out.value)) + out + (cnt.as_dict(),)
 
     def apply_state_delta_sparse(self, policy, idx, changed, ds_rev, max_out, out=None):
         """ust_apply_state_delta_sparse: like apply_state_delta, but only the outputs that differ from the previous call's
         come back. Returns (rc, n_out, out_idx, out_next, out_actions, counters-dict); the arrays hold n_out entries
         when n_out <= max_out."""
-        idx = np.ascontiguousarray(idx, dtype=np.int64)
-        ch = {"state": np.ascontiguousarray(changed["state"], dtype=np.uint8),
-              "flags": np.ascontiguousarray(changed["flags"], dtype=np.uint32),
-              "pod_rev": np.ascontiguousarray(changed["pod_rev"], dtype=np.int32),
-              "ds_idx": np.ascontiguousarray(changed["ds_idx"], dtype=np.int32)}
-        ds_rev = np.ascontiguousarray(ds_rev, dtype=np.int32)
-        if out is None:
-            out = (np.zeros(max_out + 1, np.int64), np.zeros(max_out + 1, np.uint8), np.zeros(max_out + 1, np.uint16))
-        n_out = C.c_int64(0)
-        cnt = abi.Counters()
-        rc = self._lib.ust_apply_state_delta_sparse(
-            self._h, C.addressof(policy) if policy is not None else None, int(idx.shape[0]), _p(idx), _p(ch["state"]),
-            _p(ch["flags"]), _p(ch["pod_rev"]), _p(ch["ds_idx"]), int(ds_rev.shape[0]), _p(ds_rev), C.c_int64(int(max_out)),
-            _p(out[0]), _p(out[1]), _p(out[2]), C.addressof(n_out), C.addressof(cnt))
-        return rc, int(n_out.value), out[0], out[1], out[2], cnt.as_dict()
+        return self._delta_sparse(self._lib.ust_apply_state_delta_sparse, policy, [], idx, changed, ds_rev, max_out, out)
 
     def apply_state_delta_splice(self, policy, splice, idx, changed, ds_rev, max_out, out=None):
         """ust_apply_state_delta_splice: apply_state_delta_sparse after a membership change of the resident snapshot.
         `splice` is None or a dict with remove_idx, insert_before and the inserted nodes' state / flags / pod_rev / ds_idx;
         `idx` indexes the spliced snapshot. Returns what apply_state_delta_sparse returns, in new-index order."""
-        keep = []
-
-        def arr(a, dt):
-            a = np.ascontiguousarray(a, dtype=dt)
-            keep.append(a)
-            return a
-
-        sp = None
-        if splice is not None:
-            rm = arr(splice.get("remove_idx", np.zeros(0)), np.int64)
-            ib = arr(splice.get("insert_before", np.zeros(0)), np.int64)
-            ins = {k: arr(splice[k], dt) if k in splice else None
-                   for k, dt in (("state", np.uint8), ("flags", np.uint32), ("pod_rev", np.int32), ("ds_idx", np.int32))}
-            sp = abi.Splice(int(rm.shape[0]), _p(rm), int(ib.shape[0]), _p(ib), _p(ins["state"]), _p(ins["flags"]),
-                            _p(ins["pod_rev"]), _p(ins["ds_idx"]))
-        idx = arr(idx, np.int64)
-        ch = {"state": arr(changed["state"], np.uint8), "flags": arr(changed["flags"], np.uint32),
-              "pod_rev": arr(changed["pod_rev"], np.int32), "ds_idx": arr(changed["ds_idx"], np.int32)}
-        ds_rev = arr(ds_rev, np.int32)
-        if out is None:
-            out = (np.zeros(max_out + 1, np.int64), np.zeros(max_out + 1, np.uint8), np.zeros(max_out + 1, np.uint16))
-        n_out = C.c_int64(0)
-        cnt = abi.Counters()
-        rc = self._lib.ust_apply_state_delta_splice(
-            self._h, C.addressof(policy) if policy is not None else None, C.addressof(sp) if sp is not None else None,
-            int(idx.shape[0]), _p(idx), _p(ch["state"]), _p(ch["flags"]), _p(ch["pod_rev"]), _p(ch["ds_idx"]),
-            int(ds_rev.shape[0]), _p(ds_rev), C.c_int64(int(max_out)), _p(out[0]), _p(out[1]), _p(out[2]), C.addressof(n_out),
-            C.addressof(cnt))
-        return rc, int(n_out.value), out[0], out[1], out[2], cnt.as_dict()
+        return self._delta_sparse(self._lib.ust_apply_state_delta_splice, policy, [_splice(splice)], idx, changed, ds_rev,
+                                  max_out, out)
 
     def apply_state_delta_reorder(self, policy, reorder, idx, changed, ds_rev, max_out, out=None):
         """ust_apply_state_delta_reorder: apply_state_delta_sparse after the resident snapshot took a new node order.
         `reorder` is None or a dict with run_src, run_len and the inserted nodes' state / flags / pod_rev / ds_idx;
         `idx` indexes the reordered snapshot. Returns what apply_state_delta_sparse returns, in new-index order."""
-        keep = []
-
-        def arr(a, dt):
-            a = np.ascontiguousarray(a, dtype=dt)
-            keep.append(a)
-            return a
-
-        ro = None
-        if reorder is not None:
-            src = arr(reorder.get("run_src", np.zeros(0)), np.int64)
-            ln = arr(reorder.get("run_len", np.zeros(0)), np.int64)
-            ins = {k: arr(reorder[k], dt) if k in reorder else None
-                   for k, dt in (("state", np.uint8), ("flags", np.uint32), ("pod_rev", np.int32), ("ds_idx", np.int32))}
-            n_ins = reorder.get("n_insert", 0 if ins["state"] is None else int(ins["state"].shape[0]))
-            ro = abi.Reorder(int(src.shape[0]), _p(src), _p(ln), int(n_ins), _p(ins["state"]), _p(ins["flags"]),
-                             _p(ins["pod_rev"]), _p(ins["ds_idx"]))
-        idx = arr(idx, np.int64)
-        ch = {"state": arr(changed["state"], np.uint8), "flags": arr(changed["flags"], np.uint32),
-              "pod_rev": arr(changed["pod_rev"], np.int32), "ds_idx": arr(changed["ds_idx"], np.int32)}
-        ds_rev = arr(ds_rev, np.int32)
-        if out is None:
-            out = (np.zeros(max_out + 1, np.int64), np.zeros(max_out + 1, np.uint8), np.zeros(max_out + 1, np.uint16))
-        n_out = C.c_int64(0)
-        cnt = abi.Counters()
-        rc = self._lib.ust_apply_state_delta_reorder(
-            self._h, C.addressof(policy) if policy is not None else None, C.addressof(ro) if ro is not None else None,
-            int(idx.shape[0]), _p(idx), _p(ch["state"]), _p(ch["flags"]), _p(ch["pod_rev"]), _p(ch["ds_idx"]),
-            int(ds_rev.shape[0]), _p(ds_rev), C.c_int64(int(max_out)), _p(out[0]), _p(out[1]), _p(out[2]), C.addressof(n_out),
-            C.addressof(cnt))
-        return rc, int(n_out.value), out[0], out[1], out[2], cnt.as_dict()
+        return self._delta_sparse(self._lib.ust_apply_state_delta_reorder, policy, [_reorder(reorder)], idx, changed, ds_rev,
+                                  max_out, out)
 
     def apply_state_delta_pods(self, policy, lists, idx, changed, ds_rev, max_out, out=None):
         """ust_apply_state_delta_pods: apply_state_delta_sparse on the resident pod-list snapshot after replacing the pod lists
         of some nodes. `lists` is None or a dict with node_idx, pod_off and pod_flags. Returns (rc, n_out, out_idx, out_next,
         out_actions, out_outcome, counters-dict); the arrays hold n_out entries when n_out <= max_out."""
-        keep = []
-
-        def arr(a, dt):
-            a = np.ascontiguousarray(a, dtype=dt)
-            keep.append(a)
-            return a
-
-        pl = None
-        if lists is not None:
-            ni = arr(lists["node_idx"], np.int64)
-            off = arr(lists["pod_off"], np.int32)
-            pf = arr(lists["pod_flags"], np.uint16)
-            pl = abi.PodLists(int(ni.shape[0]), _p(ni), _p(off), _p(pf), int(pf.shape[0]))
-        idx = arr(idx, np.int64)
-        ch = {"state": arr(changed["state"], np.uint8), "flags": arr(changed["flags"], np.uint32),
-              "pod_rev": arr(changed["pod_rev"], np.int32), "ds_idx": arr(changed["ds_idx"], np.int32)}
-        ds_rev = arr(ds_rev, np.int32)
-        if out is None:
-            out = (np.zeros(max_out + 1, np.int64), np.zeros(max_out + 1, np.uint8), np.zeros(max_out + 1, np.uint16),
-                   np.zeros(max_out + 1, np.uint8))
-        n_out = C.c_int64(0)
-        cnt = abi.Counters()
-        rc = self._lib.ust_apply_state_delta_pods(
-            self._h, C.addressof(policy) if policy is not None else None, C.addressof(pl) if pl is not None else None,
-            int(idx.shape[0]), _p(idx), _p(ch["state"]), _p(ch["flags"]), _p(ch["pod_rev"]), _p(ch["ds_idx"]),
-            int(ds_rev.shape[0]), _p(ds_rev), C.c_int64(int(max_out)), _p(out[0]), _p(out[1]), _p(out[2]), _p(out[3]),
-            C.addressof(n_out), C.addressof(cnt))
-        return rc, int(n_out.value), out[0], out[1], out[2], out[3], cnt.as_dict()
+        return self._delta_sparse(self._lib.ust_apply_state_delta_pods, policy, [_pod_lists(lists)], idx, changed, ds_rev,
+                                  max_out, out, pods=True)
 
     def apply_state_delta_pods_reorder(self, policy, reorder, lists, idx, changed, ds_rev, max_out, out=None):
         """ust_apply_state_delta_pods_reorder: apply_state_delta_pods after the resident pod-list snapshot took a new node
         order. `reorder` is None or a dict as for apply_state_delta_reorder, `lists` None or a dict as for
         apply_state_delta_pods; lists["node_idx"] and `idx` index the reordered snapshot, and every inserted node needs a
         list. Returns what apply_state_delta_pods returns, in new-index order."""
-        keep = []
-
-        def arr(a, dt):
-            a = np.ascontiguousarray(a, dtype=dt)
-            keep.append(a)
-            return a
-
-        ro = None
-        if reorder is not None:
-            src = arr(reorder.get("run_src", np.zeros(0)), np.int64)
-            ln = arr(reorder.get("run_len", np.zeros(0)), np.int64)
-            ins = {k: arr(reorder[k], dt) if k in reorder else None
-                   for k, dt in (("state", np.uint8), ("flags", np.uint32), ("pod_rev", np.int32), ("ds_idx", np.int32))}
-            n_ins = reorder.get("n_insert", 0 if ins["state"] is None else int(ins["state"].shape[0]))
-            ro = abi.Reorder(int(src.shape[0]), _p(src), _p(ln), int(n_ins), _p(ins["state"]), _p(ins["flags"]),
-                             _p(ins["pod_rev"]), _p(ins["ds_idx"]))
-        pl = None
-        if lists is not None:
-            ni = arr(lists["node_idx"], np.int64)
-            off = arr(lists["pod_off"], np.int32)
-            pf = arr(lists["pod_flags"], np.uint16)
-            pl = abi.PodLists(int(ni.shape[0]), _p(ni), _p(off), _p(pf), int(pf.shape[0]))
-        idx = arr(idx, np.int64)
-        ch = {"state": arr(changed["state"], np.uint8), "flags": arr(changed["flags"], np.uint32),
-              "pod_rev": arr(changed["pod_rev"], np.int32), "ds_idx": arr(changed["ds_idx"], np.int32)}
-        ds_rev = arr(ds_rev, np.int32)
-        if out is None:
-            out = (np.zeros(max_out + 1, np.int64), np.zeros(max_out + 1, np.uint8), np.zeros(max_out + 1, np.uint16),
-                   np.zeros(max_out + 1, np.uint8))
-        n_out = C.c_int64(0)
-        cnt = abi.Counters()
-        rc = self._lib.ust_apply_state_delta_pods_reorder(
-            self._h, C.addressof(policy) if policy is not None else None, C.addressof(ro) if ro is not None else None,
-            C.addressof(pl) if pl is not None else None, int(idx.shape[0]), _p(idx), _p(ch["state"]), _p(ch["flags"]),
-            _p(ch["pod_rev"]), _p(ch["ds_idx"]), int(ds_rev.shape[0]), _p(ds_rev), C.c_int64(int(max_out)), _p(out[0]),
-            _p(out[1]), _p(out[2]), _p(out[3]), C.addressof(n_out), C.addressof(cnt))
-        return rc, int(n_out.value), out[0], out[1], out[2], out[3], cnt.as_dict()
+        return self._delta_sparse(self._lib.ust_apply_state_delta_pods_reorder, policy, [_reorder(reorder), _pod_lists(lists)],
+                                  idx, changed, ds_rev, max_out, out, pods=True)
 
     def apply_state_clocked(self, policy, now, wait_timeout_seconds, start, soa, pods, out=None, clock_start=True):
         """ust_apply_state_clocked: apply_state with pod lists, the two timeouts derived on the device from `now` and the
@@ -430,8 +359,8 @@ class Handle:
         clock. Returns (rc, next_state, actions, outcome, counters-dict)."""
         n = int(soa["state"].shape[0])
         nxt, act, oc = out if out is not None else (np.zeros(n, np.uint8), np.zeros(n, np.uint16), np.full(n, 0xFF, np.uint8))
-        st = np.ascontiguousarray(start, dtype=np.int64) if start is not None else None
-        ck = abi.Clock(int(now), int(wait_timeout_seconds), _p(st) if clock_start else None, None) if now is not None else None
+        # `keep`: the start array `ck` points into, alive until the call returns
+        ck, keep = _clock(now, wait_timeout_seconds, start if clock_start else None, None) if now is not None else (None, [])
         ps = None
         if pods is not None:
             off = np.ascontiguousarray(pods["pod_off"], dtype=np.int32)
@@ -439,7 +368,7 @@ class Handle:
             ps = abi.Pods(off.ctypes.data, pf.ctypes.data, int(pf.shape[0]))
         cnt = abi.Counters()
         rc = self._lib.ust_apply_state_clocked(
-            self._h, C.addressof(policy) if policy is not None else None, C.addressof(ck) if ck is not None else None, n,
+            self._h, _ref(policy), _ref(ck), n,
             _p(soa["state"]), _p(soa["flags"]), _p(soa["pod_rev"]), _p(soa["ds_idx"]), int(soa["ds_rev"].shape[0]),
             _p(soa["ds_rev"]), C.addressof(ps) if ps is not None else None, _p(nxt), _p(act), _p(oc), C.addressof(cnt))
         return rc, nxt, act, oc, cnt.as_dict()
@@ -449,46 +378,9 @@ class Handle:
         """ust_apply_state_delta_pods_clocked: apply_state_delta_pods_reorder on a clocked snapshot. `start` holds the start
         times of the nodes at `idx`, `insert_start` those of the reorder's inserted nodes (None: NULL); clock=False passes a
         NULL clock. Returns what apply_state_delta_pods returns."""
-        keep = []
-
-        def arr(a, dt):
-            a = np.ascontiguousarray(a, dtype=dt)
-            keep.append(a)
-            return a
-
-        ro = None
-        if reorder is not None:
-            src = arr(reorder.get("run_src", np.zeros(0)), np.int64)
-            ln = arr(reorder.get("run_len", np.zeros(0)), np.int64)
-            ins = {k: arr(reorder[k], dt) if k in reorder else None
-                   for k, dt in (("state", np.uint8), ("flags", np.uint32), ("pod_rev", np.int32), ("ds_idx", np.int32))}
-            n_ins = reorder.get("n_insert", 0 if ins["state"] is None else int(ins["state"].shape[0]))
-            ro = abi.Reorder(int(src.shape[0]), _p(src), _p(ln), int(n_ins), _p(ins["state"]), _p(ins["flags"]),
-                             _p(ins["pod_rev"]), _p(ins["ds_idx"]))
-        pl = None
-        if lists is not None:
-            ni = arr(lists["node_idx"], np.int64)
-            off = arr(lists["pod_off"], np.int32)
-            pf = arr(lists["pod_flags"], np.uint16)
-            pl = abi.PodLists(int(ni.shape[0]), _p(ni), _p(off), _p(pf), int(pf.shape[0]))
-        idx = arr(idx, np.int64)
-        ch = {"state": arr(changed["state"], np.uint8), "flags": arr(changed["flags"], np.uint32),
-              "pod_rev": arr(changed["pod_rev"], np.int32), "ds_idx": arr(changed["ds_idx"], np.int32)}
-        st = arr(start, np.int64) if start is not None else None
-        ist = arr(insert_start, np.int64) if insert_start is not None else None
-        ck = abi.Clock(int(now), int(wait_timeout_seconds), _p(st), _p(ist)) if clock else None
-        ds_rev = arr(ds_rev, np.int32)
-        if out is None:
-            out = (np.zeros(max_out + 1, np.int64), np.zeros(max_out + 1, np.uint8), np.zeros(max_out + 1, np.uint16),
-                   np.zeros(max_out + 1, np.uint8))
-        n_out = C.c_int64(0)
-        cnt = abi.Counters()
-        rc = self._lib.ust_apply_state_delta_pods_clocked(
-            self._h, C.addressof(policy) if policy is not None else None, C.addressof(ck) if ck is not None else None,
-            C.addressof(ro) if ro is not None else None, C.addressof(pl) if pl is not None else None, int(idx.shape[0]), _p(idx),
-            _p(ch["state"]), _p(ch["flags"]), _p(ch["pod_rev"]), _p(ch["ds_idx"]), int(ds_rev.shape[0]), _p(ds_rev),
-            C.c_int64(int(max_out)), _p(out[0]), _p(out[1]), _p(out[2]), _p(out[3]), C.addressof(n_out), C.addressof(cnt))
-        return rc, int(n_out.value), out[0], out[1], out[2], out[3], cnt.as_dict()
+        ck = _clock(now, wait_timeout_seconds, start, insert_start) if clock else (None, [])
+        return self._delta_sparse(self._lib.ust_apply_state_delta_pods_clocked, policy, [ck, _reorder(reorder), _pod_lists(lists)],
+                                  idx, changed, ds_rev, max_out, out, pods=True)
 
     def fetch_outputs_pods(self, n):
         """ust_fetch_outputs_pods: (rc, next_state, actions, actuator_outcome) of the last call on the pod-list snapshot."""
