@@ -535,28 +535,53 @@ static uint16_t validationPodFlags(const Pod& p) {
   return (uint16_t)(UST_POD_MATCH_VALIDATION_SELECTOR | (ready ? UST_POD_READY : 0));
 }
 
-// The one List of a ValidateOnDevice reconcile, grouped by node. The reference lists per node, with the selector and the
-// field selector spec.nodeName=<node> (validation_manager.go:77-79); this takes one cluster-wide List and keeps its
-// order within each node. That rests on one assumption: the API server returns a node's pods in the same relative order
-// in both Lists (it sorts a List by namespace and name). Validate's answer depends on that order: a ready pod listed
-// before a not-ready one resets the start time (INTEGRATION.md, "Encoding the validation pods").
+// A wait-selector pod as ScheduleCheckOnPodCompletion sees it (pod_manager.go:263, :371-391): it matched the selector,
+// and only its phase matters; a phase IsPodRunningOrPending does not name counts as not running.
+static uint16_t waitPodFlags(const Pod& p) {
+  const unsigned phase = p.Phase == "Running" ? UST_PHASE_RUNNING : p.Phase == "Pending" ? UST_PHASE_PENDING
+                         : p.Phase == "Succeeded" ? UST_PHASE_SUCCEEDED : p.Phase == "Failed" ? UST_PHASE_FAILED : UST_PHASE_OTHER;
+  return (uint16_t)(UST_POD_MATCH_WAIT_SELECTOR | phase);
+}
+// "any wait pod Running or Pending" (pod_manager.go:278-284) over a node's list as handed to the device
+static bool anyWaitRunning(const uint16_t* b, const uint16_t* e) {
+  for (; b != e; b++) {
+    const unsigned phase = *b & UST_POD_PHASE_MASK;
+    if ((*b & UST_POD_MATCH_WAIT_SELECTOR) && (phase == UST_PHASE_RUNNING || phase == UST_PHASE_PENDING)) return true;
+  }
+  return false;
+}
+
+// The one List per selector of a ValidateOnDevice / WaitForCompletionOnDevice reconcile, grouped by node. The reference
+// lists per node, with the selector and the field selector spec.nodeName=<node> (validation_manager.go:77-79,
+// pod_manager.go:320-329); this takes one cluster-wide List and keeps its order within each node. That rests on one
+// assumption: the API server returns a node's pods in the same relative order in both Lists (it sorts a List by
+// namespace and name). Validate's answer depends on that order: a ready pod listed before a not-ready one resets the
+// start time (INTEGRATION.md, "Encoding the validation pods"); the wait-for-completion check does not ("any pod Running
+// or Pending").
 using PodsByNode = std::unordered_map<std::string, std::vector<const Pod*>>;
-static Error listValidationPods(K8sClient* client, const std::string& selector, PodsByNode* byNode) {
-  if (client == nullptr) return Errorf("no K8sClient to list the validation pods with");
+static Error listPodsBySelector(K8sClient* client, const std::string& selector, const char* what, PodsByNode* byNode) {
+  if (client == nullptr) return Errorf(std::string("no K8sClient to list the ") + what + " pods with");
   std::vector<Pod*> pods;
   if (Error e = client->ListPodsBySelector(selector, "", &pods)) return e;
   for (const Pod* p : pods)
     if (!p->NodeName.empty()) (*byNode)[p->NodeName].push_back(p);
   return std::nullopt;
 }
+// A node's pods in one List, in the List's order; nullptr: none.
+static const std::vector<const Pod*>* podsOf(const PodsByNode& byNode, const std::string& node) {
+  auto it = byNode.find(node);
+  return it == byNode.end() ? nullptr : &it->second;
+}
 
 // One snapshot entry -> its four SoA values. `ds` / `dsErr`: index of its DaemonSet in the table (-1 = orphaned) and
 // whether that DaemonSet's revision-hash lookup failed; `deferred` receives an error the reference would raise when
-// its pass reaches the node; `validationStart` (ValidateOnDevice only, else nullptr) the parsed validation start time.
+// its pass reaches the node; `start` (the clocked calls only, else nullptr) the node's start time: the parsed validation
+// start time with `validation` (ValidateOnDevice), replaced on a wait-for-jobs-required node by the parsed wait start
+// time with `wait` (WaitForCompletionOnDevice), 0 otherwise. The device reads it only in those two states.
 Error ClusterUpgradeStateManagerImpl::encodeOne(const NodeUpgradeState* ns, int code, int32_t ds, bool dsErr,
                                                 std::map<std::string, int32_t>* intern, const std::vector<int32_t>& ds_rev,
                                                 uint8_t* hot_out, uint32_t* flags_out, int32_t* rev_out, std::string* deferred,
-                                                int64_t* validationStart) {
+                                                int64_t* start, bool validation, bool wait) {
   auto internHash = [&](const std::string& h) {  // find first: emplace would build (and throw away) a map node per node
     auto it = intern->find(h);
     return it != intern->end() ? it->second : intern->emplace(h, (int32_t)intern->size() + 1).first->second;
@@ -615,19 +640,30 @@ Error ClusterUpgradeStateManagerImpl::encodeOne(const NodeUpgradeState* ns, int 
     f |= UST_F_NM_PRESENT;
     if (ns->NodeMaintenance->ReadyConditionWithReasonReady) f |= UST_F_NM_READY;
   }
-  if (validationStart) {  // StateOptions::ValidateOnDevice: the start-time annotation handleTimeout reads (validation_manager.go:142-160)
-    *validationStart = 0;
+  if (start) *start = 0;
+  if (start && validation) {  // StateOptions::ValidateOnDevice: the start-time annotation handleTimeout reads (validation_manager.go:142-160)
     auto it = n.Annotations.find(keys().validationStart);
     if (it != n.Annotations.end()) {
       f |= UST_F_VALIDATION_START_ANNO;
       std::string err;
-      if (!parseInt64(it->second, validationStart, &err)) {
+      if (!parseInt64(it->second, start, &err)) {
         f |= UST_F_VALIDATION_START_INVALID;
-        *validationStart = 0;
+        *start = 0;
         // Validate's error when it reaches the node (:97-101); the device returns UST_ERR_VALIDATION there
         if (code == UST_STATE_VALIDATION_REQUIRED) *deferred = "unable to handle timeout for validation state: " + err;
       }
     }
+  }
+  if (start && wait) {  // StateOptions::WaitForCompletionOnDevice: the start-time annotation HandleTimeoutOnPodCompletions
+                        // reads (pod_manager.go:336-353); a value that does not parse is an error the check swallows
+    auto it = n.Annotations.find(keys().waitStart);
+    int64_t v = 0;
+    if (it != n.Annotations.end()) {
+      f |= UST_F_WAIT_START_ANNO;
+      std::string err;
+      if (!parseInt64(it->second, &v, &err)) { f |= UST_F_WAIT_START_INVALID; v = 0; }
+    }
+    if (code == UST_STATE_WAIT_FOR_JOBS_REQUIRED) *start = v;
   }
   *hot_out = hot;
   *flags_out = f;
@@ -682,7 +718,9 @@ Error ClusterUpgradeStateManagerImpl::Encode(const ClusterUpgradeState& s, const
   e.flags.assign(n, 0);
   e.pod_rev.assign(n, 0);
   e.validateOnDevice = validateOnDevice();
-  if (e.validateOnDevice) e.start.assign(n, 0);
+  e.waitOnDevice = waitOnDevice(policy);
+  const bool clocked = e.validateOnDevice || e.waitOnDevice;
+  if (clocked) e.start.assign(n, 0);
   const int32_t base = (int32_t)intern.size();
   const size_t workers = (size_t)std::max(1, std::min(opts_.EncodeThreads, (int)(n / 4096 + 1)));
   struct Part { std::map<std::string, int32_t> intern; std::vector<std::pair<size_t, std::string>> deferred; Error err; size_t errAt = 0; };
@@ -695,7 +733,7 @@ Error ClusterUpgradeStateManagerImpl::Encode(const ClusterUpgradeState& s, const
       const int32_t ds = e.ds_idx[i];
       uint8_t hot; uint32_t f; int32_t rev; std::string deferred;
       if (Error err = encodeOne(e.entries[i], codes[i], ds, ds >= 0 && dsHashError[(size_t)ds], &p.intern, e.ds_rev, &hot, &f, &rev, &deferred,
-                                e.validateOnDevice ? &e.start[i] : nullptr)) {
+                                clocked ? &e.start[i] : nullptr, e.validateOnDevice, e.waitOnDevice)) {
         p.err = err; p.errAt = i;
         return;
       }
@@ -731,17 +769,27 @@ Error ClusterUpgradeStateManagerImpl::Encode(const ClusterUpgradeState& s, const
         if (e.pod_rev[i] > base) e.pod_rev[i] = remap[(size_t)e.pod_rev[i]];
     }
   }
-  // 4. ValidateOnDevice: every entry's validation pods (an empty list when it has none), from one List
-  if (e.validateOnDevice) {
-    e.policy.evaluate_actuators = UST_EVAL_ACTUATORS | UST_EVAL_VALIDATION;
+  // 4. ValidateOnDevice / WaitForCompletionOnDevice: every entry's list (an empty one when it has no pod), from one List
+  //    per selector: its validation pods, then its wait-selector pods. A pod both selectors match is in the list twice,
+  //    each entry with its own selector bit: each pass reads only its own bit.
+  if (clocked) {
+    e.policy.evaluate_actuators = UST_EVAL_ACTUATORS | (e.validateOnDevice ? UST_EVAL_VALIDATION : 0);
     e.now = opts_.Now();
-    PodsByNode byNode;
-    e.listError = listValidationPods(K8sClient, validationSelector_, &byNode);
+    PodsByNode vpods, wpods;
+    if (e.validateOnDevice) e.listError = listPodsBySelector(K8sClient, validationSelector_, "validation", &vpods);
+    if (e.waitOnDevice) {
+      e.waitListError = listPodsBySelector(K8sClient, policy.WaitForCompletion->PodSelector, "wait-for-completion", &wpods);
+      e.waitRunning.assign(n, 0);
+    }
     e.pod_off.assign(n + 1, 0);
     for (size_t i = 0; i < n; i++) {
-      auto it = e.listError ? byNode.end() : byNode.find(e.entries[i]->Node->Name);
-      if (it != byNode.end())
-        for (const Pod* p : it->second) e.pod_flags.push_back(validationPodFlags(*p));
+      const std::string& name = e.entries[i]->Node->Name;
+      if (const auto* v = e.listError ? nullptr : podsOf(vpods, name))
+        for (const Pod* p : *v) e.pod_flags.push_back(validationPodFlags(*p));
+      const size_t w0 = e.pod_flags.size();
+      if (const auto* w = e.waitListError ? nullptr : podsOf(wpods, name))
+        for (const Pod* p : *w) e.pod_flags.push_back(waitPodFlags(*p));
+      if (e.waitOnDevice) e.waitRunning[i] = anyWaitRunning(e.pod_flags.data() + w0, e.pod_flags.data() + e.pod_flags.size());
       e.pod_off[i + 1] = (int32_t)e.pod_flags.size();
     }
   }
@@ -750,7 +798,7 @@ Error ClusterUpgradeStateManagerImpl::Encode(const ClusterUpgradeState& s, const
 
 Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const DriverUpgradePolicySpec& policy,
                                              const uint8_t* next_state, const uint16_t* actions, int abi_rc,
-                                             const ust_counters& counters) {
+                                             const ust_counters& counters, const uint8_t* actuator_outcome) {
   const size_t n = enc.entries.size();
   const bool drainEnabled = policy.DrainSpec && policy.DrainSpec->Enable;
   const bool waitSelector = policy.WaitForCompletion && !policy.WaitForCompletion->PodSelector.empty();
@@ -827,7 +875,32 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
     const bool cut = abi_rc != UST_OK && counters.error_pass == pass;  // the kernel stopped inside this pass
     switch (code) {
       case UST_STATE_WAIT_FOR_JOBS_REQUIRED:
-        if (waitSelector && !batchNodes.empty()) {  // common_manager.go:404-418
+        if (enc.waitOnDevice && i > begin) {
+          // the calls ScheduleCheckOnPodCompletion makes (pod_manager.go:256-317), as the device answered it. Its per-node
+          // List came first: a failed one returns before any node's check has started.
+          if (enc.waitListError) return enc.waitListError;
+          if (actuator_outcome == nullptr) return Errorf("Replay: the wait-for-jobs pass on the device needs actuator_outcome");
+          const std::string& key = GetWaitForPodCompletionStartTimeAnnotationKey();
+          for (size_t k = begin; k < i; k++) {
+            if (!(actions[k] & UST_A_SCHEDULE_WAIT_CHECK)) continue;
+            // The reference checks each node in a goroutine that took the node by value (go func(node corev1.Node), :275):
+            // its calls get a copy, so that they do not write to the caller's snapshot object. Every error is logged as an
+            // event and dropped there (:290-312).
+            Node node = *enc.entries[k]->Node;
+            if (actuator_outcome[k] == UST_STATE_POD_DELETION_REQUIRED) {
+              if (!enc.waitRunning[k]) {  // no wait pod Running or Pending: delete the start time, then the state (:300-309)
+                if (!NodeUpgradeStateProvider->ChangeNodeUpgradeAnnotation(&node, key, kNullString))
+                  (void)NodeUpgradeStateProvider->ChangeNodeUpgradeState(&node, UpgradeStatePodDeletionRequired);
+              } else {  // still running, timed out: the state, then the start time (HandleTimeoutOnPodCompletions :354-365)
+                (void)NodeUpgradeStateProvider->ChangeNodeUpgradeState(&node, UpgradeStatePodDeletionRequired);
+                (void)NodeUpgradeStateProvider->ChangeNodeUpgradeAnnotation(&node, key, kNullString);
+              }
+            } else if (actions[k] & UST_A_SET_WAIT_START) {  // running, no start time yet (:336-345)
+              (void)NodeUpgradeStateProvider->ChangeNodeUpgradeAnnotation(&node, key, std::to_string(enc.now));
+            }
+            // otherwise still waiting, or the start time does not parse (:348-353), or no timeout: no call
+          }
+        } else if (waitSelector && !batchNodes.empty()) {  // common_manager.go:404-418
           PodManagerConfig cfg;
           cfg.WaitForCompletionSpec = &*policy.WaitForCompletion;
           cfg.Nodes = batchNodes;
@@ -892,8 +965,9 @@ Error ClusterUpgradeStateManagerImpl::ApplyState(ClusterUpgradeState* currentSta
   enc.state.push_back(0); enc.flags.push_back(0); enc.pod_rev.push_back(0); enc.ds_idx.push_back(0);  // never pass NULL for n == 0
   enc.ds_rev.push_back(0);
   int rc;
-  if (enc.validateOnDevice) {  // Validate on the device: the validation pods, the start times and `now` go with the call
-    std::vector<uint8_t> outcome(n + 1);
+  std::vector<uint8_t> outcome(n + 1, UST_OUTCOME_NONE);
+  if (enc.validateOnDevice || enc.waitOnDevice) {  // Validate / the wait check on the device: the pods, the start times and
+                                                   // `now` go with the call
     enc.pod_flags.push_back(0); enc.start.push_back(0);
     const ust_pods pods = {enc.pod_off.data(), enc.pod_flags.data(), (int64_t)enc.pod_flags.size() - 1};
     const ust_clock clock = {enc.now, upgradePolicy->WaitForCompletion ? upgradePolicy->WaitForCompletion->TimeoutSecond : 0, enc.start.data(), nullptr};
@@ -905,7 +979,7 @@ Error ClusterUpgradeStateManagerImpl::ApplyState(ClusterUpgradeState* currentSta
                          (int32_t)enc.ds_rev.size() - 1, enc.ds_rev.data(), nullptr, next.data(), actions.data(), nullptr, &last_);
   }
   if (rc == UST_ERR_CUDA || rc == UST_ERR_INVALID_ARGUMENT || rc == UST_ERR_NIL_STATE) return Errorf(ust_last_error(handle_));
-  return Replay(enc, *upgradePolicy, next.data(), actions.data(), rc, last_);
+  return Replay(enc, *upgradePolicy, next.data(), actions.data(), rc, last_, outcome.data());
 }
 
 // ---- incremental ApplyState: the resourceVersion-keyed encode cache (upgrade.hpp) --------------------------------------
@@ -998,10 +1072,10 @@ int ClusterUpgradeStateManagerImpl::EvaluateCachedPods(const ust_policy& policy,
     }
     pf.push_back(0);
   };
-  std::vector<uint8_t> outcome(n + 1);
   if (full) {
     k.next.assign(n + 1, 0);
     k.actions.assign(n + 1, 0);
+    k.outcome.assign(n + 1, UST_OUTCOME_NONE);
     std::vector<uint8_t> st = k.state; st.push_back(0);
     std::vector<uint32_t> fl = k.flags; fl.push_back(0);
     std::vector<int32_t> rv = k.pod_rev; rv.push_back(0);
@@ -1011,7 +1085,7 @@ int ClusterUpgradeStateManagerImpl::EvaluateCachedPods(const ust_policy& policy,
     const ust_pods pods = {off.data(), pf.data(), (int64_t)pf.size() - 1};
     const ust_clock clock = {now, waitTimeout, sv.data(), nullptr};
     return ust_apply_state_clocked(handle_, &policy, &clock, (int64_t)n, st.data(), fl.data(), rv.data(), di.data(), (int32_t)k.ds_rev.size(),
-                                   dsrev.data(), &pods, k.next.data(), k.actions.data(), outcome.data(), c);
+                                   dsrev.data(), &pods, k.next.data(), k.actions.data(), k.outcome.data(), c);
   }
   const size_t m = changed.size();
   std::vector<uint8_t> st(m + 1);
@@ -1055,11 +1129,15 @@ int ClusterUpgradeStateManagerImpl::EvaluateCachedPods(const ust_policy& policy,
     stats_.outputs_received += (int64_t)n;
     k.next.resize(n + 1);
     k.actions.resize(n + 1);
-    const int frc = ust_fetch_outputs_pods(handle_, k.next.data(), k.actions.data(), outcome.data());
+    k.outcome.resize(n + 1, UST_OUTCOME_NONE);
+    const int frc = ust_fetch_outputs_pods(handle_, k.next.data(), k.actions.data(), k.outcome.data());
     if (frc != UST_OK) return frc;
     return rc == UST_ERR_TRUNCATED ? UST_OK : rc;
   }
-  for (int64_t j = 0; j < n_out; j++) { k.next[(size_t)oi[(size_t)j]] = on[(size_t)j]; k.actions[(size_t)oi[(size_t)j]] = oa[(size_t)j]; }
+  for (int64_t j = 0; j < n_out; j++) {
+    const size_t i = (size_t)oi[(size_t)j];
+    k.next[i] = on[(size_t)j]; k.actions[i] = oa[(size_t)j]; k.outcome[i] = oo[(size_t)j];
+  }
   stats_.outputs_received += n_out;
   return rc;
 }
@@ -1071,17 +1149,19 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
   flatten_policy(*upgradePolicy, podDeletionStateEnabled_, validationStateEnabled_, opts_.Requestor.UseMaintenanceOperator, &pol);
   Cache& k = cache_;
   stats_.reconciles++;
-  // ValidateOnDevice: the cache holds the clocked pod-list snapshot; a change of mode starts it over
-  const bool dev = validateOnDevice();
-  if (k.valid && k.pods != dev) ResetIncremental();
-  k.pods = dev;
+  // ValidateOnDevice / WaitForCompletionOnDevice: the cache holds the clocked pod-list snapshot; a change of mode starts
+  // it over
+  const bool val = validateOnDevice(), wait = waitOnDevice(*upgradePolicy), dev = val || wait;
+  if (k.valid && (k.validation != val || k.wait != wait)) ResetIncremental();
+  k.pods = dev; k.validation = val; k.wait = wait;
   int64_t now = 0;
-  PodsByNode byNode;
-  Error listErr;
+  PodsByNode byNode, waitByNode;
+  Error listErr, waitListErr;
   if (dev) {
-    pol.evaluate_actuators = UST_EVAL_ACTUATORS | UST_EVAL_VALIDATION;
+    pol.evaluate_actuators = UST_EVAL_ACTUATORS | (val ? UST_EVAL_VALIDATION : 0);
     now = opts_.Now();
-    listErr = listValidationPods(K8sClient, validationSelector_, &byNode);
+    if (val) listErr = listPodsBySelector(K8sClient, validationSelector_, "validation", &byNode);
+    if (wait) waitListErr = listPodsBySelector(K8sClient, upgradePolicy->WaitForCompletion->PodSelector, "wait-for-completion", &waitByNode);
   }
   const bool full = !k.valid;
   for (auto& sl : k.slots) sl.seen = false;
@@ -1167,6 +1247,7 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
     Cache nk;
     nk.slots.reserve(nNew); nk.state.reserve(nNew); nk.flags.reserve(nNew); nk.pod_rev.reserve(nNew); nk.ds_idx.reserve(nNew);
     nk.next.reserve(nNew); nk.actions.reserve(nNew); nk.deferredMsg.reserve(nNew);
+    if (dev) nk.outcome.reserve(nNew);
     joined.assign(nNew, 0);
     for (size_t p = 0; p < nNew; p++) {
       if (from[p] < 0) {
@@ -1180,7 +1261,10 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
         nk.slots.back().id = id;
         nk.state.push_back(UST_STATE_EXCLUDED); nk.flags.push_back(0); nk.pod_rev.push_back(0); nk.ds_idx.push_back(-1);
         nk.next.push_back(0); nk.actions.push_back(0); nk.deferredMsg.emplace_back();
-        if (dev) { nk.lists.emplace_back(); nk.listSig.emplace_back("\x01"); nk.start.push_back(0); }
+        if (dev) {
+          nk.lists.emplace_back(); nk.listSig.emplace_back("\x01"); nk.start.push_back(0);
+          nk.nval.push_back(0); nk.waitSig.emplace_back("\x01"); nk.outcome.push_back(UST_OUTCOME_NONE);
+        }
         continue;
       }
       const size_t q = (size_t)from[p];
@@ -1188,11 +1272,16 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
       nk.state.push_back(k.state[q]); nk.flags.push_back(k.flags[q]); nk.pod_rev.push_back(k.pod_rev[q]); nk.ds_idx.push_back(k.ds_idx[q]);
       nk.next.push_back(q < k.next.size() ? k.next[q] : 0); nk.actions.push_back(q < k.actions.size() ? k.actions[q] : 0);
       nk.deferredMsg.push_back(std::move(k.deferredMsg[q]));
-      if (dev) { nk.lists.push_back(std::move(k.lists[q])); nk.listSig.push_back(std::move(k.listSig[q])); nk.start.push_back(k.start[q]); }
+      if (dev) {
+        nk.lists.push_back(std::move(k.lists[q])); nk.listSig.push_back(std::move(k.listSig[q])); nk.start.push_back(k.start[q]);
+        nk.nval.push_back(k.nval[q]); nk.waitSig.push_back(std::move(k.waitSig[q]));
+        nk.outcome.push_back(q < k.outcome.size() ? k.outcome[q] : UST_OUTCOME_NONE);
+      }
     }
     k.slots.swap(nk.slots); k.state.swap(nk.state); k.flags.swap(nk.flags); k.pod_rev.swap(nk.pod_rev); k.ds_idx.swap(nk.ds_idx);
     k.next.swap(nk.next); k.actions.swap(nk.actions); k.deferredMsg.swap(nk.deferredMsg);
     k.lists.swap(nk.lists); k.listSig.swap(nk.listSig); k.start.swap(nk.start);
+    k.nval.swap(nk.nval); k.waitSig.swap(nk.waitSig); k.outcome.swap(nk.outcome);
     for (size_t i = 0; i < k.slots.size(); i++) k.slotOfId[k.slots[i].id] = i;
   }
   if (!full) {
@@ -1205,9 +1294,11 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
   // this reconcile's view in pass order (what Replay walks): entry, its slot
   EncodedSnapshot view;
   view.policy = pol;
-  view.validateOnDevice = dev;
+  view.validateOnDevice = val;
+  view.waitOnDevice = wait;
   view.now = now;
   view.listError = listErr;
+  view.waitListError = waitListErr;
   std::vector<char> sendList(dev ? k.slots.size() : 0, 0);
   std::vector<size_t> slotOfView;
   bool orderBroken = false;
@@ -1228,7 +1319,8 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
     if (!versioned || sig != sl.sig || sl.code != code) {
       uint8_t hot; uint32_t f; int32_t rev; std::string deferred;
       int64_t start = 0;
-      if (Error err = encodeOne(ns, code, ds, dsErr, &k.intern, k.ds_rev, &hot, &f, &rev, &deferred, dev ? &start : nullptr)) return err;
+      if (Error err = encodeOne(ns, code, ds, dsErr, &k.intern, k.ds_rev, &hot, &f, &rev, &deferred, dev ? &start : nullptr, val, wait))
+        return err;
       stats_.encoded++;
       if (hot != k.state[i] || f != k.flags[i] || rev != k.pod_rev[i] || ds != k.ds_idx[i] || (dev && start != k.start[i])) {
         k.state[i] = hot; k.flags[i] = f; k.pod_rev[i] = rev; k.ds_idx[i] = ds;
@@ -1242,28 +1334,41 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
       stats_.reused++;
     }
     if (dev) {
-      // the node's validation pods: rebuilt when the (pod, resourceVersion) sequence changed, sent when the bits did (or the
-      // node joined: an inserted node brings its list). After a failed List the resident lists stay as they are.
+      // the node's list, validation pods first, then wait-selector pods: each half is rebuilt when its (pod,
+      // resourceVersion) sequence changed, and the list is sent when its bits did (or the node joined: an inserted node
+      // brings its list). After a failed List that half stays as it is.
       const bool joinedNode = !joined.empty() && joined[i];
-      if (!listErr) {
-        auto it = byNode.find(n.Name);
+      auto refresh = [&](const PodsByNode& by, std::string* sigStore, uint16_t (*flagsOf)(const Pod&), std::vector<uint16_t>* half) {
+        const std::vector<const Pod*>* pods = podsOf(by, n.Name);
         std::string lsig;
         bool lversioned = true;
-        if (it != byNode.end())
-          for (const Pod* p : it->second) {
+        if (pods)
+          for (const Pod* p : *pods) {
             lversioned = lversioned && !p->ResourceVersion.empty();
             lsig += p->Namespace + "/" + p->Name + "@" + p->ResourceVersion + ";";
           }
-        if (!lversioned || lsig != k.listSig[i]) {
-          std::vector<uint16_t> fl;
-          if (it != byNode.end())
-            for (const Pod* p : it->second) fl.push_back(validationPodFlags(*p));
-          if (fl != k.lists[i]) { k.lists[i].swap(fl); sendList[i] = 1; }
-          k.listSig[i] = lversioned ? lsig : std::string("\x01");
-        }
+        if (lversioned && lsig == *sigStore) return false;
+        half->clear();
+        if (pods)
+          for (const Pod* p : *pods) half->push_back(flagsOf(*p));
+        *sigStore = lversioned ? lsig : std::string("\x01");
+        return true;
+      };
+      std::vector<uint16_t>& list = k.lists[i];
+      std::vector<uint16_t> vhalf, whalf;
+      const bool newV = val && !listErr && refresh(byNode, &k.listSig[i], validationPodFlags, &vhalf);
+      const bool newW = wait && !waitListErr && refresh(waitByNode, &k.waitSig[i], waitPodFlags, &whalf);
+      if (newV || newW) {
+        if (!newV) vhalf.assign(list.begin(), list.begin() + k.nval[i]);
+        if (!newW) whalf.assign(list.begin() + k.nval[i], list.end());
+        const int32_t nv = (int32_t)vhalf.size();
+        vhalf.insert(vhalf.end(), whalf.begin(), whalf.end());
+        if (vhalf != list) { list.swap(vhalf); sendList[i] = 1; }
+        k.nval[i] = nv;
       }
       if (joinedNode) sendList[i] = 1;
-      if (code == UST_STATE_VALIDATION_REQUIRED) stats_.validate_avoided++;
+      if (val && code == UST_STATE_VALIDATION_REQUIRED) stats_.validate_avoided++;
+      if (wait && code == UST_STATE_WAIT_FOR_JOBS_REQUIRED) stats_.wait_avoided++;
     }
     if (!slotOfView.empty() && (int)(view.state.back() & UST_HOT_STATE_MASK) == code && slotOfView.back() > i)
       orderBroken = true;  // within a bucket, slot order must be the slice order: slots are handed out in it
@@ -1316,17 +1421,23 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
   k.valid = true;
   // Replay walks this reconcile's view: gather its outputs, translate the abort position
   const size_t nv = view.entries.size();
-  std::vector<uint8_t> next(nv + 1);
+  std::vector<uint8_t> next(nv + 1), outcome(nv + 1, UST_OUTCOME_NONE);
   std::vector<uint16_t> actions(nv + 1);
+  if (wait) view.waitRunning.assign(nv, 0);
   ust_counters c = last_;
   for (size_t v = 0; v < nv; v++) {
     const size_t i = slotOfView[v];
     next[v] = k.next[i];
     actions[v] = k.actions[i];
+    if (dev) outcome[v] = k.outcome[i];
+    if (wait && (view.state[v] & UST_HOT_STATE_MASK) == UST_STATE_WAIT_FOR_JOBS_REQUIRED) {
+      const std::vector<uint16_t>& l = k.lists[i];  // the list the device holds for the node
+      view.waitRunning[v] = anyWaitRunning(l.data() + k.nval[i], l.data() + l.size());
+    }
     if (!k.deferredMsg[i].empty()) view.deferred[v] = k.deferredMsg[i];
     if (last_.error_index == (int64_t)i) c.error_index = (int64_t)v;
   }
-  return Replay(view, *upgradePolicy, next.data(), actions.data(), rc, c);
+  return Replay(view, *upgradePolicy, next.data(), actions.data(), rc, c, outcome.data());
 }
 
 }  // namespace upgrade

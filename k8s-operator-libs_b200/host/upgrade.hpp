@@ -183,9 +183,10 @@ struct K8sClient {
   // (:370-414), the NodeMaintenance CRUD of the upgrade-required and uncordon-required passes
   virtual Error CreateOrUpdateNodeMaintenance(NodeUpgradeState* nodeState) { (void)nodeState; return std::nullopt; }
   virtual Error DeleteOrUpdateNodeMaintenance(NodeUpgradeState* nodeState) { (void)nodeState; return std::nullopt; }
-  // The ValidationManager's List (validation_manager.go:77-79): the pods of every namespace that match the label selector
-  // `selector` ("k=v[,k=v]") and run on node `nodeName` ("" = on any node), in the order the API returns them. Used by
-  // StateOptions::ValidateOnDevice, which makes one such List per reconcile with nodeName "".
+  // The ValidationManager's List (validation_manager.go:77-79) and the PodManager's (pod_manager.go:320-329): the pods of
+  // every namespace that match the label selector `selector` ("k=v[,k=v]") and run on node `nodeName` ("" = on any node),
+  // in the order the API returns them. Used by StateOptions::ValidateOnDevice and WaitForCompletionOnDevice, which make
+  // one such List per reconcile each, with nodeName "".
   virtual Error ListPodsBySelector(const std::string& selector, const std::string& nodeName, std::vector<Pod*>* out) {
     (void)selector; (void)nodeName; (void)out;
     return Errorf("this K8sClient cannot list pods by label selector");
@@ -206,8 +207,16 @@ struct StateOptions {                                                 // upgrade
   // annotation to the clocked pod-list calls, and replay the annotation and state calls Validate would have made; the
   // injected ValidationManager is never called. ApplyStateIncremental then keeps the lists and start times resident too.
   bool ValidateOnDevice = false;
-  // The reconcile's time.Now().Unix(): read once per ApplyState call; the device derives the validation timeout from it
-  // and a new validation start-time annotation is set to it.
+  // Not in the reference: answer PodManager::ScheduleCheckOnPodCompletion on the device (UST_EVAL_ACTUATORS) instead of
+  // calling it. With a policy whose WaitForCompletion has a non-empty PodSelector, ApplyState and ApplyStateIncremental
+  // make one K8sClient::ListPodsBySelector per reconcile for that selector, hand every node its wait-selector pods (after
+  // its validation pods when ValidateOnDevice is on too) and its parsed wait-for-pod-completion start-time annotation to
+  // the clocked pod-list calls, and replay the annotation and state calls the check would have made; the injected
+  // PodManager is never asked to check. Eviction, drain and pod restarts still go to the injected managers. Without a
+  // selector the wait-for-jobs pass moves its nodes on by itself and the option changes nothing.
+  bool WaitForCompletionOnDevice = false;
+  // The reconcile's time.Now().Unix(): read once per ApplyState call; the device derives the validation and
+  // wait-for-completion timeouts from it, and a new start-time annotation of either kind is set to it.
   std::function<int64_t()> Now = [] { return (int64_t)time(nullptr); };
 };
 
@@ -228,6 +237,14 @@ struct EncodedSnapshot {
   std::vector<int64_t> start;
   int64_t now = 0;
   Error listError;
+  // StateOptions::WaitForCompletionOnDevice (with a wait selector): the wait-selector pods follow each entry's validation
+  // pods in pod_off / pod_flags (UST_POD_MATCH_WAIT_SELECTOR + phase), a wait-for-jobs-required entry's start is its parsed
+  // wait start-time annotation; per entry whether one of its wait pods is Running or Pending (Replay tells the two
+  // pod-deletion-required call orders apart with it); and the wait List's error, which Replay returns at the
+  // wait-for-jobs pass when that pass has nodes.
+  bool waitOnDevice = false;
+  std::vector<char> waitRunning;
+  Error waitListError;
 };
 
 // ---- common_manager.go:23-41 --------------------------------------------------------------------------------
@@ -294,10 +311,11 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
 
   // The two halves of ApplyState around the kernel call. Public so that they can be audited separately:
   // Encode evaluates every reference predicate once and fills the struct-of-arrays; Replay performs the calls
-  // named by the action bits, in the reference's pass order, stopping at the first error.
+  // named by the action bits, in the reference's pass order, stopping at the first error. `actuator_outcome` is read
+  // only for the wait-for-jobs pass of an enc.waitOnDevice snapshot, which needs it.
   Error Encode(const ClusterUpgradeState& s, const DriverUpgradePolicySpec& policy, EncodedSnapshot* out);
   Error Replay(const EncodedSnapshot& enc, const DriverUpgradePolicySpec& policy, const uint8_t* next_state,
-               const uint16_t* actions, int abi_rc, const ust_counters& counters);
+               const uint16_t* actions, int abi_rc, const ust_counters& counters, const uint8_t* actuator_outcome = nullptr);
 
   const ust_counters& LastCounters() const { return last_; }
 
@@ -323,14 +341,18 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
     int64_t inserted = 0, removed = 0;  // nodes that joined / left the cached snapshot by a splice or reorder
     int64_t reorders = 0;               // reconciles that went to the device as a reorder (a surviving node moved)
     int64_t slots = 0;                  // size of the cached snapshot after the last reconcile
-    // StateOptions::ValidateOnDevice: validation pod lists sent to the device / left resident, reconciles that sent no node
-    // and no list (only time passed), and the ValidationManager::Validate calls (one API List each) not made
-    int64_t lists_sent = 0, lists_reused = 0, time_only = 0, validate_avoided = 0;
+    // StateOptions::ValidateOnDevice / WaitForCompletionOnDevice: pod lists sent to the device / left resident (a node has
+    // one list, its validation and wait-selector pods together, so both options share these two counters), reconciles
+    // that sent no node and no list (only time passed), the ValidationManager::Validate calls (one API List each) not made,
+    // and the per-node Lists of PodManager::ScheduleCheckOnPodCompletion not made (one per wait-for-jobs-required node)
+    int64_t lists_sent = 0, lists_reused = 0, time_only = 0, validate_avoided = 0, wait_avoided = 0;
   };
   const IncrementalStats& Stats() const { return stats_; }
   void ResetIncremental();
   // Switches StateOptions::ValidateOnDevice; the incremental cache starts over on the next call when the mode changes.
   void SetValidateOnDevice(bool on) { opts_.ValidateOnDevice = on; }
+  // Switches StateOptions::WaitForCompletionOnDevice, with the same effect on the incremental cache.
+  void SetWaitForCompletionOnDevice(bool on) { opts_.WaitForCompletionOnDevice = on; }
 
   // ---- incremental BuildState: the driver-pod list stays on the device (ust_build_state_delta) -----------------------------
   // The same contract, result and errors as BuildState, for a reconcile loop that calls it again and again. The manager keeps
@@ -412,11 +434,20 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
     std::vector<std::string> listSig;
     std::vector<int64_t> start;
     std::vector<int64_t> listChanged;
+    // Which of the two options filled the lists (a change starts the cache over). With WaitForCompletionOnDevice a slot's
+    // list is its validation pods (the first nval entries) followed by its wait-selector pods, whose (pod, resourceVersion)
+    // sequence is waitSig; each half is rebuilt from its own List. In either mode, actuator_outcome per slot, patched
+    // like next / actions: the replay of a wait-for-jobs-required node reads it on every reconcile.
+    bool validation = false, wait = false;
+    std::vector<int32_t> nval;
+    std::vector<std::string> waitSig;
+    std::vector<uint8_t> outcome;
   };
   virtual int EvaluateCached(const ust_policy& policy, bool full, const std::vector<int64_t>& changed, Cache* cache, ust_counters* c);
-  // The same on the clocked pod-list snapshot (StateOptions::ValidateOnDevice): full: ust_apply_state_clocked with every
-  // list and start time; else ust_apply_state_delta_pods_clocked with cache->pending as runs, the lists of
-  // cache->listChanged and the start times of `changed` and of the inserted slots. `now` / `waitTimeout` make the ust_clock.
+  // The same on the clocked pod-list snapshot (StateOptions::ValidateOnDevice / WaitForCompletionOnDevice): full:
+  // ust_apply_state_clocked with every list and start time; else ust_apply_state_delta_pods_clocked with cache->pending as
+  // runs, the lists of cache->listChanged and the start times of `changed` and of the inserted slots, patching
+  // cache->outcome too. `now` / `waitTimeout` make the ust_clock.
   virtual int EvaluateCachedPods(const ust_policy& policy, int64_t now, int64_t waitTimeout, bool full,
                                  const std::vector<int64_t>& changed, Cache* cache, ust_counters* c);
   ClusterUpgradeStateManagerImpl() = default;
@@ -425,8 +456,11 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
  private:
   Error encodeOne(const NodeUpgradeState* ns, int code, int32_t ds, bool dsErr, std::map<std::string, int32_t>* intern,
                   const std::vector<int32_t>& ds_rev, uint8_t* hot, uint32_t* flags, int32_t* rev, std::string* deferred,
-                  int64_t* validationStart);
+                  int64_t* start, bool validation, bool wait);
   bool validateOnDevice() const { return opts_.ValidateOnDevice && validationStateEnabled_; }
+  bool waitOnDevice(const DriverUpgradePolicySpec& p) const {
+    return opts_.WaitForCompletionOnDevice && p.WaitForCompletion && !p.WaitForCompletion->PodSelector.empty();
+  }
   Error assembleState(const std::vector<Pod*>& podList, const uint8_t* podState, const int32_t* owner_idx,
                       std::map<std::string, DaemonSet*>& daemonSets, std::unique_ptr<ClusterUpgradeState>* out);
   Cache cache_;
