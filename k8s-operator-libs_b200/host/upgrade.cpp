@@ -5,7 +5,10 @@
 #include <climits>
 #include <thread>
 #include <unordered_map>
+#include <unordered_set>
 #include <cstring>
+
+#include "../csrc/ust_lut.h"  // ust_pod_chain_keeps: the pods a drain evicts
 
 namespace upgrade {
 
@@ -102,7 +105,51 @@ std::unique_ptr<ClusterUpgradeStateManagerImpl> ClusterUpgradeStateManagerImpl::
   m->opts_ = opts;
   return m;
 }
-ClusterUpgradeStateManagerImpl::~ClusterUpgradeStateManagerImpl() { if (handle_) ust_destroy(handle_); }
+ClusterUpgradeStateManagerImpl::~ClusterUpgradeStateManagerImpl() {
+  {
+    std::unique_lock<std::mutex> l(actMu_);
+    actCv_.wait(l, [&] { return actQueue_.empty() && actRunning_ == 0; });
+    actStop_ = true;
+  }
+  actCv_.notify_all();
+  for (auto& t : actThreads_) t.join();
+  if (handle_) ust_destroy(handle_);
+}
+
+// ---- the PodEvictor's workers (StateOptions::EvictionOnDevice) ---------------------------------------------------
+void ClusterUpgradeStateManagerImpl::handOff(std::set<std::string>* dedupe, const std::string& name, std::function<void()> job) {
+  std::lock_guard<std::mutex> l(actMu_);
+  dedupe->insert(name);
+  actQueue_.push_back([this, dedupe, name, job = std::move(job)] {
+    job();
+    std::lock_guard<std::mutex> g(actMu_);
+    dedupe->erase(name);  // defer m.nodesInProgress.Remove / m.drainingNodes.Remove (pod_manager.go:165, drain_manager.go:110)
+  });
+  if (actIdle_ < actQueue_.size() && actThreads_.size() < kActuatorWorkers) {
+    actThreads_.emplace_back([this] {
+      std::unique_lock<std::mutex> l(actMu_);
+      for (;;) {
+        actIdle_++;
+        actCv_.wait(l, [&] { return actStop_ || !actQueue_.empty(); });
+        actIdle_--;
+        if (actQueue_.empty()) return;  // stopping
+        std::function<void()> f = std::move(actQueue_.front());
+        actQueue_.pop_front();
+        actRunning_++;
+        l.unlock();
+        f();
+        l.lock();
+        actRunning_--;
+        actCv_.notify_all();
+      }
+    });
+  }
+  actCv_.notify_all();
+}
+void ClusterUpgradeStateManagerImpl::WaitForActuators() {
+  std::unique_lock<std::mutex> l(actMu_);
+  actCv_.wait(l, [&] { return actQueue_.empty() && actRunning_ == 0; });
+}
 
 ClusterUpgradeStateManager& ClusterUpgradeStateManagerImpl::WithPodDeletionEnabled(PodDeletionFilter filter) {
   if (!filter) return *this;  // "Cannot enable PodDeletion state as PodDeletionFilter is nil"  upgrade_state.go:330-333
@@ -537,11 +584,12 @@ static uint16_t validationPodFlags(const Pod& p) {
 
 // A wait-selector pod as ScheduleCheckOnPodCompletion sees it (pod_manager.go:263, :371-391): it matched the selector,
 // and only its phase matters; a phase IsPodRunningOrPending does not name counts as not running.
-static uint16_t waitPodFlags(const Pod& p) {
-  const unsigned phase = p.Phase == "Running" ? UST_PHASE_RUNNING : p.Phase == "Pending" ? UST_PHASE_PENDING
-                         : p.Phase == "Succeeded" ? UST_PHASE_SUCCEEDED : p.Phase == "Failed" ? UST_PHASE_FAILED : UST_PHASE_OTHER;
-  return (uint16_t)(UST_POD_MATCH_WAIT_SELECTOR | phase);
+// a pod phase as UST_PHASE_*; a phase IsPodRunningOrPending does not name is UST_PHASE_OTHER
+static uint16_t phaseBits(const Pod& p) {
+  return (uint16_t)(p.Phase == "Running" ? UST_PHASE_RUNNING : p.Phase == "Pending" ? UST_PHASE_PENDING
+                    : p.Phase == "Succeeded" ? UST_PHASE_SUCCEEDED : p.Phase == "Failed" ? UST_PHASE_FAILED : UST_PHASE_OTHER);
 }
+static uint16_t waitPodFlags(const Pod& p) { return (uint16_t)(UST_POD_MATCH_WAIT_SELECTOR | phaseBits(p)); }
 // "any wait pod Running or Pending" (pod_manager.go:278-284) over a node's list as handed to the device
 static bool anyWaitRunning(const uint16_t* b, const uint16_t* e) {
   for (; b != e; b++) {
@@ -549,6 +597,64 @@ static bool anyWaitRunning(const uint16_t* b, const uint16_t* e) {
     if ((*b & UST_POD_MATCH_WAIT_SELECTOR) && (phase == UST_PHASE_RUNNING || phase == UST_PHASE_PENDING)) return true;
   }
   return false;
+}
+
+// A workload pod as the kubectl drain filter chain sees it (k8s.io/kubectl pkg/drain/filters.go; ust_pod_chain_keeps):
+// phase, metav1.GetControllerOf (the first owner reference with Controller set) and whether that controller is a
+// DaemonSet the DaemonSet List does not hold (daemonSetFilter's Get by namespace and name, NotFound), the mirror-pod
+// annotation, an emptyDir volume; and whether the pod-deletion filter and the drain's PodSelector select it. kubectl's
+// skipDeletedFilter never skips a pod here: both helpers leave SkipWaitForDeleteTimeoutSeconds at 0 (pod_manager.go:146-157,
+// drain_manager.go:76-96), and shouldSkipPod requires it to be > 0 (filters.go).
+static const OwnerReference* controllerOf(const Pod& p) {
+  for (const auto& o : p.OwnerReferences)
+    if (o.Controller) return &o;
+  return nullptr;
+}
+static const char* const kMirrorPodAnnotationKey = "kubernetes.io/config.mirror";  // corev1.MirrorPodAnnotationKey
+// What the workload entries of one reconcile are derived from: every pod by node (ListPodsBySelector("", "")), the pods
+// the drain's PodSelector matches (a second List, only for a non-empty selector: the mirror matches no label selector
+// itself) and every DaemonSet (ListDaemonSets), keyed by Namespace/Name.
+struct WorkloadLists {
+  std::unordered_map<std::string, std::vector<const Pod*>> byNode;
+  bool drainAll = true;
+  std::unordered_set<std::string> drainSelected, daemonSets;
+  const PodDeletionFilter* filter = nullptr;  // nullptr: the pod-deletion pass is not answered on the device
+  bool drain = false;                         // the drain pass is
+  Error podsError, selectorError, dsError;
+};
+static void listWorkload(K8sClient* client, const DriverUpgradePolicySpec& policy, const PodDeletionFilter* filter, bool drain,
+                         WorkloadLists* w) {
+  w->filter = filter;
+  w->drain = drain;
+  if (client == nullptr) { w->podsError = Errorf("no K8sClient to list the workload pods with"); return; }
+  std::vector<Pod*> pods;
+  if ((w->podsError = client->ListPodsBySelector("", "", &pods))) return;
+  for (const Pod* p : pods)
+    if (!p->NodeName.empty()) w->byNode[p->NodeName].push_back(p);
+  if (drain && !policy.DrainSpec->PodSelector.empty()) {
+    w->drainAll = false;
+    std::vector<Pod*> sel;
+    if (!(w->selectorError = client->ListPodsBySelector(policy.DrainSpec->PodSelector, "", &sel)))
+      for (const Pod* p : sel) w->drainSelected.insert(p->Namespace + "/" + p->Name);
+  }
+  std::vector<DaemonSet*> dss;
+  if (!(w->dsError = client->ListDaemonSets("", {}, &dss)))
+    for (const DaemonSet* d : dss) w->daemonSets.insert(d->Namespace + "/" + d->Name);
+}
+static uint16_t workloadPodFlags(const Pod& p, const WorkloadLists& w) {
+  uint16_t f = phaseBits(p);
+  if (const OwnerReference* c = controllerOf(p)) {
+    f |= UST_POD_HAS_CONTROLLER;
+    if (c->Kind == "DaemonSet") {
+      f |= UST_POD_CONTROLLED_BY_DS;
+      if (!w.daemonSets.count(p.Namespace + "/" + c->Name)) f |= UST_POD_DS_MISSING;
+    }
+  }
+  if (p.Annotations.count(kMirrorPodAnnotationKey)) f |= UST_POD_MIRROR;
+  if (p.HasEmptyDirVolume) f |= UST_POD_HAS_EMPTYDIR;
+  if (w.filter && (*w.filter)(p)) f |= UST_POD_MATCH_DELETION_FILTER;
+  if (w.drain && (w.drainAll || w.drainSelected.count(p.Namespace + "/" + p.Name))) f |= UST_POD_MATCH_DRAIN_SELECTOR;
+  return f;
 }
 
 // The one List per selector of a ValidateOnDevice / WaitForCompletionOnDevice reconcile, grouped by node. The reference
@@ -719,7 +825,8 @@ Error ClusterUpgradeStateManagerImpl::Encode(const ClusterUpgradeState& s, const
   e.pod_rev.assign(n, 0);
   e.validateOnDevice = validateOnDevice();
   e.waitOnDevice = waitOnDevice(policy);
-  const bool clocked = e.validateOnDevice || e.waitOnDevice;
+  e.evictOnDevice = evictOnDevice(policy);
+  const bool clocked = e.validateOnDevice || e.waitOnDevice || e.evictOnDevice;
   if (clocked) e.start.assign(n, 0);
   const int32_t base = (int32_t)intern.size();
   const size_t workers = (size_t)std::max(1, std::min(opts_.EncodeThreads, (int)(n / 4096 + 1)));
@@ -769,9 +876,10 @@ Error ClusterUpgradeStateManagerImpl::Encode(const ClusterUpgradeState& s, const
         if (e.pod_rev[i] > base) e.pod_rev[i] = remap[(size_t)e.pod_rev[i]];
     }
   }
-  // 4. ValidateOnDevice / WaitForCompletionOnDevice: every entry's list (an empty one when it has no pod), from one List
-  //    per selector: its validation pods, then its wait-selector pods. A pod both selectors match is in the list twice,
-  //    each entry with its own selector bit: each pass reads only its own bit.
+  // 4. ValidateOnDevice / WaitForCompletionOnDevice / EvictionOnDevice: every entry's list (an empty one when it has no
+  //    pod), from one List per selector: its validation pods, then its wait-selector pods, then (pod-deletion-required and
+  //    drain-required entries only) every pod on its node. A pod several Lists hold is in the list once per List, each
+  //    entry with its own role's bits: each pass reads only the entries that carry its own selector bit.
   if (clocked) {
     e.policy.evaluate_actuators = UST_EVAL_ACTUATORS | (e.validateOnDevice ? UST_EVAL_VALIDATION : 0);
     e.now = opts_.Now();
@@ -780,6 +888,12 @@ Error ClusterUpgradeStateManagerImpl::Encode(const ClusterUpgradeState& s, const
     if (e.waitOnDevice) {
       e.waitListError = listPodsBySelector(K8sClient, policy.WaitForCompletion->PodSelector, "wait-for-completion", &wpods);
       e.waitRunning.assign(n, 0);
+    }
+    WorkloadLists wl;
+    if (e.evictOnDevice) {
+      listWorkload(K8sClient, policy, evictPodDeletion(policy) ? &filter_ : nullptr, evictDrain(policy), &wl);
+      e.evictListError = wl.podsError ? wl.podsError : wl.dsError;
+      e.drainListError = e.evictListError ? e.evictListError : wl.selectorError;
     }
     e.pod_off.assign(n + 1, 0);
     for (size_t i = 0; i < n; i++) {
@@ -790,6 +904,16 @@ Error ClusterUpgradeStateManagerImpl::Encode(const ClusterUpgradeState& s, const
       if (const auto* w = e.waitListError ? nullptr : podsOf(wpods, name))
         for (const Pod* p : *w) e.pod_flags.push_back(waitPodFlags(*p));
       if (e.waitOnDevice) e.waitRunning[i] = anyWaitRunning(e.pod_flags.data() + w0, e.pod_flags.data() + e.pod_flags.size());
+      const int code = codes[i];
+      if (e.evictOnDevice && !e.evictListError && (code == UST_STATE_POD_DELETION_REQUIRED || code == UST_STATE_DRAIN_REQUIRED))
+        if (const auto* a = podsOf(wl.byNode, name)) {
+          EncodedSnapshot::Workload& wk = e.workload[i];
+          for (const Pod* p : *a) {
+            wk.pods.push_back(p);
+            wk.bits.push_back(workloadPodFlags(*p, wl));
+          }
+          e.pod_flags.insert(e.pod_flags.end(), wk.bits.begin(), wk.bits.end());
+        }
       e.pod_off[i + 1] = (int32_t)e.pod_flags.size();
     }
   }
@@ -908,7 +1032,52 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
         }
         break;
       case UST_STATE_POD_DELETION_REQUIRED:
-        if (podDeletionStateEnabled_ && !batchNodes.empty()) {  // common_manager.go:437-452
+        if (enc.evictOnDevice && evictPodDeletion(policy)) {
+          if (i == begin) break;
+          // the goroutines of SchedulePodEviction (pod_manager.go:159-227), as the device answered them. The List they
+          // were answered from came first: a failed one returns before any node is touched.
+          if (enc.evictListError) return enc.evictListError;
+          if (actuator_outcome == nullptr) return Errorf("Replay: the pod-deletion pass on the device needs actuator_outcome");
+          const PodDeletionSpec& spec = *policy.PodDeletion;
+          for (size_t k = begin; k < i; k++) {
+            if (!(actions[k] & UST_A_SCHEDULE_POD_EVICTION)) continue;
+            const std::string& name = enc.entries[k]->Node->Name;
+            {
+              std::lock_guard<std::mutex> l(actMu_);
+              if (nodesInProgress_.count(name)) continue;  // "Node is already getting pods deleted, skipping" (:224-226)
+            }
+            Node node = *enc.entries[k]->Node;  // go func(node corev1.Node) (:164, :223): the calls act on a copy
+            const auto w = enc.workload.find(k);
+            // toDelete: the pods the filter selects (:176-182). GetPodsForDeletion(node).Pods() holds a pod only when every
+            // filter says "delete", and the deletion filter says "skip" for any other pod (:138-144), so Pods() is a subset
+            // of toDelete; with numPodsCanDelete == numPodsToDelete (:193-201) the two sets are equal, in the List's order.
+            std::vector<Pod> toDelete;
+            if (w != enc.workload.end())
+              for (size_t j = 0; j < w->second.pods.size(); j++)
+                if (w->second.bits[j] & UST_POD_MATCH_DELETION_FILTER) toDelete.push_back(*w->second.pods[j]);
+            const uint8_t out = actuator_outcome[k];
+            if (out == UST_STATE_DRAIN_REQUIRED || out == UST_STATE_FAILED) {  // updateNodeToDrainOrFailed (:194-201, :393-403)
+              (void)NodeUpgradeStateProvider->ChangeNodeUpgradeState(&node, StateNameOfCode(out));
+            } else if (out != UST_STATE_POD_RESTART_REQUIRED) {
+              return Errorf("Replay: no pod-deletion outcome for node " + name);
+            } else if (toDelete.empty()) {  // "No pods require deletion" (:184-188)
+              (void)NodeUpgradeStateProvider->ChangeNodeUpgradeState(&node, UpgradeStatePodRestartRequired);
+            } else {  // DeleteOrEvictPods, then the state (:210-222)
+              EvictionOptions o;
+              o.Force = spec.Force; o.DeleteEmptyDir = spec.DeleteEmptyDir; o.TimeoutSecond = spec.TimeoutSecond;
+              upgrade::NodeUpgradeStateProvider* provider = NodeUpgradeStateProvider;
+              upgrade::PodEvictor* evictor = PodEvictor;
+              stats_.actuator_handoffs++;
+              handOff(&nodesInProgress_, name, [provider, evictor, node, pods = std::move(toDelete), o, drainEnabled]() mutable {
+                std::vector<Pod*> ptrs;
+                for (Pod& p : pods) ptrs.push_back(&p);
+                const Error err = evictor ? evictor->DeleteOrEvictPods(node, ptrs, o) : Errorf("no PodEvictor");
+                (void)provider->ChangeNodeUpgradeState(&node, !err ? UpgradeStatePodRestartRequired
+                                                                   : drainEnabled ? UpgradeStateDrainRequired : UpgradeStateFailed);
+              });
+            }
+          }
+        } else if (podDeletionStateEnabled_ && !batchNodes.empty()) {  // common_manager.go:437-452
           PodManagerConfig cfg;
           cfg.DeletionSpec = policy.PodDeletion ? &*policy.PodDeletion : nullptr;
           cfg.DrainEnabled = drainEnabled;
@@ -917,7 +1086,56 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
         }
         break;
       case UST_STATE_DRAIN_REQUIRED:
-        if (drainEnabled) {  // common_manager.go:346-356 (called even with an empty node list)
+        if (enc.evictOnDevice && drainEnabled) {
+          if (i == begin) break;
+          // the goroutines of ScheduleNodesDrain (drain_manager.go:98-137), as the device answered RunNodeDrain's filter
+          // chain; the cordon, the eviction and the state change after them run on a worker
+          if (enc.drainListError) return enc.drainListError;
+          if (actuator_outcome == nullptr) return Errorf("Replay: the drain pass on the device needs actuator_outcome");
+          const upgrade::DrainSpec& spec = *policy.DrainSpec;
+          for (size_t k = begin; k < i; k++) {
+            if (!(actions[k] & UST_A_SCHEDULE_DRAIN)) continue;
+            const std::string& name = enc.entries[k]->Node->Name;
+            {
+              std::lock_guard<std::mutex> l(actMu_);
+              if (drainingNodes_.count(name)) continue;  // "Node is already being drained, skipping" (:134-136)
+            }
+            const uint8_t out = actuator_outcome[k];
+            if (out != UST_STATE_FAILED && out != UST_STATE_POD_RESTART_REQUIRED) return Errorf("Replay: no drain outcome for node " + name);
+            // list.Pods() of GetPodsForDeletion: the selected pods the chain does not keep, in the List's order
+            std::vector<Pod> toEvict;
+            const auto w = enc.workload.find(k);
+            if (out == UST_STATE_POD_RESTART_REQUIRED && w != enc.workload.end())
+              for (size_t j = 0; j < w->second.pods.size(); j++) {
+                bool isError = false;
+                const uint16_t b = w->second.bits[j];
+                if ((b & UST_POD_MATCH_DRAIN_SELECTOR) && !ust_pod_chain_keeps(b, spec.Force, spec.DeleteEmptyDir, &isError))
+                  toEvict.push_back(*w->second.pods[j]);
+              }
+            EvictionOptions o;
+            o.Force = spec.Force; o.DeleteEmptyDir = spec.DeleteEmptyDir; o.TimeoutSecond = spec.TimeoutSecond;
+            upgrade::NodeUpgradeStateProvider* provider = NodeUpgradeStateProvider;
+            upgrade::CordonManager* cordon = CordonManager;
+            upgrade::PodEvictor* evictor = PodEvictor;
+            stats_.actuator_handoffs++;
+            Node node = *enc.entries[k]->Node;  // the worker's copy: it outlives this call
+            handOff(&drainingNodes_, name, [provider, cordon, evictor, node, pods = std::move(toEvict), o, out]() mutable {
+              if (cordon->Cordon(&node)) {  // drain.RunCordonOrUncordon (:111-118)
+                (void)provider->ChangeNodeUpgradeState(&node, UpgradeStateFailed);
+                return;
+              }
+              Error err;
+              if (out == UST_STATE_FAILED) {
+                err = Errorf("the drain filter chain reports an error");  // GetPodsForDeletion's errors (:121-128)
+              } else if (!pods.empty()) {  // DeleteOrEvictPods returns at once for no pods
+                std::vector<Pod*> ptrs;
+                for (Pod& p : pods) ptrs.push_back(&p);
+                err = evictor ? evictor->DeleteOrEvictPods(node, ptrs, o) : Errorf("no PodEvictor");
+              }
+              (void)provider->ChangeNodeUpgradeState(&node, err ? UpgradeStateFailed : UpgradeStatePodRestartRequired);  // :121-132
+            });
+          }
+        } else if (drainEnabled) {  // common_manager.go:346-356 (called even with an empty node list)
           DrainConfiguration cfg;
           cfg.Spec = &*policy.DrainSpec;
           cfg.Nodes = batchNodes;
@@ -966,8 +1184,9 @@ Error ClusterUpgradeStateManagerImpl::ApplyState(ClusterUpgradeState* currentSta
   enc.ds_rev.push_back(0);
   int rc;
   std::vector<uint8_t> outcome(n + 1, UST_OUTCOME_NONE);
-  if (enc.validateOnDevice || enc.waitOnDevice) {  // Validate / the wait check on the device: the pods, the start times and
-                                                   // `now` go with the call
+  if (enc.validateOnDevice || enc.waitOnDevice || enc.evictOnDevice) {  // Validate / the wait check / the eviction and drain
+                                                                       // decisions on the device: the pods, the start times
+                                                                       // and `now` go with the call
     enc.pod_flags.push_back(0); enc.start.push_back(0);
     const ust_pods pods = {enc.pod_off.data(), enc.pod_flags.data(), (int64_t)enc.pod_flags.size() - 1};
     const ust_clock clock = {enc.now, upgradePolicy->WaitForCompletion ? upgradePolicy->WaitForCompletion->TimeoutSecond : 0, enc.start.data(), nullptr};
@@ -1151,12 +1370,20 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
   stats_.reconciles++;
   // ValidateOnDevice / WaitForCompletionOnDevice: the cache holds the clocked pod-list snapshot; a change of mode starts
   // it over
-  const bool val = validateOnDevice(), wait = waitOnDevice(*upgradePolicy), dev = val || wait;
-  if (k.valid && (k.validation != val || k.wait != wait)) ResetIncremental();
-  k.pods = dev; k.validation = val; k.wait = wait;
+  const bool val = validateOnDevice(), wait = waitOnDevice(*upgradePolicy), evict = evictOnDevice(*upgradePolicy);
+  const bool dev = val || wait || evict;
+  if (k.valid && (k.validation != val || k.wait != wait || k.evict != evict)) ResetIncremental();
+  k.pods = dev; k.validation = val; k.wait = wait; k.evict = evict;
   int64_t now = 0;
   PodsByNode byNode, waitByNode;
-  Error listErr, waitListErr;
+  Error listErr, waitListErr, evictListErr;
+  WorkloadLists wl;
+  std::string workPolicy;  // what the workload bits depend on besides the pods: which passes, the drain's selector
+  if (evict) {
+    listWorkload(K8sClient, *upgradePolicy, evictPodDeletion(*upgradePolicy) ? &filter_ : nullptr, evictDrain(*upgradePolicy), &wl);
+    evictListErr = wl.podsError ? wl.podsError : wl.dsError;
+    workPolicy = std::string(wl.filter ? "F" : "-") + (wl.drain ? "D" + upgradePolicy->DrainSpec->PodSelector : "-") + "|";
+  }
   if (dev) {
     pol.evaluate_actuators = UST_EVAL_ACTUATORS | (val ? UST_EVAL_VALIDATION : 0);
     now = opts_.Now();
@@ -1264,6 +1491,7 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
         if (dev) {
           nk.lists.emplace_back(); nk.listSig.emplace_back("\x01"); nk.start.push_back(0);
           nk.nval.push_back(0); nk.waitSig.emplace_back("\x01"); nk.outcome.push_back(UST_OUTCOME_NONE);
+          nk.nwork.push_back(0); nk.workSig.emplace_back("\x01");
         }
         continue;
       }
@@ -1275,6 +1503,7 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
       if (dev) {
         nk.lists.push_back(std::move(k.lists[q])); nk.listSig.push_back(std::move(k.listSig[q])); nk.start.push_back(k.start[q]);
         nk.nval.push_back(k.nval[q]); nk.waitSig.push_back(std::move(k.waitSig[q]));
+        nk.nwork.push_back(k.nwork[q]); nk.workSig.push_back(std::move(k.workSig[q]));
         nk.outcome.push_back(q < k.outcome.size() ? k.outcome[q] : UST_OUTCOME_NONE);
       }
     }
@@ -1282,6 +1511,7 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
     k.next.swap(nk.next); k.actions.swap(nk.actions); k.deferredMsg.swap(nk.deferredMsg);
     k.lists.swap(nk.lists); k.listSig.swap(nk.listSig); k.start.swap(nk.start);
     k.nval.swap(nk.nval); k.waitSig.swap(nk.waitSig); k.outcome.swap(nk.outcome);
+    k.nwork.swap(nk.nwork); k.workSig.swap(nk.workSig);
     for (size_t i = 0; i < k.slots.size(); i++) k.slotOfId[k.slots[i].id] = i;
   }
   if (!full) {
@@ -1299,6 +1529,9 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
   view.now = now;
   view.listError = listErr;
   view.waitListError = waitListErr;
+  view.evictOnDevice = evict;
+  view.evictListError = evictListErr;
+  view.drainListError = evictListErr ? evictListErr : wl.selectorError;
   std::vector<char> sendList(dev ? k.slots.size() : 0, 0);
   std::vector<size_t> slotOfView;
   bool orderBroken = false;
@@ -1334,9 +1567,9 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
       stats_.reused++;
     }
     if (dev) {
-      // the node's list, validation pods first, then wait-selector pods: each half is rebuilt when its (pod,
-      // resourceVersion) sequence changed, and the list is sent when its bits did (or the node joined: an inserted node
-      // brings its list). After a failed List that half stays as it is.
+      // the node's list, validation pods first, then wait-selector pods, then workload pods: each part is rebuilt when its
+      // (pod, resourceVersion) sequence changed, and the list is sent when its bits did (or the node joined: an inserted
+      // node brings its list). After a failed List that part stays as it is.
       const bool joinedNode = !joined.empty() && joined[i];
       auto refresh = [&](const PodsByNode& by, std::string* sigStore, uint16_t (*flagsOf)(const Pod&), std::vector<uint16_t>* half) {
         const std::vector<const Pod*>* pods = podsOf(by, n.Name);
@@ -1355,20 +1588,56 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
         return true;
       };
       std::vector<uint16_t>& list = k.lists[i];
-      std::vector<uint16_t> vhalf, whalf;
+      std::vector<uint16_t> vhalf, whalf, ahalf;
       const bool newV = val && !listErr && refresh(byNode, &k.listSig[i], validationPodFlags, &vhalf);
       const bool newW = wait && !waitListErr && refresh(waitByNode, &k.waitSig[i], waitPodFlags, &whalf);
-      if (newV || newW) {
-        if (!newV) vhalf.assign(list.begin(), list.begin() + k.nval[i]);
-        if (!newW) whalf.assign(list.begin() + k.nval[i], list.end());
-        const int32_t nv = (int32_t)vhalf.size();
+      // the workload part: every pod of a pod-deletion-required or drain-required node, nothing for any other node. Its
+      // bits also depend on whether the DaemonSet each pod's controller names exists, and on the policy; after a failed
+      // drain-selector List the part is rebuilt (its drain bits unknown: that pass returns the error) and again next time.
+      const bool workNode = evict && (code == UST_STATE_POD_DELETION_REQUIRED || code == UST_STATE_DRAIN_REQUIRED);
+      const std::vector<const Pod*>* work = workNode && !evictListErr ? podsOf(wl.byNode, n.Name) : nullptr;
+      bool newA = false;
+      if (evict && !evictListErr) {
+        std::string asig = workNode ? workPolicy : std::string();
+        bool aversioned = !wl.selectorError;
+        if (work)
+          for (const Pod* p : *work) {
+            aversioned = aversioned && !p->ResourceVersion.empty();
+            const OwnerReference* c = controllerOf(*p);
+            const bool dsMissing = c && c->Kind == "DaemonSet" && !wl.daemonSets.count(p->Namespace + "/" + c->Name);
+            asig += p->Namespace + "/" + p->Name + "@" + p->ResourceVersion + (dsMissing ? "!;" : ";");
+          }
+        if (!aversioned || asig != k.workSig[i]) {
+          newA = true;
+          if (work)
+            for (const Pod* p : *work) ahalf.push_back(workloadPodFlags(*p, wl));
+          k.workSig[i] = aversioned ? asig : std::string("\x01");
+        }
+      }
+      if (newV || newW || newA) {
+        const size_t nv0 = (size_t)k.nval[i], na0 = (size_t)k.nwork[i];
+        if (!newV) vhalf.assign(list.begin(), list.begin() + nv0);
+        if (!newW) whalf.assign(list.begin() + nv0, list.end() - na0);
+        if (!newA) ahalf.assign(list.end() - na0, list.end());
+        const int32_t nv = (int32_t)vhalf.size(), na = (int32_t)ahalf.size();
         vhalf.insert(vhalf.end(), whalf.begin(), whalf.end());
+        vhalf.insert(vhalf.end(), ahalf.begin(), ahalf.end());
         if (vhalf != list) { list.swap(vhalf); sendList[i] = 1; }
         k.nval[i] = nv;
+        k.nwork[i] = na;
       }
       if (joinedNode) sendList[i] = 1;
       if (val && code == UST_STATE_VALIDATION_REQUIRED) stats_.validate_avoided++;
       if (wait && code == UST_STATE_WAIT_FOR_JOBS_REQUIRED) stats_.wait_avoided++;
+      if ((code == UST_STATE_POD_DELETION_REQUIRED && evictPodDeletion(*upgradePolicy)) ||
+          (code == UST_STATE_DRAIN_REQUIRED && evictDrain(*upgradePolicy)))
+        stats_.evict_lists_avoided++;
+      // Replay reads the node's workload pods beside the bits the device holds for them: the same sequence of pods
+      if (work && work->size() == (size_t)k.nwork[i]) {
+        EncodedSnapshot::Workload& wk = view.workload[view.entries.size()];
+        wk.pods = *work;
+        wk.bits.assign(list.end() - k.nwork[i], list.end());
+      }
     }
     if (!slotOfView.empty() && (int)(view.state.back() & UST_HOT_STATE_MASK) == code && slotOfView.back() > i)
       orderBroken = true;  // within a bucket, slot order must be the slice order: slots are handed out in it
@@ -1432,7 +1701,7 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
     if (dev) outcome[v] = k.outcome[i];
     if (wait && (view.state[v] & UST_HOT_STATE_MASK) == UST_STATE_WAIT_FOR_JOBS_REQUIRED) {
       const std::vector<uint16_t>& l = k.lists[i];  // the list the device holds for the node
-      view.waitRunning[v] = anyWaitRunning(l.data() + k.nval[i], l.data() + l.size());
+      view.waitRunning[v] = anyWaitRunning(l.data() + k.nval[i], l.data() + l.size() - k.nwork[i]);
     }
     if (!k.deferredMsg[i].empty()) view.deferred[v] = k.deferredMsg[i];
     if (last_.error_index == (int64_t)i) c.error_index = (int64_t)v;

@@ -15,13 +15,18 @@
 // ust_apply_state (H100 kernel) and replays the returned per-node action bitmasks through the actuator interfaces
 // in the reference's pass order. Without libust.so / a H100 every ApplyState returns an error.
 #pragma once
+#include <condition_variable>
 #include <cstdint>
 #include <ctime>
+#include <deque>
 #include <functional>
 #include <map>
 #include <memory>
+#include <mutex>
 #include <optional>
+#include <set>
 #include <string>
+#include <thread>
 #include <unordered_map>
 #include <vector>
 
@@ -71,7 +76,7 @@ struct Node {
   std::vector<NodeCondition> Conditions;  // Status.Conditions
 };
 struct ContainerStatus { bool Ready = false; int RestartCount = 0; };
-struct OwnerReference { std::string Kind, Name, UID; };
+struct OwnerReference { std::string Kind, Name, UID; bool Controller = false; };  // Controller: *Controller == true
 struct Pod {
   std::string Name, Namespace, NodeName;  // Spec.NodeName
   std::string ResourceVersion;
@@ -80,6 +85,8 @@ struct Pod {
   std::string Phase;                      // Status.Phase
   std::vector<ContainerStatus> ContainerStatuses, InitContainerStatuses;
   bool DeletionTimestampSet = false;      // !DeletionTimestamp.IsZero()
+  StringMap Annotations;
+  bool HasEmptyDirVolume = false;         // a Spec.Volumes entry with EmptyDir != nil
 };
 struct DaemonSet {
   std::string Name, Namespace, UID;
@@ -164,6 +171,16 @@ struct PodManager {
   virtual Error GetPodControllerRevisionHash(const Pod* pod, std::string* hash) = 0;
   virtual Error GetDaemonsetControllerRevisionHash(const DaemonSet* daemonset, std::string* hash) = 0;
 };
+// The options of the kubectl drain.Helper that deletes or evicts a node's pods (pod_manager.go:146-157,
+// drain_manager.go:76-96): Force, DeleteEmptyDirData, Timeout and GracePeriodSeconds.
+struct EvictionOptions { bool Force = false, DeleteEmptyDir = false; int TimeoutSecond = 0; int GracePeriodSeconds = -1; };
+// Not in the reference: the side effect of a pod-deletion or drain goroutine, drain.Helper.DeleteOrEvictPods(pods), which
+// StateOptions::EvictionOnDevice calls on a mirror-owned worker thread. `node` is the worker's copy of the node; `pods` are
+// copies of the pods to delete, in the List's order. Called concurrently for different nodes.
+struct PodEvictor {
+  virtual ~PodEvictor() = default;
+  virtual Error DeleteOrEvictPods(const Node& node, const std::vector<Pod*>& pods, const EvictionOptions& o) = 0;
+};
 struct ValidationManager {
   virtual ~ValidationManager() = default;
   virtual Error Validate(Node* node, bool* done) = 0;
@@ -212,9 +229,21 @@ struct StateOptions {                                                 // upgrade
   // make one K8sClient::ListPodsBySelector per reconcile for that selector, hand every node its wait-selector pods (after
   // its validation pods when ValidateOnDevice is on too) and its parsed wait-for-pod-completion start-time annotation to
   // the clocked pod-list calls, and replay the annotation and state calls the check would have made; the injected
-  // PodManager is never asked to check. Eviction, drain and pod restarts still go to the injected managers. Without a
-  // selector the wait-for-jobs pass moves its nodes on by itself and the option changes nothing.
+  // PodManager is never asked to check. Eviction and drain go to the injected managers unless EvictionOnDevice is on too;
+  // pod restarts always do. Without a selector the wait-for-jobs pass moves its nodes on by itself and the option changes
+  // nothing.
   bool WaitForCompletionOnDevice = false;
+  // Not in the reference: decide PodManager::SchedulePodEviction (with WithPodDeletionEnabled and policy.PodDeletion) and
+  // DrainManager::ScheduleNodesDrain (with policy.DrainSpec->Enable) on the device (UST_EVAL_ACTUATORS) instead of calling
+  // them. ApplyState and ApplyStateIncremental make one K8sClient::ListPodsBySelector("", "") per reconcile (a second one
+  // for a non-empty DrainSpec.PodSelector) and one ListDaemonSets, hand every pod-deletion-required and drain-required node
+  // its pods with the kubectl filter chain's inputs (after its validation and wait pods), and replay the state changes the
+  // goroutines would make from the device's actuator_outcome. Deleting or evicting pods, and the drain's cordon, run on
+  // mirror-owned worker threads through the injected PodEvictor and CordonManager; a node being worked on is skipped as the
+  // reference skips it. The injected PodManager then only restarts driver pods and looks up revision hashes. The workers
+  // call the PodEvictor, the CordonManager and the NodeUpgradeStateProvider while the reconcile (and the next ones) make
+  // their own calls, as the reference's goroutines do: those three must be safe to call concurrently.
+  bool EvictionOnDevice = false;
   // The reconcile's time.Now().Unix(): read once per ApplyState call; the device derives the validation and
   // wait-for-completion timeouts from it, and a new start-time annotation of either kind is set to it.
   std::function<int64_t()> Now = [] { return (int64_t)time(nullptr); };
@@ -245,6 +274,14 @@ struct EncodedSnapshot {
   bool waitOnDevice = false;
   std::vector<char> waitRunning;
   Error waitListError;
+  // StateOptions::EvictionOnDevice: a pod-deletion-required or drain-required entry's workload pods follow its wait pods in
+  // pod_off / pod_flags; here, by entry index, the same pods (the List's objects) beside their bits, which Replay reads to
+  // tell "nothing to delete" apart and to pick the pods to evict. The error of the pod or DaemonSet List, returned at the
+  // pod-deletion pass when it has nodes; and that error or the drain-selector List's, returned at the drain pass.
+  struct Workload { std::vector<const Pod*> pods; std::vector<uint16_t> bits; };
+  bool evictOnDevice = false;
+  std::unordered_map<size_t, Workload> workload;
+  Error evictListError, drainListError;
 };
 
 // ---- common_manager.go:23-41 --------------------------------------------------------------------------------
@@ -280,6 +317,7 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
   upgrade::NodeUpgradeStateProvider* NodeUpgradeStateProvider = nullptr;
   upgrade::ValidationManager* ValidationManager = nullptr;
   upgrade::SafeDriverLoadManager* SafeDriverLoadManager = nullptr;
+  upgrade::PodEvictor* PodEvictor = nullptr;  // StateOptions::EvictionOnDevice only
 
   // NewClusterUpgradeStateManager (upgrade_state.go:65-92): binds CUDA device `device` through ust_create
   static Error New(int device, StateOptions opts, std::unique_ptr<ClusterUpgradeStateManagerImpl>* out);
@@ -312,7 +350,8 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
   // The two halves of ApplyState around the kernel call. Public so that they can be audited separately:
   // Encode evaluates every reference predicate once and fills the struct-of-arrays; Replay performs the calls
   // named by the action bits, in the reference's pass order, stopping at the first error. `actuator_outcome` is read
-  // only for the wait-for-jobs pass of an enc.waitOnDevice snapshot, which needs it.
+  // only for the wait-for-jobs pass of an enc.waitOnDevice snapshot and the pod-deletion and drain passes of an
+  // enc.evictOnDevice one, which need it.
   Error Encode(const ClusterUpgradeState& s, const DriverUpgradePolicySpec& policy, EncodedSnapshot* out);
   Error Replay(const EncodedSnapshot& enc, const DriverUpgradePolicySpec& policy, const uint8_t* next_state,
                const uint16_t* actions, int abi_rc, const ust_counters& counters, const uint8_t* actuator_outcome = nullptr);
@@ -346,6 +385,9 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
     // that sent no node and no list (only time passed), the ValidationManager::Validate calls (one API List each) not made,
     // and the per-node Lists of PodManager::ScheduleCheckOnPodCompletion not made (one per wait-for-jobs-required node)
     int64_t lists_sent = 0, lists_reused = 0, time_only = 0, validate_avoided = 0, wait_avoided = 0;
+    // StateOptions::EvictionOnDevice: the per-node pod Lists not made (one per pod-deletion-required or drain-required node
+    // of a pass the option answers), and the nodes handed to the PodEvictor's workers (by Replay, in either ApplyState)
+    int64_t evict_lists_avoided = 0, actuator_handoffs = 0;
   };
   const IncrementalStats& Stats() const { return stats_; }
   void ResetIncremental();
@@ -353,6 +395,11 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
   void SetValidateOnDevice(bool on) { opts_.ValidateOnDevice = on; }
   // Switches StateOptions::WaitForCompletionOnDevice, with the same effect on the incremental cache.
   void SetWaitForCompletionOnDevice(bool on) { opts_.WaitForCompletionOnDevice = on; }
+  // Switches StateOptions::EvictionOnDevice, with the same effect on the incremental cache.
+  void SetEvictionOnDevice(bool on) { opts_.EvictionOnDevice = on; }
+  // Blocks until every eviction and drain handed to the workers has ended (their state changes made). The destructor
+  // waits too.
+  void WaitForActuators();
 
   // ---- incremental BuildState: the driver-pod list stays on the device (ust_build_state_delta) -----------------------------
   // The same contract, result and errors as BuildState, for a reconcile loop that calls it again and again. The manager keeps
@@ -442,6 +489,11 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
     std::vector<int32_t> nval;
     std::vector<std::string> waitSig;
     std::vector<uint8_t> outcome;
+    // With EvictionOnDevice the list ends with the node's workload pods (the last nwork entries; none unless the node is
+    // pod-deletion-required or drain-required), built from the (pod, resourceVersion, DaemonSet found) sequence workSig.
+    bool evict = false;
+    std::vector<int32_t> nwork;
+    std::vector<std::string> workSig;
   };
   virtual int EvaluateCached(const ust_policy& policy, bool full, const std::vector<int64_t>& changed, Cache* cache, ust_counters* c);
   // The same on the clocked pod-list snapshot (StateOptions::ValidateOnDevice / WaitForCompletionOnDevice): full:
@@ -461,6 +513,12 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
   bool waitOnDevice(const DriverUpgradePolicySpec& p) const {
     return opts_.WaitForCompletionOnDevice && p.WaitForCompletion && !p.WaitForCompletion->PodSelector.empty();
   }
+  // StateOptions::EvictionOnDevice: the pod-deletion pass / the drain pass it answers, and whether it answers either
+  bool evictPodDeletion(const DriverUpgradePolicySpec& p) const { return opts_.EvictionOnDevice && podDeletionStateEnabled_ && p.PodDeletion; }
+  bool evictDrain(const DriverUpgradePolicySpec& p) const { return opts_.EvictionOnDevice && p.DrainSpec && p.DrainSpec->Enable; }
+  bool evictOnDevice(const DriverUpgradePolicySpec& p) const { return evictPodDeletion(p) || evictDrain(p); }
+  // Runs `job` on a worker thread; `name` stays in `*dedupe` until the job has ended.
+  void handOff(std::set<std::string>* dedupe, const std::string& name, std::function<void()> job);
   Error assembleState(const std::vector<Pod*>& podList, const uint8_t* podState, const int32_t* owner_idx,
                       std::map<std::string, DaemonSet*>& daemonSets, std::unique_ptr<ClusterUpgradeState>* out);
   Cache cache_;
@@ -473,6 +531,16 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
   PodDeletionFilter filter_;
   std::string validationSelector_;
   ust_counters last_{};
+  // The PodEvictor's workers: a queue served by up to kActuatorWorkers threads, and the reference's two dedupe sets
+  // (pod_manager.go:160-165, drain_manager.go:104-110), guarded by actMu_.
+  static constexpr size_t kActuatorWorkers = 16;
+  std::mutex actMu_;
+  std::condition_variable actCv_;
+  std::deque<std::function<void()>> actQueue_;
+  std::vector<std::thread> actThreads_;
+  size_t actIdle_ = 0, actRunning_ = 0;
+  bool actStop_ = false;
+  std::set<std::string> nodesInProgress_, drainingNodes_;
 };
 
 const char* StateNameOfCode(unsigned code);  // "" for unknown; nullptr for codes without a label
