@@ -50,9 +50,10 @@ def build_host(force=False):
 
 def build_host_tests(root):
     """tests/host/_build/{upgrade_state_test,host_logic_test,membership_test,reorder_test,build_state_test,validation_test,
-    wait_test,eviction_test}: the reference's specs against the mirror, the incremental path under membership changes and nodes
-    that move in the list, the incremental BuildState + ApplyState loop, and ValidationManager.Validate,
-    PodManager.ScheduleCheckOnPodCompletion, SchedulePodEviction and DrainManager.ScheduleNodesDrain answered on the device."""
+    wait_test,eviction_test,events_test}: the reference's specs against the mirror, the incremental path under membership changes
+    and nodes that move in the list, the incremental BuildState + ApplyState loop, ValidationManager.Validate,
+    PodManager.ScheduleCheckOnPodCompletion, SchedulePodEviction and DrainManager.ScheduleNodesDrain answered on the device, and
+    the events those managers record."""
     tdir = os.path.join(root, "tests", "host")
     bdir = os.path.join(tdir, "_build")
     os.makedirs(bdir, exist_ok=True)
@@ -63,7 +64,7 @@ def build_host_tests(root):
     oracle = ["-L" + os.path.join(root, "oracle"), "-lust_oracle", "-Wl,-rpath," + os.path.join(root, "oracle")]
     for name, extra in (("upgrade_state_test", []), ("host_logic_test", oracle), ("membership_test", oracle),
                         ("reorder_test", oracle), ("build_state_test", oracle), ("validation_test", []), ("wait_test", []),
-                        ("eviction_test", ["-pthread"])):
+                        ("eviction_test", ["-pthread"]), ("events_test", ["-pthread"])):
         exe = os.path.join(bdir, name)
         if not os.path.exists(exe) or any(os.path.getmtime(x) > os.path.getmtime(exe) for x in srcs):
             subprocess.check_call(common + [os.path.join(tdir, name + ".cpp"), "-o", exe] + link + extra)

@@ -318,18 +318,30 @@ static inline uint32_t ust_lut_lookup(const uint32_t* lut, unsigned s, uint32_t 
 #define UST_PODSUM_CANNOT_DELETE 0x04u /* ... but the base filter chain keeps it */
 #define UST_PODSUM_DRAIN_ERROR 0x08u
 
-static inline bool ust_pod_chain_keeps(unsigned pf, bool force, bool delete_emptydir, bool* is_error) {
+// Which filter of the chain stopped a pod (ust_pod_chain_keeps's `stop`): none, or the filter and whether it is an error.
+#define UST_CHAIN_NONE 0u
+#define UST_CHAIN_DAEMONSET 1u      /* daemonSetFilter: skipped with a warning (IgnoreAllDaemonSets) */
+#define UST_CHAIN_DS_MISSING 2u     /* daemonSetFilter: an error, its DaemonSet is NotFound and there is no force */
+#define UST_CHAIN_MIRROR 3u         /* mirrorPodFilter: skipped */
+#define UST_CHAIN_LOCAL_STORAGE 4u  /* localStorageFilter: an error */
+#define UST_CHAIN_UNREPLICATED 5u   /* unreplicatedFilter: an error */
+
+static inline bool ust_pod_chain_keeps(unsigned pf, bool force, bool delete_emptydir, bool* is_error, unsigned* stop = nullptr) {
   const unsigned phase = pf & UST_POD_PHASE_MASK;
   const bool finished = phase == UST_PHASE_SUCCEEDED || phase == UST_PHASE_FAILED;
-  *is_error = false;
+  unsigned s = UST_CHAIN_NONE;
   if ((pf & UST_POD_HAS_CONTROLLER) && (pf & UST_POD_CONTROLLED_BY_DS) && !finished) {
-    if (pf & UST_POD_DS_MISSING) { if (!force) { *is_error = true; return true; } }
-    else return true;  // skipped with a warning (IgnoreAllDaemonSets)
+    if (pf & UST_POD_DS_MISSING) { if (!force) s = UST_CHAIN_DS_MISSING; }
+    else s = UST_CHAIN_DAEMONSET;
   }
-  if (pf & UST_POD_MIRROR) return true;
-  if ((pf & UST_POD_HAS_EMPTYDIR) && !finished && !delete_emptydir) { *is_error = true; return true; }
-  if (!finished && !(pf & UST_POD_HAS_CONTROLLER) && !force) { *is_error = true; return true; }
-  return false;
+  if (s == UST_CHAIN_NONE) {
+    if (pf & UST_POD_MIRROR) s = UST_CHAIN_MIRROR;
+    else if ((pf & UST_POD_HAS_EMPTYDIR) && !finished && !delete_emptydir) s = UST_CHAIN_LOCAL_STORAGE;
+    else if (!finished && !(pf & UST_POD_HAS_CONTROLLER) && !force) s = UST_CHAIN_UNREPLICATED;
+  }
+  *is_error = s == UST_CHAIN_DS_MISSING || s == UST_CHAIN_LOCAL_STORAGE || s == UST_CHAIN_UNREPLICATED;
+  if (stop) *stop = s;
+  return s != UST_CHAIN_NONE;
 }
 
 static inline void ust_build_pod_lut(const ust_policy* p, uint8_t* podlut) {

@@ -29,6 +29,7 @@ const char* const PodControllerRevisionHashLabelKey = "controller-revision-hash"
 
 static const char* const kNullString = "null";  // consts.go:90
 static const char* const kTrueString = "true";  // consts.go:92
+static const char* const kDrainInsteadMessage = "Pod deletion failed but drain is enabled in spec. Will attempt a node drain";  // pod_manager.go:396-399
 static std::string g_driver_name;                 // util.go:91-99
 
 // The eight keys are functions of the driver name only (util.go:101-133). The reference formats them on every use; an
@@ -63,6 +64,15 @@ std::string GetUpgradeRequestorModeAnnotationKey() { return keys().requestorMode
 std::string GetUpgradeInitialStateAnnotationKey() { return keys().initialState; }
 std::string GetWaitForPodCompletionStartTimeAnnotationKey() { return keys().waitStart; }
 std::string GetValidationStartTimeAnnotationKey() { return keys().validationStart; }
+std::string GetEventReason() {
+  std::string s = g_driver_name;
+  for (char& c : s)
+    if (c >= 'a' && c <= 'z') c = (char)(c - 'a' + 'A');
+  return s + "DriverUpgrade";
+}
+
+const char* const EventTypeNormal = "Normal";
+const char* const EventTypeWarning = "Warning";
 
 bool IsOrphanedPod(const Pod& pod) { return pod.OwnerReferences.empty(); }
 bool IsNodeInRequestorMode(const Node& node) { return node.Annotations.count(keys().requestorMode) != 0; }
@@ -611,6 +621,36 @@ static const OwnerReference* controllerOf(const Pod& p) {
   return nullptr;
 }
 static const char* const kMirrorPodAnnotationKey = "kubernetes.io/config.mirror";  // corev1.MirrorPodAnnotationKey
+
+// The text of kubectl's drain errors: the filters' fatal messages (k8s.io/kubectl v0.35.1 pkg/drain/filters.go:
+// localStorageFatal, unmanagedFatal; daemonSetFilter returns the Get's error, the API's NotFound text), PodDeleteList.errors
+// (drain.go: "cannot delete <message>: <ns/name, ...>" per distinct message) and utilerrors.NewAggregate's Error
+// (k8s.io/apimachinery pkg/util/errors: one error prints itself, several print "[a, b]"). Restated from upstream, not
+// pinned by the reference's tests. Upstream groups the pods in a Go map, so its message order varies from run to run;
+// here the messages come in the order of their first pod in the List, and each message's pods in List order.
+Error DrainFilterError(const std::vector<const Pod*>& pods, const std::vector<uint16_t>& bits, const DrainSpec& spec) {
+  std::vector<std::pair<std::string, std::string>> failed;  // message, its pods
+  for (size_t j = 0; j < pods.size() && j < bits.size(); j++) {
+    bool isError = false;
+    unsigned stop = UST_CHAIN_NONE;
+    if (!(bits[j] & UST_POD_MATCH_DRAIN_SELECTOR)) continue;
+    ust_pod_chain_keeps(bits[j], spec.Force, spec.DeleteEmptyDir, &isError, &stop);
+    if (!isError) continue;
+    const Pod& p = *pods[j];
+    std::string msg;
+    if (stop == UST_CHAIN_DS_MISSING) msg = "daemonsets.apps \"" + controllerOf(p)->Name + "\" not found";
+    else if (stop == UST_CHAIN_LOCAL_STORAGE) msg = "Pods with local storage (use --delete-emptydir-data to override)";
+    else msg = "Pods declare no controller (use --force to override)";
+    auto it = std::find_if(failed.begin(), failed.end(), [&](const auto& f) { return f.first == msg; });
+    if (it == failed.end()) it = failed.insert(failed.end(), {msg, ""});
+    else it->second += ", ";
+    it->second += p.Namespace + "/" + p.Name;
+  }
+  if (failed.empty()) return std::nullopt;
+  std::string s;
+  for (const auto& f : failed) s += (s.empty() ? "" : ", ") + ("cannot delete " + f.first + ": " + f.second);
+  return Errorf(failed.size() == 1 ? s : "[" + s + "]");
+}
 // What the workload entries of one reconcile are derived from: every pod by node (ListPodsBySelector("", "")), the pods
 // the drain's PodSelector matches (a second List, only for a non-empty selector: the mirror matches no label selector
 // itself) and every DaemonSet (ListDaemonSets), keyed by Namespace/Name.
@@ -930,6 +970,17 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
   auto setState = [&](size_t i) { return NodeUpgradeStateProvider->ChangeNodeUpgradeState(enc.entries[i]->Node, StateNameOfCode(next_state[i])); };
   auto anno = [&](size_t i, const std::string& k, const char* v) { return NodeUpgradeStateProvider->ChangeNodeUpgradeAnnotation(enc.entries[i]->Node, k, v); };
   auto validationError = [](const Error& e) { return Errorf("unable to handle timeout for validation state: " + *e); };  // :97-101
+  // The events of the managers an option replaces (logEvent / logEventf, util.go:162-176). Workers take `recorder` and
+  // `reason` by value.
+  upgrade::EventRecorder* const recorder = EventRecorder;
+  const std::string reason = recorder ? GetEventReason() : std::string();
+  auto event = [recorder, reason](const Node& n, const char* type, const std::string& message) {
+    if (recorder) recorder->Event(n, type, reason, message);
+  };
+  // validation_manager.go:97-101 passes err.Error() to a format without a verb: Go appends it as %!(EXTRA string=...)
+  auto validationEvent = [&](const Node& n, const std::string& err) {
+    event(n, EventTypeWarning, "Failed to handle timeout for validation state%!(EXTRA string=" + err + ")");
+  };
   auto abortError = [&](long long idx = -1) -> Error {
     if (idx >= 0) { auto it = enc.deferred.find((size_t)idx); if (it != enc.deferred.end()) return Errorf(it->second); }
     return Errorf(ust_last_error(handle_));
@@ -964,17 +1015,23 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
       if (onDevice) {
         // the calls Validate makes (validation_manager.go:71-175), as the device answered it
         if (enc.listError) return enc.listError;  // its List failed (:79-83)
-        if (a & UST_A_ERROR) return abortError((long long)i);  // the start time does not parse (:155-160)
         const std::string& key = GetValidationStartTimeAnnotationKey();
+        if (a & UST_A_ERROR) {  // the start time does not parse (:155-160)
+          auto it = node->Annotations.find(key);
+          int64_t start = 0;
+          std::string err;
+          if (it != node->Annotations.end() && !parseInt64(it->second, &start, &err)) validationEvent(*node, err);
+          return abortError((long long)i);
+        }
         if (next_state[i] == UST_STATE_FAILED) {  // handleTimeout: timed out (:161-172)
           (void)NodeUpgradeStateProvider->ChangeNodeUpgradeState(node, UpgradeStateFailed);  // error ignored (:163)
-          if (Error e = anno(i, key, kNullString)) return validationError(e);
+          if (Error e = anno(i, key, kNullString)) { validationEvent(*node, *e); return validationError(e); }
           continue;
         }
         if (a & UST_A_CLEAR_WAIT_START)  // a ready pod (:106-113)
           if (Error e = anno(i, key, kNullString)) return e;
         if (a & UST_A_SET_WAIT_START)    // handleTimeout: no start time yet (:143-152)
-          if (Error e = anno(i, key, std::to_string(enc.now).c_str())) return validationError(e);
+          if (Error e = anno(i, key, std::to_string(enc.now).c_str())) { validationEvent(*node, *e); return validationError(e); }
         if (!(a & UST_A_SET_STATE)) continue;  // "Validations not complete on the node"
       } else if (code == UST_STATE_VALIDATION_REQUIRED) {
         bool done = false;
@@ -1008,21 +1065,32 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
           for (size_t k = begin; k < i; k++) {
             if (!(actions[k] & UST_A_SCHEDULE_WAIT_CHECK)) continue;
             // The reference checks each node in a goroutine that took the node by value (go func(node corev1.Node), :275):
-            // its calls get a copy, so that they do not write to the caller's snapshot object. Every error is logged as an
+            // its calls get a copy, so that they do not write to the caller's snapshot object. Every error is recorded as an
             // event and dropped there (:290-312).
             Node node = *enc.entries[k]->Node;
+            auto timeoutEvent = [&](const std::string& err) {  // :290-296
+              event(node, EventTypeWarning, "Failed to handle timeout for job completions, " + err);
+            };
             if (actuator_outcome[k] == UST_STATE_POD_DELETION_REQUIRED) {
               if (!enc.waitRunning[k]) {  // no wait pod Running or Pending: delete the start time, then the state (:300-309)
-                if (!NodeUpgradeStateProvider->ChangeNodeUpgradeAnnotation(&node, key, kNullString))
+                if (Error e = NodeUpgradeStateProvider->ChangeNodeUpgradeAnnotation(&node, key, kNullString))
+                  event(node, EventTypeWarning, "Failed to remove annotation used to track job completions: " + *e);
+                else
                   (void)NodeUpgradeStateProvider->ChangeNodeUpgradeState(&node, UpgradeStatePodDeletionRequired);
               } else {  // still running, timed out: the state, then the start time (HandleTimeoutOnPodCompletions :354-365)
                 (void)NodeUpgradeStateProvider->ChangeNodeUpgradeState(&node, UpgradeStatePodDeletionRequired);
-                (void)NodeUpgradeStateProvider->ChangeNodeUpgradeAnnotation(&node, key, kNullString);
+                if (Error e = NodeUpgradeStateProvider->ChangeNodeUpgradeAnnotation(&node, key, kNullString)) timeoutEvent(*e);
               }
             } else if (actions[k] & UST_A_SET_WAIT_START) {  // running, no start time yet (:336-345)
-              (void)NodeUpgradeStateProvider->ChangeNodeUpgradeAnnotation(&node, key, std::to_string(enc.now));
+              if (Error e = NodeUpgradeStateProvider->ChangeNodeUpgradeAnnotation(&node, key, std::to_string(enc.now))) timeoutEvent(*e);
+            } else if (enc.waitRunning[k] && waitSelector && policy.WaitForCompletion->TimeoutSecond != 0) {
+              // still waiting, or the start time does not parse (:348-353): only the latter has an event
+              auto it = node.Annotations.find(key);
+              int64_t start = 0;
+              std::string err;
+              if (it != node.Annotations.end() && !parseInt64(it->second, &start, &err)) timeoutEvent(err);
             }
-            // otherwise still waiting, or the start time does not parse (:348-353), or no timeout: no call
+            // otherwise no timeout: no call
           }
         } else if (waitSelector && !batchNodes.empty()) {  // common_manager.go:404-418
           PodManagerConfig cfg;
@@ -1057,6 +1125,7 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
                 if (w->second.bits[j] & UST_POD_MATCH_DELETION_FILTER) toDelete.push_back(*w->second.pods[j]);
             const uint8_t out = actuator_outcome[k];
             if (out == UST_STATE_DRAIN_REQUIRED || out == UST_STATE_FAILED) {  // updateNodeToDrainOrFailed (:194-201, :393-403)
+              if (drainEnabled) event(node, EventTypeWarning, kDrainInsteadMessage);
               (void)NodeUpgradeStateProvider->ChangeNodeUpgradeState(&node, StateNameOfCode(out));
             } else if (out != UST_STATE_POD_RESTART_REQUIRED) {
               return Errorf("Replay: no pod-deletion outcome for node " + name);
@@ -1068,12 +1137,18 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
               upgrade::NodeUpgradeStateProvider* provider = NodeUpgradeStateProvider;
               upgrade::PodEvictor* evictor = PodEvictor;
               stats_.actuator_handoffs++;
-              handOff(&nodesInProgress_, name, [provider, evictor, node, pods = std::move(toDelete), o, drainEnabled]() mutable {
+              handOff(&nodesInProgress_, name, [provider, evictor, node, pods = std::move(toDelete), o, drainEnabled, event]() mutable {
                 std::vector<Pod*> ptrs;
                 for (Pod& p : pods) ptrs.push_back(&p);
                 const Error err = evictor ? evictor->DeleteOrEvictPods(node, ptrs, o) : Errorf("no PodEvictor");
-                (void)provider->ChangeNodeUpgradeState(&node, !err ? UpgradeStatePodRestartRequired
-                                                                   : drainEnabled ? UpgradeStateDrainRequired : UpgradeStateFailed);
+                if (err) {
+                  event(node, EventTypeWarning, "Failed to delete workload pods on the node for the driver upgrade, " + *err);
+                  if (drainEnabled) event(node, EventTypeWarning, kDrainInsteadMessage);
+                  (void)provider->ChangeNodeUpgradeState(&node, drainEnabled ? UpgradeStateDrainRequired : UpgradeStateFailed);
+                } else {
+                  (void)provider->ChangeNodeUpgradeState(&node, UpgradeStatePodRestartRequired);
+                  event(node, EventTypeNormal, "Deleted workload pods on the node for the driver upgrade");
+                }
               });
             }
           }
@@ -1112,27 +1187,39 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
                 if ((b & UST_POD_MATCH_DRAIN_SELECTOR) && !ust_pod_chain_keeps(b, spec.Force, spec.DeleteEmptyDir, &isError))
                   toEvict.push_back(*w->second.pods[j]);
               }
+            // GetPodsForDeletion's errors (:121-128), as RunNodeDrain returns them
+            Error filterError;
+            if (out == UST_STATE_FAILED) {
+              if (w != enc.workload.end()) filterError = DrainFilterError(w->second.pods, w->second.bits, spec);
+              if (!filterError) filterError = Errorf("the drain filter chain reports an error");
+            }
             EvictionOptions o;
             o.Force = spec.Force; o.DeleteEmptyDir = spec.DeleteEmptyDir; o.TimeoutSecond = spec.TimeoutSecond;
             upgrade::NodeUpgradeStateProvider* provider = NodeUpgradeStateProvider;
             upgrade::CordonManager* cordon = CordonManager;
             upgrade::PodEvictor* evictor = PodEvictor;
             stats_.actuator_handoffs++;
+            event(*enc.entries[k]->Node, EventTypeNormal, "Scheduling drain of the node");  // :104-107
             Node node = *enc.entries[k]->Node;  // the worker's copy: it outlives this call
-            handOff(&drainingNodes_, name, [provider, cordon, evictor, node, pods = std::move(toEvict), o, out]() mutable {
-              if (cordon->Cordon(&node)) {  // drain.RunCordonOrUncordon (:111-118)
+            handOff(&drainingNodes_, name, [provider, cordon, evictor, node, pods = std::move(toEvict), o, filterError, event]() mutable {
+              if (Error e = cordon->Cordon(&node)) {  // drain.RunCordonOrUncordon (:111-118)
                 (void)provider->ChangeNodeUpgradeState(&node, UpgradeStateFailed);
+                event(node, EventTypeWarning, "Failed to cordon the node, " + *e);
                 return;
               }
-              Error err;
-              if (out == UST_STATE_FAILED) {
-                err = Errorf("the drain filter chain reports an error");  // GetPodsForDeletion's errors (:121-128)
-              } else if (!pods.empty()) {  // DeleteOrEvictPods returns at once for no pods
+              Error err = filterError;
+              if (!err && !pods.empty()) {  // DeleteOrEvictPods returns at once for no pods
                 std::vector<Pod*> ptrs;
                 for (Pod& p : pods) ptrs.push_back(&p);
                 err = evictor ? evictor->DeleteOrEvictPods(node, ptrs, o) : Errorf("no PodEvictor");
               }
-              (void)provider->ChangeNodeUpgradeState(&node, err ? UpgradeStateFailed : UpgradeStatePodRestartRequired);  // :121-132
+              if (err) {  // :121-127
+                (void)provider->ChangeNodeUpgradeState(&node, UpgradeStateFailed);
+                event(node, EventTypeWarning, "Failed to drain the node, " + *err);
+              } else {    // :129-132
+                event(node, EventTypeNormal, "Successfully drained the node");
+                (void)provider->ChangeNodeUpgradeState(&node, UpgradeStatePodRestartRequired);
+              }
             });
           }
         } else if (drainEnabled) {  // common_manager.go:346-356 (called even with an empty node list)

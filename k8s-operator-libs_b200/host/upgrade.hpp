@@ -64,6 +64,9 @@ std::string GetUpgradeRequestorModeAnnotationKey();
 std::string GetUpgradeInitialStateAnnotationKey();
 std::string GetWaitForPodCompletionStartTimeAnnotationKey();
 std::string GetValidationStartTimeAnnotationKey();
+// util.go:158-160: strings.ToUpper(DriverName) + "DriverUpgrade", the reason of every event the managers record. Driver
+// names are ASCII (they are label-key prefixes), so ASCII upper-casing is Go's ToUpper here.
+std::string GetEventReason();
 
 // ---- the slice of corev1 / appsv1 the path reads --------------------------------------------------------
 using StringMap = std::map<std::string, std::string>;
@@ -181,6 +184,21 @@ struct PodEvictor {
   virtual ~PodEvictor() = default;
   virtual Error DeleteOrEvictPods(const Node& node, const std::vector<Pod*>& pods, const EvictionOptions& o) = 0;
 };
+// record.EventRecorder (k8s.io/client-go/tools/record), the slice the managers use: Event(object, eventtype, reason,
+// message) on a node. `message` is the final text, as fmt.Sprintf made it in the reference. The three on-device options
+// call it from the reconcile's thread and from the mirror's worker threads at once (as the reference's goroutines call
+// theirs): it must be safe to call concurrently.
+extern const char* const EventTypeNormal;   // corev1.EventTypeNormal
+extern const char* const EventTypeWarning;  // corev1.EventTypeWarning
+struct EventRecorder {
+  virtual ~EventRecorder() = default;
+  virtual void Event(const Node& object, const std::string& eventType, const std::string& reason, const std::string& message) = 0;
+};
+// The error kubectl's drain.RunNodeDrain returns before it evicts anything: utilerrors.NewAggregate over the errors of
+// GetPodsForDeletion, for a node's pods (the List's objects, in its order) with their UST_POD_* bits as Encode made them,
+// under `spec`'s Force and DeleteEmptyDir. Only pods with UST_POD_MATCH_DRAIN_SELECTOR take part. nullopt: no pod stops
+// the drain.
+Error DrainFilterError(const std::vector<const Pod*>& pods, const std::vector<uint16_t>& bits, const DrainSpec& spec);
 struct ValidationManager {
   virtual ~ValidationManager() = default;
   virtual Error Validate(Node* node, bool* done) = 0;
@@ -318,6 +336,10 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
   upgrade::ValidationManager* ValidationManager = nullptr;
   upgrade::SafeDriverLoadManager* SafeDriverLoadManager = nullptr;
   upgrade::PodEvictor* PodEvictor = nullptr;  // StateOptions::EvictionOnDevice only
+  // The manager's EventRecorder (common_manager.go:84-100, upgrade_state.go:65-92). The mirror records only the events of
+  // the managers an on-device option replaces (ValidateOnDevice, WaitForCompletionOnDevice, EvictionOnDevice), at the
+  // reference's points; the injected managers record their own. nullptr records nothing (util.go:162-176).
+  upgrade::EventRecorder* EventRecorder = nullptr;
 
   // NewClusterUpgradeStateManager (upgrade_state.go:65-92): binds CUDA device `device` through ust_create
   static Error New(int device, StateOptions opts, std::unique_ptr<ClusterUpgradeStateManagerImpl>* out);
