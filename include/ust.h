@@ -491,7 +491,9 @@ int ust_fetch_outputs_pods(ust_handle* h, uint8_t* next_state, uint16_t* actions
  *                           UST_F_VALIDATION_TIMED_OUT = 0
  *   validation-required     UST_F_VALIDATION_TIMED_OUT = now > start + UST_VALIDATION_TIMEOUT_SECONDS  (validation_manager.go:161)
  *                           UST_F_WAIT_TIMED_OUT       = 0
- * Input bits 18 and 27 are ignored by clocked calls (no other state reads them). */
+ * Input bits 18 and 27 are ignored by clocked calls (no other state reads them).
+ * Every clocked call also computes when a reconcile in which only time passes will next return something: see
+ * ust_next_deadline below. */
 #define UST_VALIDATION_TIMEOUT_SECONDS 600 /* validation_manager.go:32 */
 typedef struct ust_clock {
   int64_t now;                  /* time.Now().Unix() of this reconcile */
@@ -528,6 +530,28 @@ int ust_apply_state_delta_pods_clocked(ust_handle* h, const ust_policy* policy, 
                                        const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev,
                                        int64_t max_out, int64_t* out_idx, uint8_t* out_next_state, uint16_t* out_actions,
                                        uint8_t* out_outcome, int64_t* n_out, ust_counters* out);
+/* When the next time-only reconcile is worth running. Nothing changes in the API when a deadline passes, so no watch event
+ * tells a controller to reconcile then; this call does. After a clocked call at time `now`, *t receives the call's next
+ * deadline: the smallest t > now such that ust_apply_state_delta_pods_clocked at clock->now = t with nothing else
+ * (n_changed == 0, no lists, no reorder) on that snapshot returns a non-empty sparse output - at least one node whose
+ * next_state, actions or actuator_outcome differs from what the call at `now` returned. INT64_MIN when there is none
+ * (unambiguous: t > now >= INT64_MIN).
+ * Only bits 18 and 27 depend on the clock, and each on its own node. With d = start + timeout (wrapped as above), a node's
+ * bit turns on at d + 1, which can happen after `now` only when now <= d < INT64_MAX and its state's *_START_ANNO bit is
+ * set and *_START_INVALID clear. The value is the smallest d + 1 over the nodes for which that flip changes the node's own
+ * outputs, as the call evaluated it: its pod-list verdict (wait pods running, the validation walk) and the call's abort
+ * point included - e.g. the wait timeout matters only with wait_timeout_nonzero and a wait pod Running or Pending, the
+ * validation timeout only when the first matching pod is not ready and no ready pod precedes it, neither past an abort.
+ * Every clocked call computes it on the device: the clock kernel lists the candidate nodes, a kernel behind the
+ * verification kernel evaluates each a second time with its bit set and min-reduces d + 1. It is not copied back unless
+ * asked for: this call makes one 8-byte device-to-host copy on the handle's stream and changes nothing resident.
+ * A clock that later moves backwards is outside the definition: only t > now counts.
+ * UST_ERR_INVALID_ARGUMENT, with a message, when t is NULL, when no clocked pod-list snapshot is resident, or when the last
+ * ApplyState, BuildState or simulation call on the handle was not a clocked call that produced counters (UST_OK, a
+ * reference-level abort or UST_ERR_TRUNCATED: the calls that leave the snapshot resident) - e.g. a clocked call refused for
+ * its arguments. ust_sync, the fetches and this call itself do not count as calls here. One GPU: after ust_comm_init
+ * with more than one rank it returns UST_ERR_INVALID_ARGUMENT (a rank would know only its own shard's nodes). */
+int ust_next_deadline(ust_handle* h, int64_t* t);
 
 /* Rollout simulation (SURVEY 8f.3) on the resident snapshot (see ust_apply_state_delta): `steps` reconciles in a row,
  * entirely on the device. After each ApplyState the decisions are fed back into the snapshot under "ideal

@@ -228,6 +228,14 @@ struct ust_handle {
   // clocked pod-list calls: the start time of every node of the pod-list snapshot, the gather target of a reorder (swapped
   // with it afterwards), the starts of the changed and of the inserted nodes as uploaded. Only clocked calls allocate them.
   DevBuf<long long> s_start, s_start2, chg_start, ins_start;
+  // the next deadline of a clocked call (ust_next_deadline): the clock launch's geometry, its candidate list and per-CTA
+  // counts, the reduced value; deadline_ready: the last ApplyState, BuildState or simulation call on the handle was a clocked
+  // call that left its snapshot resident (set by adopt_resident, cleared by every such entry point)
+  UstClockGrid clk_grid = {0, 0};
+  DevBuf<uint32_t> clk_cand;
+  DevBuf<unsigned int> clk_count;
+  DevBuf<unsigned long long> clk_deadline;
+  bool deadline_ready = false;
   // the resident driver-pod list of ust_build_state_delta (bs_n pods, 0 until the first call; nothing else reads or drops
   // it): state bytes, owner UIDs and the owner indices of the last call in `bs`. `bs2` is the gather target of a reorder
   // (hot / uid allocated on the first reorder; swapped with `bs` afterwards); bs2.owner receives a call's owner indices
@@ -457,11 +465,15 @@ static int check_pod_offsets_host(ust_handle* h, int64_t n, const int32_t* pod_o
   return UST_OK;
 }
 
-// core: everything device-resident, enqueue on `st`
+static int launch_deadline(ust_handle* h, const UstParams& P, const ust_clock* clock, int validation, int64_t n_pods, cudaStream_t st);
+
+// core: everything device-resident, enqueue on `st`. `clock` (clocked calls, whose clock kernel has run): the call's next
+// deadline is evaluated behind the verification kernel.
 static int apply_device(ust_handle* h, const ust_policy* policy, int64_t n, const uint8_t* state, const uint32_t* flags,
                         const int32_t* pod_rev, const int32_t* ds_idx, int32_t n_ds, const int32_t* ds_rev,
                         const int32_t* pod_off, const uint16_t* pod_flags, int64_t n_pods, uint8_t* next_state,
-                        uint16_t* actions, uint8_t* outcome, ust_counters* out_dev, cudaStream_t st) {
+                        uint16_t* actions, uint8_t* outcome, ust_counters* out_dev, cudaStream_t st,
+                        const ust_clock* clock = nullptr) {
   const bool chain = h->chain_entry;  // called by ust_apply_state_device itself: the call may overlap the previous one
   h->chain_entry = false;
   if (!chain) h->prev_n = -1;
@@ -483,14 +495,14 @@ static int apply_device(ust_handle* h, const ust_policy* policy, int64_t n, cons
                       outcome, out_dev, st, &P, &grid);
   if (rc) return rc;
 
+  // UST_EVAL_VALIDATION: the validation-required nodes get their byte too (ust_lut.h); an empty selector reads no pod
+  const int validation = !P.eval_pods || !ust_validation_mode(policy) ? 0 : (policy->validation_enabled ? 2 : 1);
   if (P.eval_pods) {
     // pod lists: one byte per node first (only the nodes whose actuator looks at its pods are read),
     // then the ordinary streaming pass with that byte as a fifth input stream
     UST_CUDA(h, h->s_podsum.reserve((size_t)n + 16));
     P.podsum = h->s_podsum.p;
     P.evict_first_inputs = 1;  // the pod-list pass was not measured faster with evict-normal inputs
-    // UST_EVAL_VALIDATION: the validation-required nodes get their byte too (ust_lut.h); an empty selector reads no pod
-    const int validation = !ust_validation_mode(policy) ? 0 : (policy->validation_enabled ? 2 : 1);
     int e = ust_launch_pod_summary(n, P.active, P.hot, P.pod_off, P.pod_flags, n_pods, P.podlut, P.podsum, P.flags, validation,
                                    &P.ws->errinv[P.parity], h->num_sms * 6, st);
     if (e) return h->fail(UST_ERR_CUDA, "pod-summary kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
@@ -529,6 +541,10 @@ static int apply_device(ust_handle* h, const ust_policy* policy, int64_t n, cons
   rc = launch_verify(h, P, st, h->pdl);
   if (rc) return rc;
   h->ws_dirty = false;
+  if (clock) {
+    rc = launch_deadline(h, P, clock, validation, n_pods, st);
+    if (rc) return rc;
+  }
   if (chain && st == h->stream && !P.eval_pods) {
     for (int i = 0; i < 4; i++) h->prev_in[i] = in[i];
     for (int i = 0; i < 3; i++) h->prev_out[i] = outs[i];
@@ -623,6 +639,7 @@ static int adopt_resident(ust_handle* h, int rc, int64_t n, int32_t n_ds, bool o
       h->pods_n = n;
       h->pods_total = n_pods;
       h->pods_clocked = clocked;
+      h->deadline_ready = clocked;
       return rc;
     }
     h->resident_n = n;
@@ -714,12 +731,27 @@ static int check_clock(ust_handle* h, const ust_policy* policy, const ust_clock*
   return UST_OK;
 }
 
-// Clocked calls: bits 18 and 27 of the staged flags from the resident start column, just before the evaluation reads them
+// Clocked calls: bits 18 and 27 of the staged flags from the resident start column, just before the evaluation reads them,
+// and the candidates of the call's next deadline (evaluated by launch_deadline behind the verification kernel)
 static int launch_clock(ust_handle* h, const ust_clock* clock, int64_t n, cudaStream_t st) {
+  const UstClockGrid g = ust_clock_grid((long long)n, 8 * h->num_sms);
+  UST_CUDA(h, h->clk_cand.reserve((size_t)g.ctas * (size_t)g.region + 1));
+  UST_CUDA(h, h->clk_count.reserve((size_t)g.ctas + 1));
+  UST_CUDA(h, h->clk_deadline.reserve(1));
+  h->clk_grid = g;
   int e = ust_launch_clock((long long)n, h->staged.hot.p, h->staged.flags.p, h->s_start.p, (long long)clock->now,
-                           (long long)clock->wait_timeout_seconds, 8 * h->num_sms, st);
+                           (long long)clock->wait_timeout_seconds, g, h->clk_cand.p, h->clk_count.p, h->clk_deadline.p, st);
   if (e) return h->fail(UST_ERR_CUDA, "clock kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
   h->launches += n > 0 ? 1 : 0;
+  return UST_OK;
+}
+
+// The candidates of launch_clock evaluated a second time, behind the call's verification kernel (`P`: its parameters)
+static int launch_deadline(ust_handle* h, const UstParams& P, const ust_clock* clock, int validation, int64_t n_pods, cudaStream_t st) {
+  int e = ust_launch_deadline(P, h->clk_grid, h->clk_cand.p, h->clk_count.p, h->s_start.p, (long long)clock->wait_timeout_seconds,
+                              validation, (long long)n_pods, h->clk_deadline.p, st);
+  if (e) return h->fail(UST_ERR_CUDA, "deadline kernel launch failed: %s", cudaGetErrorString((cudaError_t)e));
+  h->launches += h->clk_grid.ctas > 0 ? 1 : 0;
   return UST_OK;
 }
 
@@ -769,7 +801,7 @@ static int apply_host(ust_handle* h, const ust_policy* policy, int64_t n, const 
   }
   rc = apply_device(h, policy, n, h->staged.hot.p, h->staged.flags.p, h->staged.rev.p, h->staged.ds.p, n_ds, h->s_dsrev.p,
                     pods ? h->s_podoff.p : nullptr, pods ? h->s_podflags.p : nullptr, pods ? pods->n_pods : 0, h->outs.next.p,
-                    h->outs.actions.p, outcome ? h->s_outcome.p : nullptr, nullptr, st);
+                    h->outs.actions.p, outcome ? h->s_outcome.p : nullptr, nullptr, st, clock);
   if (rc) return rc;
   if (N) {
     UST_CUDA(h, cudaMemcpyAsync(next_state, h->outs.next.p, N, cudaMemcpyDeviceToHost, st));
@@ -969,6 +1001,7 @@ int ust_apply_state_device(ust_handle* h, const ust_policy* policy, int64_t n_no
                            uint8_t* actuator_outcome, ust_counters* out_device, void* stream) {
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
+  h->deadline_ready = false;
   h->chain_entry = true;  // the one entry point whose calls may overlap the previous call's tail (apply_device)
   cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
   if (pods && (!pods->pod_off || pods->n_pods < 0 || (pods->n_pods > 0 && !pods->pod_flags)))
@@ -985,6 +1018,7 @@ static int apply_state_common(ust_handle* h, const ust_policy* policy, const ust
                               const int32_t* ds_rev, const ust_pods* pods, uint8_t* next_state, uint16_t* actions,
                               uint8_t* actuator_outcome, ust_counters* out) {
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
+  h->deadline_ready = false;
   if (n < 0 || (n > 0 && (!state || !flags || !pod_rev || !ds_idx || !next_state || !actions)))
     return h->fail(UST_ERR_NIL_STATE, "currentState should not be empty");
   if (n_ds < 0 || (n_ds > 0 && !ds_rev)) return h->fail(UST_ERR_INVALID_ARGUMENT, "bad DaemonSet table");
@@ -1027,6 +1061,7 @@ int ust_apply_state_clocked(ust_handle* h, const ust_policy* policy, const ust_c
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
   h->prev_n = -1;
+  h->deadline_ready = false;  // (also cleared by apply_state_common: a call refused here counts as well)
   if (!clock) return h->fail(UST_ERR_INVALID_ARGUMENT, "clock: required");
   return apply_state_common(h, policy, clock, n, state, flags, pod_rev, ds_idx, n_ds, ds_rev, pods, next_state, actions,
                             actuator_outcome, out);
@@ -1436,7 +1471,7 @@ static int run_delta(ust_handle* h, const DeltaCall& c, const DeltaPlan& p) {
   if (c.sparse && c.pods) std::swap(h->s_outcome, h->s_outcome_prev);
   int rc = apply_device(h, c.policy, p.n, h->staged.hot.p, h->staged.flags.p, h->staged.rev.p, h->staged.ds.p, c.n_ds, h->s_dsrev.p,
                         c.pods ? h->s_podoff.p : nullptr, c.pods ? h->s_podflags.p : nullptr, c.pods ? p.new_total : 0, h->outs.next.p,
-                        h->outs.actions.p, c.actuator_outcome || c.pods ? h->s_outcome.p : nullptr, nullptr, st);
+                        h->outs.actions.p, c.actuator_outcome || c.pods ? h->s_outcome.p : nullptr, nullptr, st, c.clock);
   if (rc) return rc;
   if (!c.sparse) {
     if (N) {
@@ -1475,6 +1510,7 @@ static int delta_entry(ust_handle* h, const char* one_gpu, const DeltaCall& c) {
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
+  h->deadline_ready = false;
   if (one_gpu && h->world > 1) return h->fail(UST_ERR_INVALID_ARGUMENT, "%s runs on one GPU", one_gpu);
   DeltaPlan p;
   const int rc = plan_delta(h, c, &p);
@@ -1566,6 +1602,26 @@ int ust_fetch_outputs_pods(ust_handle* h, uint8_t* next_state, uint16_t* actions
   return UST_OK;
 }
 
+int ust_next_deadline(ust_handle* h, int64_t* t) {
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(h->mu);
+  h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
+  if (!t) return h->fail(UST_ERR_INVALID_ARGUMENT, "t: required");
+  if (h->world > 1)  // each rank would know only its shard's candidates, and its abort point only by the global index
+    return h->fail(UST_ERR_INVALID_ARGUMENT, "ust_next_deadline runs on one GPU: more than one rank is set up by ust_comm_init");
+  if (h->pods_n < 0 || !h->pods_clocked)
+    return h->fail(UST_ERR_INVALID_ARGUMENT, "no clocked pod-list snapshot is resident: call ust_apply_state_clocked first");
+  if (!h->deadline_ready)
+    return h->fail(UST_ERR_INVALID_ARGUMENT, "the last call on the handle was not a clocked call that left its snapshot resident");
+  UST_CUDA(h, cudaSetDevice(h->device));
+  unsigned long long key = 0;
+  UST_CUDA(h, cudaMemcpyAsync(&key, h->clk_deadline.p, sizeof(key), cudaMemcpyDeviceToHost, h->stream));
+  UST_CUDA(h, cudaStreamSynchronize(h->stream));
+  // key: the smallest deadline d with its sign bit flipped, ~0 = none; the bit turns on at d + 1 (d < INT64_MAX)
+  *t = key == ~0ull ? INT64_MIN : (int64_t)(key ^ (1ull << 63)) + 1;
+  return UST_OK;
+}
+
 int ust_fetch_outputs(ust_handle* h, uint8_t* next_state, uint16_t* actions) {
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
@@ -1587,6 +1643,7 @@ int ust_apply_state_packed(ust_handle* h, const ust_policy* policy, int64_t n, c
                            uint8_t* next_state, uint16_t* actions, uint8_t* actuator_outcome, ust_counters* out) {
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
+  h->deadline_ready = false;
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   if (n < 0 || (n > 0 && (!state || !flags || !pod_rev16 || !ds_idx8 || !next_state || !actions)))
     return h->fail(UST_ERR_NIL_STATE, "currentState should not be empty");
@@ -1664,6 +1721,7 @@ int ust_simulate_rollout(ust_handle* h, const ust_policy* policy, int32_t steps,
                          uint32_t* final_flags, int32_t* final_pod_rev, int32_t* steps_done) {
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
+  h->deadline_ready = false;
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   return simulate_common(h, policy, nullptr, steps, history, final_state, final_flags, final_pod_rev, steps_done);
 }
@@ -1671,8 +1729,10 @@ int ust_simulate_rollout(ust_handle* h, const ust_policy* policy, int32_t steps,
 int ust_simulate_rollout_timed(ust_handle* h, const ust_policy* policy, const ust_sim_options* options, int32_t steps,
                                ust_counters* history, uint8_t* final_state, uint32_t* final_flags, int32_t* final_pod_rev,
                                int32_t* steps_done) {
-  if (!h || !options) return UST_ERR_INVALID_ARGUMENT;
+  if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
+  h->deadline_ready = false;
+  if (!options) return UST_ERR_INVALID_ARGUMENT;
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   return simulate_common(h, policy, options, steps, history, final_state, final_flags, final_pod_rev, steps_done);
 }
@@ -1681,6 +1741,7 @@ int ust_build_state(ust_handle* h, int64_t n_pods, const uint8_t* state, const i
                     const int32_t* ds_desired, ust_counters* out) {
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
+  h->deadline_ready = false;
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   if (n_pods < 0 || (n_pods > 0 && (!state || !ds_idx)) || n_ds < 0 || (n_ds > 0 && !ds_desired))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
@@ -1709,6 +1770,7 @@ int ust_build_state_uids(ust_handle* h, int64_t n_pods, const uint8_t* state, co
                          const uint64_t* ds_uid, const int32_t* ds_desired, int32_t* ds_idx_out, ust_counters* out) {
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
+  h->deadline_ready = false;
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   if (n_pods < 0 || (n_pods > 0 && (!state || !owner_uid || !ds_idx_out)) || n_ds < 0 || (n_ds > 0 && (!ds_uid || !ds_desired)))
     return h->fail(UST_ERR_INVALID_ARGUMENT, "bad arguments");
@@ -1742,6 +1804,7 @@ int ust_build_state_delta(ust_handle* h, const ust_driver_pod_reorder* reorder, 
                           ust_counters* out) {
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
+  h->deadline_ready = false;
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   // the new order and every argument, checked in full before anything is touched
   const int64_t n_old = h->bs_n;
@@ -1959,6 +2022,7 @@ int ust_get_unique_id(void* out_bytes) {
 int ust_comm_init(ust_handle* h, int rank, int world_size, const void* unique_id_bytes) {
   if (!h) return UST_ERR_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(h->mu);
+  h->deadline_ready = false;
   h->prev_n = -1;  // whatever this entry point enqueues sits between two device calls: they keep the strict order
   if (world_size < 1 || world_size > UST_MAX_WORLD || rank < 0 || rank >= world_size)
     return h->fail(UST_ERR_INVALID_ARGUMENT, "world size must be 1..%d", UST_MAX_WORLD);

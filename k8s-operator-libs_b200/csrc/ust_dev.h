@@ -197,9 +197,22 @@ int ust_launch_patch(long long m, const long long* idx, const uint8_t* state, co
                      const int32_t* ds_idx, uint8_t* hot_out, uint32_t* flags_out, int32_t* rev_out, int32_t* ds_out, void* stream,
                      const long long* start = nullptr, long long* start_out = nullptr);
 // clocked pod-list calls: bits 18 and 27 of the wait-for-jobs-required and validation-required nodes' flags, derived in place
-// from their start times (include/ust.h, ust_clock); hot carries 16 bytes of padding
+// from their start times (include/ust.h, ust_clock); hot carries 16 bytes of padding. The same launch lists the candidates
+// of the call's next deadline (ust_next_deadline): CTA b of the launch writes up to `region` candidates into cand
+// [b * region, (b + 1) * region) (32-bit offsets among the CTA's own nodes) and their count into cand_count[b], and resets *deadline (n == 0: a memset does). The
+// deadline launch behind the verification kernel (`p`: the call's parameters) evaluates them and min-reduces into *deadline:
+// the smallest d = start + timeout (wrapped) whose flip changes the node's entry, with its sign bit flipped; ~0 = none.
+// `validation` as for ust_launch_pod_summary.
+struct UstClockGrid {
+  int ctas;            // CTAs of both launches (0 when n == 0)
+  long long region;    // candidate slots per CTA: cand holds ctas * region entries
+};
+UstClockGrid ust_clock_grid(long long n, int grid);
 int ust_launch_clock(long long n, const uint8_t* hot, uint32_t* flags, const long long* start, long long now, long long wait_timeout,
-                     int grid, void* stream);
+                     const UstClockGrid& g, uint32_t* cand, unsigned int* cand_count, unsigned long long* deadline, void* stream);
+int ust_launch_deadline(const UstParams& p, const UstClockGrid& g, const uint32_t* cand, const unsigned int* cand_count,
+                        const long long* start, long long wait_timeout, int validation, long long n_pods, unsigned long long* deadline,
+                        void* stream);
 // membership splice (ust_apply_state_delta_splice): the resident columns and the previous outputs, rewritten in the new node
 // order into the o_* arrays (n - n_rm + n_ins entries); rm / ib sorted and checked by the caller
 int ust_launch_splice(long long n, long long n_rm, const long long* rm, long long n_ins, const long long* ib, const uint8_t* ins_hot,

@@ -73,6 +73,14 @@ __device__ __forceinline__ uint32_t node_entry(const UstParams& P, const Shared&
   return *reinterpret_cast<const uint32_t*>(reinterpret_cast<const char*>(S.lut) + off);
 }
 
+// A node's pod-list summary byte `ps` (ust_pod_summary_kernel; layout: pods_apply() in ust_common.cuh) folded into its flags
+// word `fl` and the derived bits `extra` node_entry takes: bit 4 says the list overrides UST_F_WAIT_PODS_RUNNING, which bit
+// 0 then gives; bits 1-3 and 5-7 land at w bits 22-24 and 26-28. Every evaluation of a node with pod lists goes through it.
+__device__ __forceinline__ void fold_podsum(uint32_t ps, uint32_t& fl, uint32_t& extra) {
+  fl &= ~((ps & 0x10u) << 12);
+  extra = extra | ((ps & 1u) << 16) | ((ps & 0xEEu) << 21);
+}
+
 __device__ __forceinline__ uint32_t noop_entry(uint32_t hb) { return ((hb & 15u) << 16) | 0xFF000000u; }
 
 // abort semantics: nodes the sequential passes had not reached when the reference returned its error
@@ -168,11 +176,7 @@ __device__ void general_step(const UstParams& P, Shared& S, long long base, long
 #pragma unroll
   for (int k = 0; k < 4; k++) {
     uint32_t extra = gbits[k], f = fl[k];
-    if (P.podsum && k < nvalid) {  // pod-list summary of the node (ust_pod_summary_kernel), see pods_apply()
-      const uint32_t ps = P.podsum[i0 + k];
-      f &= ~((ps & 0x10u) << 12);
-      extra |= ((ps & 1u) << 16) | ((ps & 0xEEu) << 21);
-    }
+    if (P.podsum && k < nvalid) fold_podsum(P.podsum[i0 + k], f, extra);  // pod-list summary of the node
     e[k] = node_entry(P, S, ds_smem, hb[k], f, rev[k], di[k], extra);
     if (aborting) e[k] = apply_abort(S, e[k], hb[k], S.node_offset + i0 + k);
   }
@@ -227,8 +231,9 @@ __device__ __forceinline__ void span_eval(const UstParams& P, Shared& S, const S
 #pragma unroll
     for (int k = 0; k < 4; k++) {
       const uint32_t hb = (T.h[j] >> (8 * k)) & 0xFFu, p = (T.ps[j] >> (8 * k)) & 0xFFu;
-      const uint32_t fk = fl[k] & ~((p & 0x10u) << 12);
-      e[k] = node_entry(P, S, ds_smem, hb, fk, (int)rv[k], dv[k], grant | ((p & 1u) << 16) | ((p & 0xEEu) << 21));
+      uint32_t fk = fl[k], extra = grant;
+      fold_podsum(p, fk, extra);
+      e[k] = node_entry(P, S, ds_smem, hb, fk, (int)rv[k], dv[k], extra);
     }
     uint32_t next4, out4;
     uint2 act4;
@@ -1218,29 +1223,135 @@ __global__ void __launch_bounds__(kThreads) ust_reorder_kernel(long long n, long
 // flags word - and, with a valid start annotation, their start - and write the word back when it changes. 1 B per node,
 // plus up to 12 B read and 4 B written per such node. (A variant that issued the flags loads of all 16 nodes first, then
 // their start loads, measured slower at C4: 67 against 53 us, DESIGN.md.)
+// On the way the kernel lists the candidates of the call's next deadline (include/ust.h, ust_next_deadline): the nodes whose
+// bit is clear now and turns on at some later time, d + 1 with d = start + timeout wrapped and now <= d < INT64_MAX. CTA b
+// appends them to its own `region` slots of `cand` (a warp scan, one shared-memory atomic per warp) and leaves their count
+// in cand_count[b]; ust_deadline_kernel reads that list and nothing else. A node is stored as its 32-bit offset among the
+// CTA's own nodes, in the order the CTA visits them (cand_node() below). CTA 0 resets the call's deadline.
 __global__ void __launch_bounds__(kThreads) ust_clock_kernel(long long n, const uint8_t* __restrict__ hot, uint32_t* __restrict__ flags,
-                                                             const long long* __restrict__ start, long long now, long long wait_timeout) {
+                                                             const long long* __restrict__ start, long long now, long long wait_timeout,
+                                                             uint32_t* __restrict__ cand, unsigned int* __restrict__ cand_count,
+                                                             long long region, unsigned long long* __restrict__ deadline) {
+  __shared__ unsigned int n_cand;
+  const int t = threadIdx.x, lane = t & 31;
+  if (t == 0) {
+    n_cand = 0;
+    if (blockIdx.x == 0) *deadline = ~0ull;
+  }
+  __syncthreads();
+  uint32_t* mine = cand + (long long)blockIdx.x * region;
   const long long chunks = (n + 15) / 16;  // the hot column carries 16 bytes of padding
   const long long stride = (long long)gridDim.x * kThreads;
-  for (long long c = (long long)blockIdx.x * kThreads + threadIdx.x; c < chunks; c += stride) {
-    const uint4 v = __ldg(reinterpret_cast<const uint4*>(hot) + c);
-    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+  uint32_t it16 = 0;  // 16 * kThreads * the iteration: the offset of this iteration's first node among the CTA's
+  for (long long c0 = (long long)blockIdx.x * kThreads; c0 < chunks; c0 += stride, it16 += 16 * kThreads) {  // warp-uniform trip count
+    const long long c = c0 + t;
+    unsigned cbits = 0;  // this chunk's candidates
+    if (c < chunks) {
+      const uint4 v = __ldg(reinterpret_cast<const uint4*>(hot) + c);
+      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-    for (int j = 0; j < 16; j++) {
-      const unsigned s = (w[j >> 2] >> (8 * (j & 3))) & UST_HOT_STATE_MASK;
-      const long long i = c * 16 + j;
-      if ((s != UST_STATE_WAIT_FOR_JOBS_REQUIRED && s != UST_STATE_VALIDATION_REQUIRED) || i >= n) continue;
-      const bool wait = s == UST_STATE_WAIT_FOR_JOBS_REQUIRED;
-      const uint32_t anno = wait ? UST_F_WAIT_START_ANNO : UST_F_VALIDATION_START_ANNO;
-      const uint32_t invalid = wait ? UST_F_WAIT_START_INVALID : UST_F_VALIDATION_START_INVALID;
-      const uint32_t f = flags[i];
-      const bool timed_out = (f & (anno | invalid)) == anno &&
-                             ust_timed_out(now, __ldg(start + i), wait ? wait_timeout : (long long)UST_VALIDATION_TIMEOUT_SECONDS);
-      const uint32_t g = (f & ~(UST_F_WAIT_TIMED_OUT | UST_F_VALIDATION_TIMED_OUT)) |
-                         (timed_out ? (wait ? UST_F_WAIT_TIMED_OUT : UST_F_VALIDATION_TIMED_OUT) : 0u);
-      if (g != f) flags[i] = g;
+      for (int j = 0; j < 16; j++) {
+        const unsigned s = (w[j >> 2] >> (8 * (j & 3))) & UST_HOT_STATE_MASK;
+        const long long i = c * 16 + j;
+        if ((s != UST_STATE_WAIT_FOR_JOBS_REQUIRED && s != UST_STATE_VALIDATION_REQUIRED) || i >= n) continue;
+        const bool wait = s == UST_STATE_WAIT_FOR_JOBS_REQUIRED;
+        const uint32_t anno = wait ? UST_F_WAIT_START_ANNO : UST_F_VALIDATION_START_ANNO;
+        const uint32_t invalid = wait ? UST_F_WAIT_START_INVALID : UST_F_VALIDATION_START_INVALID;
+        const uint32_t f = flags[i];
+        const bool valid = (f & (anno | invalid)) == anno;
+        const long long d = valid ? ust_deadline(__ldg(start + i), wait ? wait_timeout : (long long)UST_VALIDATION_TIMEOUT_SECONDS) : 0;
+        const bool timed_out = valid && now > d;
+        if (valid && !timed_out && d != LLONG_MAX) cbits |= 1u << j;
+        const uint32_t g = (f & ~(UST_F_WAIT_TIMED_OUT | UST_F_VALIDATION_TIMED_OUT)) |
+                           (timed_out ? (wait ? UST_F_WAIT_TIMED_OUT : UST_F_VALIDATION_TIMED_OUT) : 0u);
+        if (g != f) flags[i] = g;
+      }
+    }
+    const unsigned k = __popc(cbits);
+    if (__any_sync(kFull, k != 0)) {
+      unsigned incl = k;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned u = __shfl_up_sync(kFull, incl, o);
+        if (lane >= o) incl += u;
+      }
+      unsigned base = 0;
+      if (lane == 31) base = atomicAdd(&n_cand, incl);
+      unsigned pos = __shfl_sync(kFull, base, 31) + incl - k;
+      while (cbits) {
+        const int j = __ffs(cbits) - 1;
+        cbits &= cbits - 1;
+        mine[pos++] = it16 + 16u * (uint32_t)t + (uint32_t)j;
+      }
     }
   }
+  __syncthreads();
+  if (t == 0) cand_count[blockIdx.x] = n_cand;
+}
+
+// The next deadline of a clocked call (include/ust.h, ust_next_deadline), behind its verification kernel: every candidate
+// the clock kernel listed is evaluated twice with the functions of the verification kernel - node_entry on the summary byte
+// the call used, apply_abort with the call's abort point (from the counters it wrote) - once as the call saw it and once
+// with its timed-out bit set. A validation-required node in validation mode asks validation_summary again for its byte,
+// with the bit set (its pods walked again up to the first one that is not ready). The smallest d of the nodes whose entry
+// differs: warp reduction, one shared-memory atomic per warp, one global atomic per CTA. CTA b reads the list of the clock
+// kernel's CTA b. `validation`: as for ust_pod_summary_kernel.
+// node index of a candidate offset of CTA b (ust_clock_kernel's iteration order, the same grid)
+__device__ __forceinline__ long long cand_node(uint32_t off, long long b) {
+  const long long it = off / (16 * kThreads), rem = off % (16 * kThreads);
+  return ((long long)b * kThreads + it * (long long)gridDim.x * kThreads) * 16 + rem;
+}
+
+__global__ void __launch_bounds__(kThreads) ust_deadline_kernel(const __grid_constant__ UstParams P, const uint32_t* __restrict__ cand,
+                                                                const unsigned int* __restrict__ cand_count, long long region,
+                                                                const long long* __restrict__ start, long long wait_timeout,
+                                                                int validation, long long n_pods, unsigned long long* __restrict__ deadline) {
+  __shared__ Shared S;
+  __shared__ unsigned long long cta_min;
+  const int t = threadIdx.x;
+  const unsigned cnt = __ldg(cand_count + blockIdx.x);
+  if (cnt == 0) return;  // (CTA-uniform)
+  for (int k = t; k < (int)UST_LUT_WORDS; k += kThreads) S.lut[k] = __ldg(P.lut + k);  // the table, then the meta pairs behind it
+  if (t == 0) {
+    const long long pass = P.out->error_pass;  // the call's abort, as the verification kernel reported it (one GPU: node offset 0,
+                                               // ust_next_deadline refuses more than one rank)
+    S.abort_key = pass >= 0 ? UST_KEY(pass, (unsigned long long)(P.out->error_index + 1)) : ~0ull;
+    cta_min = ~0ull;
+  }
+  __syncthreads();
+  const uint32_t* mine = cand + (long long)blockIdx.x * region;
+  const unsigned char* bytes = reinterpret_cast<const unsigned char*>(P.pod_flags);
+  // a node's entry as the evaluation forms it from its flags word and summary byte (general_step; neither state reads the grant)
+  auto entry = [&](uint32_t hb, uint32_t f, uint32_t ps, int rev, uint32_t di, long long i) {
+    uint32_t extra = 0u;
+    fold_podsum(ps, f, extra);
+    return apply_abort(S, node_entry(P, S, false, hb, f, rev, di, extra), hb, i);
+  };
+  unsigned long long best = ~0ull;  // the smallest d, with its sign bit flipped (unsigned order = signed order)
+  for (unsigned q = t; q < cnt; q += kThreads) {
+    const long long i = cand_node(__ldg(mine + q), blockIdx.x);
+    const uint32_t hb = __ldg(P.hot + i), f = __ldg(P.flags + i), di = (uint32_t)__ldg(P.ds_idx + i);
+    const int rev = __ldg(P.pod_rev + i);
+    const uint32_t ps = P.podsum ? __ldg(P.podsum + i) : 0u;
+    const bool wait = (hb & UST_HOT_STATE_MASK) == UST_STATE_WAIT_FOR_JOBS_REQUIRED;
+    const long long d = ust_deadline(__ldg(start + i), wait ? wait_timeout : (long long)UST_VALIDATION_TIMEOUT_SECONDS);
+    const uint32_t f1 = f | (wait ? UST_F_WAIT_TIMED_OUT : UST_F_VALIDATION_TIMED_OUT);
+    uint32_t ps1 = ps;
+    if (!wait && P.podsum && validation)
+      ps1 = validation_summary(P.pod_flags, bytes, 2 * n_pods, __ldg(P.pod_off + i), __ldg(P.pod_off + i + 1), f1, validation == kValWalk);
+    if (entry(hb, f, ps, rev, di, i) != entry(hb, f1, ps1, rev, di, i)) {
+      const unsigned long long key = (unsigned long long)d ^ (1ull << 63);
+      best = key < best ? key : best;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const unsigned long long u = __shfl_xor_sync(kFull, best, o);
+    best = u < best ? u : best;
+  }
+  if ((t & 31) == 0 && best != ~0ull) atomicMin(&cta_min, best);
+  __syncthreads();
+  if (t == 0 && cta_min != ~0ull) atomicMin(deadline, cta_min);
 }
 
 // The resident driver-pod list of ust_build_state_delta in a new order: state byte, owner UID and previous owner index of
@@ -1776,11 +1887,30 @@ int ust_launch_patch(long long m, const long long* idx, const uint8_t* state, co
                                                                      ds_out, nullptr, nullptr);
   return (int)cudaGetLastError();
 }
+UstClockGrid ust_clock_grid(long long n, int grid) {
+  const long long chunks = (n + 15) / 16;
+  const long long want = (chunks + kThreads - 1) / kThreads;
+  UstClockGrid g;
+  // enough CTAs that a CTA's candidate offsets fit 32 bits (only past ~2^31 nodes per CTA of `grid`)
+  const long long least = ((chunks * 16) >> 31) + 1;
+  const long long ctas = want < grid ? want : (grid > least ? grid : least);
+  g.ctas = n <= 0 ? 0 : (int)ctas;
+  g.region = g.ctas ? (chunks + (long long)g.ctas * kThreads - 1) / ((long long)g.ctas * kThreads) * kThreads * 16 : 0;
+  return g;
+}
 int ust_launch_clock(long long n, const uint8_t* hot, uint32_t* flags, const long long* start, long long now, long long wait_timeout,
-                     int grid, void* stream) {
-  if (n <= 0) return 0;
-  const long long want = ((n + 15) / 16 + kThreads - 1) / kThreads;
-  ust_clock_kernel<<<(unsigned)(want < grid ? want : grid), kThreads, 0, (cudaStream_t)stream>>>(n, hot, flags, start, now, wait_timeout);
+                     const UstClockGrid& g, uint32_t* cand, unsigned int* cand_count, unsigned long long* deadline, void* stream) {
+  if (g.ctas == 0) return (int)cudaMemsetAsync(deadline, 0xFF, sizeof(unsigned long long), (cudaStream_t)stream);
+  ust_clock_kernel<<<(unsigned)g.ctas, kThreads, 0, (cudaStream_t)stream>>>(n, hot, flags, start, now, wait_timeout, cand, cand_count,
+                                                                           g.region, deadline);
+  return (int)cudaGetLastError();
+}
+int ust_launch_deadline(const UstParams& p, const UstClockGrid& g, const uint32_t* cand, const unsigned int* cand_count,
+                        const long long* start, long long wait_timeout, int validation, long long n_pods, unsigned long long* deadline,
+                        void* stream) {
+  if (g.ctas == 0) return 0;
+  ust_deadline_kernel<<<(unsigned)g.ctas, kThreads, 0, (cudaStream_t)stream>>>(p, cand, cand_count, g.region, start, wait_timeout,
+                                                                              validation, n_pods, deadline);
   return (int)cudaGetLastError();
 }
 int ust_launch_splice(long long n, long long n_rm, const long long* rm, long long n_ins, const long long* ib, const uint8_t* ins_hot,

@@ -124,10 +124,10 @@ static inline void ust_uncordon_or_done(uint32_t w, unsigned* next, unsigned* ac
 }
 
 // Go's `now > start + timeout` on int64 (pod_manager.go:354, validation_manager.go:161): the sum wraps in two's complement,
-// so a start near INT64_MAX counts as timed out. Computed in uint64: signed overflow is undefined in C++.
-UST_HD inline bool ust_timed_out(int64_t now, int64_t start, int64_t timeout) {
-  return now > (int64_t)((uint64_t)start + (uint64_t)timeout);
-}
+// so a start near INT64_MAX counts as timed out. Computed in uint64: signed overflow is undefined in C++. ust_deadline is
+// the wrapped sum d: the node is timed out at every now > d, so its bit turns on at d + 1 (never when d == INT64_MAX).
+UST_HD inline int64_t ust_deadline(int64_t start, int64_t timeout) { return (int64_t)((uint64_t)start + (uint64_t)timeout); }
+UST_HD inline bool ust_timed_out(int64_t now, int64_t start, int64_t timeout) { return now > ust_deadline(start, timeout); }
 
 // Pod-list summary byte of a validation-required node in validation mode (ust_pod_summary_kernel): bits 1-3 the outcome
 // of Validate (validation_manager.go:71-175) for the node's validation pods in list order and its start-time annotation,

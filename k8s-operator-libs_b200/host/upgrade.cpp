@@ -1258,7 +1258,16 @@ Error ClusterUpgradeStateManagerImpl::Replay(const EncodedSnapshot& enc, const D
   return std::nullopt;
 }
 
+// The next deadline of the clocked call the handle just made (ust_next_deadline); nullopt when none is pending or the handle
+// has none to give (the call failed).
+static std::optional<int64_t> next_deadline(ust_handle* h) {
+  int64_t t = INT64_MIN;
+  if (ust_next_deadline(h, &t) != UST_OK || t == INT64_MIN) return std::nullopt;
+  return t;
+}
+
 Error ClusterUpgradeStateManagerImpl::ApplyState(ClusterUpgradeState* currentState, const DriverUpgradePolicySpec* upgradePolicy) {
+  nextTimeout_.reset();
   if (currentState == nullptr) return Errorf("currentState should not be empty");  // upgrade_state.go:175-177
   if (upgradePolicy == nullptr || !upgradePolicy->AutoUpgrade) return std::nullopt;  // upgrade_state.go:179-182
   if (handle_ == nullptr) return Errorf("no H100 device bound to this manager: ApplyState has no CPU path");
@@ -1280,6 +1289,7 @@ Error ClusterUpgradeStateManagerImpl::ApplyState(ClusterUpgradeState* currentSta
     rc = ust_apply_state_clocked(handle_, &enc.policy, &clock, (int64_t)n, enc.state.data(), enc.flags.data(), enc.pod_rev.data(),
                                  enc.ds_idx.data(), (int32_t)enc.ds_rev.size() - 1, enc.ds_rev.data(), &pods, next.data(), actions.data(),
                                  outcome.data(), &last_);
+    if (enc.validateOnDevice || enc.waitOnDevice) nextTimeout_ = next_deadline(handle_);
   } else {
     rc = ust_apply_state(handle_, &enc.policy, (int64_t)n, enc.state.data(), enc.flags.data(), enc.pod_rev.data(), enc.ds_idx.data(),
                          (int32_t)enc.ds_rev.size() - 1, enc.ds_rev.data(), nullptr, next.data(), actions.data(), nullptr, &last_);
@@ -1363,6 +1373,7 @@ int ClusterUpgradeStateManagerImpl::EvaluateCachedPods(const ust_policy& policy,
                                                        const std::vector<int64_t>& changed, Cache* cache, ust_counters* c) {
   Cache& k = *cache;
   const size_t n = k.slots.size();
+  cachedDeadline_.reset();
   if (handle_ == nullptr) return UST_ERR_CUDA;
   // never pass NULL for empty arrays
   std::vector<int32_t> dsrev = k.ds_rev;
@@ -1390,8 +1401,11 @@ int ClusterUpgradeStateManagerImpl::EvaluateCachedPods(const ust_policy& policy,
     csr(n, nullptr);
     const ust_pods pods = {off.data(), pf.data(), (int64_t)pf.size() - 1};
     const ust_clock clock = {now, waitTimeout, sv.data(), nullptr};
-    return ust_apply_state_clocked(handle_, &policy, &clock, (int64_t)n, st.data(), fl.data(), rv.data(), di.data(), (int32_t)k.ds_rev.size(),
-                                   dsrev.data(), &pods, k.next.data(), k.actions.data(), k.outcome.data(), c);
+    const int rc = ust_apply_state_clocked(handle_, &policy, &clock, (int64_t)n, st.data(), fl.data(), rv.data(), di.data(),
+                                           (int32_t)k.ds_rev.size(), dsrev.data(), &pods, k.next.data(), k.actions.data(),
+                                           k.outcome.data(), c);
+    cachedDeadline_ = next_deadline(handle_);
+    return rc;
   }
   const size_t m = changed.size();
   std::vector<uint8_t> st(m + 1);
@@ -1431,6 +1445,7 @@ int ClusterUpgradeStateManagerImpl::EvaluateCachedPods(const ust_policy& policy,
                                                     rv.data(), di.data(), (int32_t)k.ds_rev.size(), dsrev.data(), cap, oi.data(), on.data(),
                                                     oa.data(), oo.data(), &n_out, c);
   if (rc == UST_ERR_CUDA || rc == UST_ERR_INVALID_ARGUMENT || rc == UST_ERR_COMM) return rc;
+  cachedDeadline_ = next_deadline(handle_);
   if (n_out > cap) {  // UST_ERR_TRUNCATED or a reference-level abort with more outputs than the arrays hold: fetch them all
     stats_.outputs_received += (int64_t)n;
     k.next.resize(n + 1);
@@ -1449,6 +1464,7 @@ int ClusterUpgradeStateManagerImpl::EvaluateCachedPods(const ust_policy& policy,
 }
 
 Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState* currentState, const DriverUpgradePolicySpec* upgradePolicy) {
+  nextTimeout_.reset();
   if (currentState == nullptr) return Errorf("currentState should not be empty");  // upgrade_state.go:175-177
   if (upgradePolicy == nullptr || !upgradePolicy->AutoUpgrade) return std::nullopt;  // upgrade_state.go:179-182
   ust_policy pol;
@@ -1765,8 +1781,10 @@ Error ClusterUpgradeStateManagerImpl::ApplyStateIncremental(ClusterUpgradeState*
     stats_.lists_sent += (int64_t)k.listChanged.size();
     stats_.lists_reused += (int64_t)(k.slots.size() - k.listChanged.size());
     if (!full && changed.empty() && k.listChanged.empty() && k.pending.empty()) stats_.time_only++;
+    cachedDeadline_.reset();
     rc = EvaluateCachedPods(pol, now, upgradePolicy->WaitForCompletion ? upgradePolicy->WaitForCompletion->TimeoutSecond : 0, full, changed,
                             &k, &last_);
+    if (val || wait) nextTimeout_ = cachedDeadline_;
   } else {
     rc = EvaluateCached(pol, full, changed, &k, &last_);
   }

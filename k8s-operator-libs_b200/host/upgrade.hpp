@@ -380,6 +380,19 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
 
   const ust_counters& LastCounters() const { return last_; }
 
+  // Not in the reference: when the next reconcile in which only time passes will do something. Nothing changes in the API
+  // when a wait-for-completion or validation deadline passes, so no watch event triggers that reconcile; a loop can sleep
+  // until this time instead of polling. The value is the device's ust_next_deadline (include/ust.h) of the last ApplyState
+  // or ApplyStateIncremental that made a clocked call with ValidateOnDevice or WaitForCompletionOnDevice in effect: the
+  // smallest t > that reconcile's `now` at which a reconcile with the same objects makes a call this one did not make (a
+  // node times out, or its outcome changes). nullopt when the last ApplyState / ApplyStateIncremental made no such call,
+  // when the call failed, or when no deadline is pending.
+  // What it does not cover, because each is an object change whose watch event triggers a reconcile of its own, and that
+  // reconcile's call includes the deadline it brings: a start-time annotation that Replay sets in this reconcile
+  // (UST_A_SET_WAIT_START, for either timeout), and evictions or drains that finish on the workers. A clock that moves
+  // backwards is not covered either.
+  std::optional<int64_t> NextTimeout() const { return nextTimeout_; }
+
   // ---- incremental ApplyState (SURVEY 8f.2): the resourceVersion-keyed encode cache -------------------------------
   // The same contract as ApplyState for a reconcile loop that calls it again and again with fresh BuildState
   // snapshots. The manager keeps the encoded snapshot (host and device) from call to call, in a node order that does
@@ -522,8 +535,11 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
   // ust_apply_state_clocked with every list and start time; else ust_apply_state_delta_pods_clocked with cache->pending as
   // runs, the lists of cache->listChanged and the start times of `changed` and of the inserted slots, patching
   // cache->outcome too. `now` / `waitTimeout` make the ust_clock.
+  // It also leaves the call's next deadline (ust_next_deadline; nullopt for none, or when the call failed) in
+  // cachedDeadline_, which ApplyStateIncremental carries out through NextTimeout(); an override sets it as well.
   virtual int EvaluateCachedPods(const ust_policy& policy, int64_t now, int64_t waitTimeout, bool full,
                                  const std::vector<int64_t>& changed, Cache* cache, ust_counters* c);
+  std::optional<int64_t> cachedDeadline_;
   ClusterUpgradeStateManagerImpl() = default;
   explicit ClusterUpgradeStateManagerImpl(StateOptions opts) : opts_(std::move(opts)) {}  // a manager without a device
 
@@ -553,6 +569,7 @@ class ClusterUpgradeStateManagerImpl : public ClusterUpgradeStateManager {
   PodDeletionFilter filter_;
   std::string validationSelector_;
   ust_counters last_{};
+  std::optional<int64_t> nextTimeout_;  // NextTimeout()
   // The PodEvictor's workers: a queue served by up to kActuatorWorkers threads, and the reference's two dedupe sets
   // (pod_manager.go:160-165, drain_manager.go:104-110), guarded by actMu_.
   static constexpr size_t kActuatorWorkers = 16;

@@ -111,6 +111,9 @@ class PodLists(C.Structure):
                 ("n_pods", C.c_int64)]
 
 
+NO_DEADLINE = -(1 << 63)  # ust_next_deadline: no time-only reconcile will return anything (INT64_MIN)
+
+
 class Clock(C.Structure):
     """ust_clock: the time of a clocked pod-list call and the start times of the nodes it carries (raw host addresses)."""
     _fields_ = [("now", C.c_int64), ("wait_timeout_seconds", C.c_int64), ("start", C.c_void_p), ("insert_start", C.c_void_p)]

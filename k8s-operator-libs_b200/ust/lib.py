@@ -61,6 +61,7 @@ def load():
         lib.ust_apply_state_delta_pods_clocked.argtypes = [vp, vp, vp, vp, vp] + nodes + sparse + [vp, vp, vp]
         lib.ust_fetch_outputs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         lib.ust_fetch_outputs_pods.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        lib.ust_next_deadline.argtypes = [C.c_void_p, C.c_void_p]
         lib.ust_simulate_rollout.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         lib.ust_simulate_rollout_timed.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                                    C.c_void_p, C.c_void_p]
@@ -82,7 +83,7 @@ def load():
 
 
 EXPORTS = ["ust_abi_version", "ust_create", "ust_destroy", "ust_last_error", "ust_create_error", "ust_launch_count",
-           "ust_host_alloc", "ust_host_free", "ust_apply_state", "ust_apply_state_device", "ust_stream", "ust_apply_state_packed", "ust_apply_state_delta", "ust_apply_state_delta_sparse", "ust_apply_state_delta_splice", "ust_apply_state_delta_reorder", "ust_apply_state_delta_pods", "ust_apply_state_delta_pods_reorder", "ust_apply_state_clocked", "ust_apply_state_delta_pods_clocked", "ust_fetch_outputs", "ust_fetch_outputs_pods", "ust_simulate_rollout", "ust_simulate_rollout_timed", "ust_sync",
+           "ust_host_alloc", "ust_host_free", "ust_apply_state", "ust_apply_state_device", "ust_stream", "ust_apply_state_packed", "ust_apply_state_delta", "ust_apply_state_delta_sparse", "ust_apply_state_delta_splice", "ust_apply_state_delta_reorder", "ust_apply_state_delta_pods", "ust_apply_state_delta_pods_reorder", "ust_apply_state_clocked", "ust_apply_state_delta_pods_clocked", "ust_fetch_outputs", "ust_fetch_outputs_pods", "ust_next_deadline", "ust_simulate_rollout", "ust_simulate_rollout_timed", "ust_sync",
            "ust_build_state", "ust_build_state_uids", "ust_build_state_delta", "ust_fetch_build_state", "ust_get_unique_id", "ust_comm_init", "ust_comm_set_mode", "ust_table_entry",
            "ust_table_window_shift", "ust_table_window"]
 
@@ -381,6 +382,19 @@ class Handle:
         ck = _clock(now, wait_timeout_seconds, start, insert_start) if clock else (None, [])
         return self._delta_sparse(self._lib.ust_apply_state_delta_pods_clocked, policy, [ck, _reorder(reorder), _pod_lists(lists)],
                                   idx, changed, ds_rev, max_out, out, pods=True)
+
+    def next_deadline(self, check=True):
+        """ust_next_deadline: the time (int) at which a time-only clocked reconcile on the resident snapshot first returns
+        something, or None when no deadline is pending (abi.NO_DEADLINE). check=False returns the code instead of raising:
+        (rc, value)."""
+        t = C.c_int64(0)
+        rc = self._lib.ust_next_deadline(self._h, C.addressof(t))
+        v = None if rc or t.value == abi.NO_DEADLINE else int(t.value)
+        if not check:
+            return rc, v
+        if rc:
+            raise UstError(rc, self.last_error())
+        return v
 
     def fetch_outputs_pods(self, n):
         """ust_fetch_outputs_pods: (rc, next_state, actions, actuator_outcome) of the last call on the pod-list snapshot."""
